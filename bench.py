@@ -2,6 +2,7 @@
 """bench.py — inpainted frames/sec of FGT full inference at 432x240, T=10 (BASELINE.json configs[1]).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl fgt_b200|reference|reference-gpu] [--config 2|3|4|5]
+                    [--dump-outputs DIR]
 
 Default (--config 2): a step is one Model.forward over one synthetic masked clip [1,10,3,240,432] (+flows,
 masks) with seeded random weights of the reference architecture. `value` is measured with the inputs already
@@ -18,10 +19,13 @@ The other BASELINE configurations are separate lines: --config 3 (RAFT + LAFC at
 --config 5 (1280x720 T=40 clip = 8 windows).
 
 --impl reference times the CPU oracle port of the reference path (oracle/fgt_oracle.py, validated against the
-unmodified reference in tests/golden) on the host cores — the reference itself is Python under
-/root/reference and does not exist on the GPU box. --impl reference-gpu (and the `gpu_eager_baseline` key of
-the default line) runs the same PyTorch restatement eagerly on the B200 (cuBLAS / cuDNN): the bar SURVEY.md
+unmodified reference in tests/golden) on the host cores. --impl reference-gpu (and the `gpu_eager_baseline` key of
+the default line) runs the same PyTorch restatement eagerly on the GPU (cuBLAS / cuDNN): the bar SURVEY.md
 §2.2 names.
+
+--dump-outputs DIR (config 2, rank 0): after the timed steps, the inpainted frames the timed forward returned in its
+last step are written as DIR/inpainted_frames.npy (float32 [T, 3, H, W], 12.4 MB). Inputs and weights are seeded, so
+two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -58,7 +62,8 @@ def load_peaks():
             d = json.load(fh)
         return dict(hbm_gbs=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0,
+                source="fallback: NVIDIA H100 SXM data sheet (dense bf16, 700 W), not a measured rate")
 
 
 class ClockSampler:
@@ -213,7 +218,7 @@ def run_reference(args, rank, world):
 
 
 def run_reference_gpu(args, rank, world):
-    """GPU-eager arm: the PyTorch restatement on the B200 through cuBLAS / cuDNN (rank 0 only)."""
+    """GPU-eager arm: the PyTorch restatement on the GPU through cuBLAS / cuDNN (rank 0 only)."""
     if rank != 0:
         return
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
@@ -276,7 +281,11 @@ def main():
     ap.add_argument("--config", type=int, default=2, choices=[2, 3, 4, 5])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output as DIR/<name>.npy (config 2)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config != 2 or args.impl != "fgt_b200"):
+        ap.error("--dump-outputs is implemented for --config 2 --impl fgt_b200 only")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -309,7 +318,7 @@ def main():
     host = [t.contiguous().pin_memory() for t in clip]
     devin = [t.to(dev) for t in host]
     out_host = torch.empty(T, 3, H, W).pin_memory()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > the 50 MB L2 of an H100
 
     def barrier():
         if world > 1:
@@ -339,8 +348,10 @@ def main():
         total_ms = sum(a.elapsed_time(b) for a, b in evs)
         return parallel.max_over_ranks(total_ms, dev) / steps, launches
 
+    last = {}
+
     def step_device():
-        model(*devin)
+        last["out"] = model(*devin)
 
     def step_e2e():
         d = [h.to(dev, non_blocking=True) for h in host]
@@ -417,6 +428,11 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()
     ms_dev, launches = timed(step_device)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "inpainted_frames.npy"), last["out"].float().cpu().numpy())
+    last.clear()
     ms_e2e_serial, _ = timed(step_e2e)
     ms_e2e, streamer = timed_streamed()
     clocks = sampler.stop()
@@ -449,21 +465,16 @@ def main():
         modules[name] = e
     worst = min((k for k in modules if "frac" in modules[k]), key=lambda k: modules[k]["frac"], default=None)
     dk, da = max(agg.items(), key=lambda kv: kv[1]["ms"])
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        with open(tpath) as fh:
-            traffic = json.load(fh).get(dk)
     if da["flops"] > 0:
         ach = da["flops"] / (da["ms"] * 1e-3) / 1e12
         roof = {"kernel": dk, "bound": "tensor", "achieved": ach, "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
-                "frac": ach / peaks["tf_sustained"], "traffic": traffic, "peak_source": peaks["source"] + ", sustained bf16",
+                "frac": ach / peaks["tf_sustained"], "peak_source": peaks["source"] + ", sustained bf16",
                 "note": "algorithmic FLOPs; split-bf16 layers execute 3 MMAs per algorithmic one (ceiling 1/3), the "
                         "flow branch 1 (see dtype)"}
     else:
         ach = da["bytes"] / (da["ms"] * 1e-3) / 1e9
         roof = {"kernel": dk, "bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": ach / peaks["hbm_gbs"], "traffic": traffic, "peak_source": peaks["source"]}
+                "frac": ach / peaks["hbm_gbs"], "peak_source": peaks["source"]}
     roof["modules"] = {k: {kk: v[kk] for kk in ("us_per_layer", "gflop_per_layer", "achieved_tflops", "frac")}
                        for k, v in modules.items() if "frac" in v}
     roof["worst_module"] = worst

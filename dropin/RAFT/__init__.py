@@ -1,5 +1,5 @@
 """Shadow of /root/reference/RAFT/__init__.py: `from RAFT import RAFT` (tool/video_inpainting.py:26)
-yields the B200-native model; other submodules (RAFT.utils, ...) still resolve from the reference's
+yields the H100-native model; other submodules (RAFT.utils, ...) still resolve from the reference's
 RAFT/ directory further down sys.path."""
 import pkgutil
 

@@ -1,4 +1,4 @@
-"""Builds libfgt_sm100a.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libfgt_sm90a.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import hashlib
 import os
 import subprocess
@@ -6,11 +6,11 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB = os.path.join(HERE, "libfgt_sm100a.so")
+LIB = os.path.join(HERE, "libfgt_sm90a.so")
 STAMP = os.path.join(HERE, "csrc", ".build_stamp")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xptxas=-v",
     "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function", "--shared", "-cudart", "static",
 ]
@@ -27,7 +27,7 @@ def _digest():
     files.append(os.path.join(root, "include", "fgt_b200.h"))
     for f in files:
         with open(f, "rb") as fh:
-            h.update(f.encode())
+            h.update(os.path.relpath(f, root).encode())
             h.update(fh.read())
     return h.hexdigest()
 
@@ -43,7 +43,7 @@ def build(force=False, verbose=False):
     if verbose or res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)
     if res.returncode != 0:
-        raise RuntimeError("nvcc failed building libfgt_sm100a.so")
+        raise RuntimeError("nvcc failed building libfgt_sm90a.so")
     with open(STAMP, "w") as fh:
         fh.write(dig)
     return LIB

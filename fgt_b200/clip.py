@@ -35,7 +35,7 @@ def inpaint_clip_device(model, frames, masks, flows, step=10, num_ref=-1, neighb
     composed clip uint8 [N,H,W,3] on the device. `model(masked_frames[1,t,3,H,W], flows[1,t,2,H,W],
     masks[1,t,1,H,W]) -> [t,3,H,W]` is the drop-in FGT model (or anything with that signature)."""
     if not frames.is_cuda:
-        raise RuntimeError("fgt_b200.clip runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+        raise RuntimeError("fgt_b200.clip runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     dev = frames.device
     N, _, H, W = frames.shape
     if tuple(masks.shape) != (N, H, W) or tuple(flows.shape) != (N, 2, H, W):
@@ -80,7 +80,7 @@ def inpaint_clip(model, frame_blends, mask, video_flow_f, step=10, num_ref=-1, n
     """Driver-layout front end (numpy in, list of N uint8 [H,W,3] RGB frames out — `comp_frames` at :745)."""
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if dev.type != "cuda":
-        raise RuntimeError("fgt_b200.clip runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+        raise RuntimeError("fgt_b200.clip runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     frames, masks, flows = prepare_clip(frame_blends, mask, video_flow_f, dev)
     out = inpaint_clip_device(model, frames, masks, flows, step, num_ref, neighbor_stride).cpu().numpy()
     return [out[i] for i in range(out.shape[0])]

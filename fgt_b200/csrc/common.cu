@@ -135,11 +135,6 @@ int encode_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t
   return encode_map_any(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box);
 }
 
-int encode_map_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                   const uint64_t* strides_bytes, const uint32_t* box) {
-  return encode_map_any(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box);
-}
-
 bool pdl_enabled() {
   static int on = -1;
   if (on < 0) {

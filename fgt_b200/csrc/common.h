@@ -31,20 +31,15 @@ int set_err(int code, const char* fmt, ...);
 // dims[0] is the contiguous dimension; strides_bytes has rank-1 entries (dims 1..rank-1).
 int encode_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                     const uint64_t* strides_bytes, const uint32_t* box);
-// Same for fp32 elements (epilogue TMA stores of fp32 outputs).
-int encode_map_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                   const uint64_t* strides_bytes, const uint32_t* box);
 
 int num_sms();
 
 // Programmatic dependent launch (PDL), opt-in with FGT_PDL=1: kernels are then launched with the
 // programmatic-stream-serialization attribute; each calls pdl_launch_dependents() once its prologue is done
-// (the next kernel may be scheduled onto SMs as they free up and run its own prologue: barrier init, TMEM
-// allocation, descriptor prefetch) and pdl_wait() before its first global access (blocks until the preceding
-// grid has completed and its memory is visible), so ordering is unchanged. Measured on the T=10 forward under
-// CUDA-graph replay: 6.75 ms with PDL vs 6.64 ms without on the same box (graph replay already keeps launch
-// gaps near 1 us and the early-resident dependents cost more than they hide) — hence off by default; without
-// the attribute both instructions are no-ops.
+// (the next kernel may be scheduled onto SMs as they free up and run its own prologue: barrier init,
+// descriptor prefetch) and pdl_wait() before its first global access (blocks until the preceding
+// grid has completed and its memory is visible), so ordering is unchanged. Off by default (under CUDA-graph
+// replay launch gaps are already small); without the attribute both instructions are no-ops.
 bool pdl_enabled();
 
 template <typename... KArgs, typename... Args>

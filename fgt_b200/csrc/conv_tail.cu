@@ -1,19 +1,18 @@
 // 3x3 convolution with a handful of output channels (the decoder's final 64 -> 3 conv + tanh, model.py:185-193; RAFT's
 // flow head 256 -> 2, update.py:13-14) as ONE kernel: tensor cores for the contraction, shared memory for the taps.
 //
-// A convolution with <= 3 output channels has no N extent for an implicit GEMM (N = 3 would waste 125/128 of every MMA
+// A convolution with <= 3 output channels has no N extent for an implicit GEMM (N = 3 would waste most of every MMA
 // and re-read the activation once per tap). Instead the taps become the N dimension: for every input position p the
 // tensor core computes Y[p, tap*cout + c] = sum_ch x[p, ch] * W[c, ch, tap]  (N = 9*cout <= 32, K = Cin), reading the
 // activation ONCE, and the output pixel is the sum of its 9 neighbours' matching columns:
 //     out[c, y, x] = act(bias[c] + sum_{ty,tx} Y[(y+ty-1, x+tx-1), (ty*3+tx)*cout + c]).
-// Round 1 did this with two launches and a 133 MB column-planar Y in HBM (fgt_gemm_tc "taps as N" + fgt_tapsum);
-// here Y of a 16x8 output tile plus its 1-pixel halo (18x10 = 180 positions = two M=128 MMA tiles) goes from TMEM to
-// shared memory and never leaves the SM: HBM traffic = the activation once + the 3-channel image.
+// Y of a 16x8 output tile plus its 1-pixel halo (18x10 = 180 positions = three M=64 wgmma blocks) goes from registers
+// to shared memory and never leaves the SM: HBM traffic = the activation once + the 3-channel image.
 //
-//   warp 0     : TMA producer (halo box (64 ch, 18, 10) per 64-channel chunk and plane; zero fill = the conv's padding)
-//   warp 1     : MMA issuer   (3-term split-bf16, M=128 x N=32, two M tiles per chunk, accumulators double-buffered)
-//   warps 2..5 : epilogue     (tcgen05.ld -> Y rows in smem (pitch 33 floats: conflict-free both ways) -> 9-tap sums ->
-//                              bias, activation, coalesced stores)
+//   warp 4     : TMA producer (halo box (64 ch, 18, 10) per 64-channel chunk and plane; zero fill = the conv's padding)
+//   warps 0..3 : one warpgroup: wgmma (3-term split-bf16, M=64 x N=32, three M blocks per chunk, fp32 accumulators in
+//                registers) -> Y rows in smem (pitch 33 floats: conflict-free both ways) -> 9-tap sums -> bias,
+//                activation, coalesced stores
 #include "common.h"
 #include "ptx.cuh"
 
@@ -22,8 +21,9 @@ namespace fgt {
 constexpr int kTailTW = 16, kTailTH = 8;               // output tile
 constexpr int kTailHW = kTailTW + 2, kTailHH = kTailTH + 2;
 constexpr int kTailRows = kTailHW * kTailHH;           // 180 halo positions
-constexpr int kTailAPlane = 256 * 128;                 // smem per plane and stage: two M tiles of 128 rows x 128 B
-constexpr int kTailAStage = 2 * kTailAPlane;           // 64 KB
+constexpr int kTailMBlocks = 3;                        // M=64 blocks covering the 180 rows
+constexpr int kTailAPlane = kTailMBlocks * 64 * 128;   // smem per plane and stage: 192 rows x 128 B
+constexpr int kTailAStage = 2 * kTailAPlane;           // 48 KB
 constexpr int kTailStages = 2;
 constexpr int kTailMaxChunks = 4;                      // Cin <= 256
 constexpr int kTailBBlk = 32 * 128;                    // one (chunk, plane) block of the weights: 32 rows x 128 B
@@ -34,6 +34,7 @@ constexpr int kTailSmemB = kTailSmemA + kTailStages * kTailAStage;
 constexpr int kTailSmemY = kTailSmemB + kTailMaxChunks * 2 * kTailBBlk;
 constexpr int kTailSmemBar = kTailSmemY + 2 * kTailYBuf;
 constexpr int kTailSmem = kTailSmemBar + 256 + 1024;
+constexpr int kTailThreads = 160;                      // one consumer warpgroup + one producer warp
 
 struct TailParams {
   CUtensorMap a_map, b_map;
@@ -44,7 +45,7 @@ struct TailParams {
   long long os_n, os_c, os_y, os_x;
 };
 
-__global__ void __launch_bounds__(192, 1) conv_tail_kernel(const __grid_constant__ TailParams p) {
+__global__ void __launch_bounds__(kTailThreads, 1) conv_tail_kernel(const __grid_constant__ TailParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sgen = smem_raw + (sbase - smem_u32(smem_raw));
@@ -52,37 +53,25 @@ __global__ void __launch_bounds__(192, 1) conv_tail_kernel(const __grid_constant
   const uint32_t bar = sbase + kTailSmemBar;
   auto full_bar = [&](int s) { return bar + 8u * s; };
   auto empty_bar = [&](int s) { return bar + 8u * (2 + s); };
-  auto accf_bar = [&](int b) { return bar + 8u * (4 + b); };
-  auto acce_bar = [&](int b) { return bar + 8u * (6 + b); };
-  const uint32_t w_bar = bar + 8u * 8;
-  const uint32_t tmem_slot = bar + 8u * 9;
+  const uint32_t w_bar = bar + 8u * 4;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     for (int s = 0; s < kTailStages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(accf_bar(b), 1);
-      mbar_init(acce_bar(b), 4);
+      mbar_init(empty_bar(s), 4);  // one arrival per consumer warp
     }
     mbar_init(w_bar, 1);
     fence_mbar_init();
     tma_prefetch_desc(&p.a_map);
     tma_prefetch_desc(&p.b_map);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem_base) : "r"(tmem_slot));
   pdl_launch_dependents();
   pdl_wait();
 
   const int tiles_per_z = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------------------------------------ TMA producer
     if (elect_one()) {
       // weights: every (chunk, plane) block once per CTA
@@ -97,7 +86,7 @@ __global__ void __launch_bounds__(192, 1) conv_tail_kernel(const __grid_constant
         const int rem = tile - z * tiles_per_z;
         const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
         for (int c = 0; c < p.chunks; ++c) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_wait_quiet(empty_bar(stage), phase ^ 1u);
           const uint32_t sa = sbase + kTailSmemA + stage * kTailAStage;
           mbar_expect_tx(full_bar(stage), 2u * kTailRows * 128u);
           tma_load_5d(sa, &p.a_map, full_bar(stage), c * 64, tx * kTailTW - 1, ty * kTailTH - 1, z, 0);
@@ -107,109 +96,93 @@ __global__ void __launch_bounds__(192, 1) conv_tail_kernel(const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (elect_one()) {
-      const uint32_t idesc = umma_idesc_bf16(128, 32);
-      int stage = 0, lt = 0;
-      uint32_t phase = 0;
-      mbar_wait(w_bar, 0);
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++lt) {
-        const int buf = lt & 1;
-        mbar_wait(acce_bar(buf), ((lt >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        for (int c = 0; c < p.chunks; ++c) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = sbase + kTailSmemA + stage * kTailAStage;
-          const uint64_t b_hi = umma_desc_sw128(sbase + kTailSmemB + (c * 2 + 0) * kTailBBlk);
-          const uint64_t b_lo = umma_desc_sw128(sbase + kTailSmemB + (c * 2 + 1) * kTailBBlk);
-#pragma unroll
-          for (int mt = 0; mt < 2; ++mt) {
-            const uint32_t d = tmem_base + static_cast<uint32_t>(buf * 64 + mt * 32);
-            const uint64_t a_hi = umma_desc_sw128(sa + mt * 128 * 128);
-            const uint64_t a_lo = umma_desc_sw128(sa + kTailAPlane + mt * 128 * 128);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t ko = static_cast<uint64_t>(k * 2);
-              umma_bf16(d, a_lo + ko, b_hi + ko, idesc, (c | k) != 0);
-              umma_bf16(d, a_hi + ko, b_lo + ko, idesc, 1u);
-              umma_bf16(d, a_hi + ko, b_hi + ko, idesc, 1u);
-            }
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == kTailStages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(accf_bar(buf));
-      }
-    }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------ epilogue (warps 2..5)
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    const int py = r / kTailTW, px = r - py * kTailTW;
-    const int cout = p.cout;
-    float bias[4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) bias[c] = c < cout ? __ldg(p.bias + c) : 0.f;
-    int lt = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++lt) {
-      const int buf = lt & 1;
-      const int z = tile / tiles_per_z;
-      const int rem = tile - z * tiles_per_z;
-      const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
-      float* Y = reinterpret_cast<float*>(sgen + kTailSmemY + buf * kTailYBuf);
-      mbar_wait(accf_bar(buf), (lt >> 1) & 1u);
-      tc_fence_after();
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        uint32_t raw[32];
-        tmem_ld32(lane_base + static_cast<uint32_t>(buf * 64 + mt * 32), raw);
-        tmem_ld_wait();
-        const int row = mt * 128 + r;
-        if (row < kTailRows) {
-          float* yr = Y + row * kTailYPitch;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) yr[j] = __uint_as_float(raw[j]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acce_bar(buf));
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");  // all 180 rows of Y are in shared memory
-      const int oy = ty * kTailTH + py, ox = tx * kTailTW + px;
-      if (oy < p.H && ox < p.W) {
-        float acc[4] = {bias[0], bias[1], bias[2], bias[3]};
-#pragma unroll
-        for (int t = 0; t < 9; ++t) {
-          const float* yr = Y + ((py + t / 3) * kTailHW + px + t % 3) * kTailYPitch + t * cout;
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-            if (c < cout) acc[c] += yr[c];
-        }
-        float* op = p.out + z * p.os_n + oy * p.os_y + ox * p.os_x;
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < cout) {
-            float v = acc[c];
-            if (p.act == FGT_ACT_TANH) v = tanhf(v);
-            else if (p.act == FGT_ACT_LEAKY02) v = v > 0.f ? v : 0.2f * v;
-            else if (p.act == FGT_ACT_RELU) v = fmaxf(v, 0.f);
-            else if (p.act == FGT_ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
-            op[c * p.os_c] = v;
-          }
-      }
-      // Y is double-buffered: the barrier of the next tile orders these reads before tile lt+2 rewrites this buffer
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
+  // -------------------------------------------------------------- warpgroup: MMA + tap sums (warps 0..3)
+  const int r = threadIdx.x;  // output pixel of the tile for the tap sums
+  const int py = r / kTailTW, px = r - py * kTailTW;
+  const int g = lane >> 2, qc = lane & 3;
+  const int cout = p.cout;
+  float bias[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) bias[c] = c < cout ? __ldg(p.bias + c) : 0.f;
+  mbar_wait_quiet(w_bar, 0);
+  int stage = 0, lt = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++lt) {
+    const int buf = lt & 1;
+    const int z = tile / tiles_per_z;
+    const int rem = tile - z * tiles_per_z;
+    const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
+    float acc[kTailMBlocks][16];
+    for (int c = 0; c < p.chunks; ++c) {
+      mbar_wait_quiet(full_bar(stage), phase);
+      const uint32_t sa = sbase + kTailSmemA + stage * kTailAStage;
+      const uint64_t b_hi = gmma_desc_sw128(sbase + kTailSmemB + (c * 2 + 0) * kTailBBlk);
+      const uint64_t b_lo = gmma_desc_sw128(sbase + kTailSmemB + (c * 2 + 1) * kTailBBlk);
+#pragma unroll
+      for (int mb = 0; mb < kTailMBlocks; ++mb) fence_regs(acc[mb]);
+      wgmma_fence();
+#pragma unroll
+      for (int mb = 0; mb < kTailMBlocks; ++mb) {
+        const uint64_t a_hi = gmma_desc_sw128(sa + mb * 64 * 128);
+        const uint64_t a_lo = gmma_desc_sw128(sa + kTailAPlane + mb * 64 * 128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t ko = static_cast<uint64_t>(k * 2);
+          wgmma_ss<32, false>(acc[mb], a_lo + ko, b_hi + ko, (c | k) != 0);
+          wgmma_ss<32, false>(acc[mb], a_hi + ko, b_lo + ko, 1u);
+          wgmma_ss<32, false>(acc[mb], a_hi + ko, b_hi + ko, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int mb = 0; mb < kTailMBlocks; ++mb) fence_regs(acc[mb]);
+      if (lane == 0) mbar_arrive(empty_bar(stage));
+      if (++stage == kTailStages) { stage = 0; phase ^= 1u; }
+    }
+    // accumulator fragment -> Y rows (acc[mb][4 jj + 2 h + e] = Y[64 mb + 16 warp + g + 8 h][8 jj + 2 qc + e])
+    float* Y = reinterpret_cast<float*>(sgen + kTailSmemY + buf * kTailYBuf);
+#pragma unroll
+    for (int mb = 0; mb < kTailMBlocks; ++mb)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = mb * 64 + warp * 16 + g + 8 * h;
+        if (row < kTailRows) {
+          float* yr = Y + row * kTailYPitch + 2 * qc;
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            yr[8 * jj] = acc[mb][4 * jj + 2 * h];
+            yr[8 * jj + 1] = acc[mb][4 * jj + 2 * h + 1];
+          }
+        }
+      }
+    asm volatile("bar.sync 1, 128;\n" ::: "memory");  // all 180 rows of Y are in shared memory
+    const int oy = ty * kTailTH + py, ox = tx * kTailTW + px;
+    if (oy < p.H && ox < p.W) {
+      float a[4] = {bias[0], bias[1], bias[2], bias[3]};
+#pragma unroll
+      for (int t = 0; t < 9; ++t) {
+        const float* yr = Y + ((py + t / 3) * kTailHW + px + t % 3) * kTailYPitch + t * cout;
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (c < cout) a[c] += yr[c];
+      }
+      float* op = p.out + z * p.os_n + oy * p.os_y + ox * p.os_x;
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (c < cout) {
+          float v = a[c];
+          if (p.act == FGT_ACT_TANH) v = tanhf(v);
+          else if (p.act == FGT_ACT_LEAKY02) v = v > 0.f ? v : 0.2f * v;
+          else if (p.act == FGT_ACT_RELU) v = fmaxf(v, 0.f);
+          else if (p.act == FGT_ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
+          op[c * p.os_c] = v;
+        }
+    }
+    // Y is double-buffered: the barrier of the next tile orders these reads before tile lt+2 rewrites this buffer
   }
 }
 
@@ -257,7 +230,7 @@ extern "C" int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, 
   }
   int grid = num_sms();
   if (grid > p.total_tiles) grid = p.total_tiles;
-  launch_k(conv_tail_kernel, dim3(grid), dim3(192), kTailSmem, reinterpret_cast<cudaStream_t>(stream), p);
+  launch_k(conv_tail_kernel, dim3(grid), dim3(kTailThreads), kTailSmem, reinterpret_cast<cudaStream_t>(stream), p);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }

@@ -1,23 +1,21 @@
-// Fused softmax(QK^T * scale) V on tcgen05 for FGT's two attentions (never materialises scores).
+// Fused softmax(QK^T * scale) V on wgmma for FGT's two attentions (never materialises scores).
 //
 // One CTA = 128 query rows x one head (head dim 128). Keys are consumed in tiles of 64:
-//   warp 0 / 6 : TMA producers (K tiles / V tiles, two independent 3-deep rings; V stays row-major
-//                [keys, d] and is consumed as an MN-major B operand, so the V projection GEMM stores
-//                through its vector path instead of a transposed scalar scatter)
-//   warp 1 / 7 : MMA issuers  (S_j = Q K_j^T / O += P_j V_j as two independent instruction streams,
-//                              3-term split-bf16, A operands in TMEM)
-//   warps 2..5 : softmax      (thread = query row: stages its Q row in TMEM once, then per key tile
-//                              online max/sum in fp32 and P written straight to TMEM as packed bf16)
-// Q and P live in tensor memory as the A operands (tcgen05.mma [d],[a],b-desc): no shared-memory
-// re-read of Q per instruction (SS-mode was smem-bandwidth bound) and no smem round trip for P.
-// S is double-buffered in TMEM (S_{j+1} runs while the softmax warps work on tile j); the O
-// accumulator stays in TMEM across key tiles and is rescaled in place only when the running max
-// outgrows the reference max by more than 2^8 (lazy rescaling), so it is read back exactly once.
+//   warp 8     : TMA producer (K tiles and V tiles, two independent 2-deep rings; V stays row-major [keys, d] and is
+//                consumed as an MN-major B operand, so the V projection GEMM stores through its paired path instead of
+//                a transposed scatter)
+//   warps 0..7 : two consumer warpgroups, warpgroup w owns query rows [64 w, 64 w + 64): S_j = Q K_j^T from shared
+//                memory (Q staged there once, 128B-swizzled), online softmax on the accumulator registers, then
+//                O += P_j V_j with P as the register A operand (the S accumulator layout is the A fragment layout),
+//                all 3-term split-bf16 with fp32 accumulation; O stays in registers across key tiles
+// The two warpgroups run independently, so one's softmax overlaps the other's MMAs. O is rescaled only when the
+// running max outgrows the reference max by more than 2^8 (lazy rescaling; softmax is shift-invariant, so exact).
 //
 // mode DENSE    (TMHSA, attention_base.py:93-99): every key tile of the (batch=zone) sequence.
 // mode WINDOWED (SWMHSA, attention_flow.py:130-164): a 128-row query tile is two 64-token windows;
 //   its key list is [global tiles..., own window tile 2i, own window tile 2i+1] with a block-diagonal
-//   mask on the two local tiles. Global (pooled) tokens live after the local rows of each frame.
+//   mask on the two local tiles (warpgroup w attends to local tile w only). Global (pooled) tokens live after the
+//   local rows of each frame.
 #include "common.h"
 #include "ptx.cuh"
 
@@ -26,18 +24,16 @@ namespace fgt {
 constexpr int kKBlk = 64 * 128;       // one (plane, k-chunk) block of K: 64 keys x 128 B
 constexpr int kVBlk = 128 * 128;      // one plane of a V tile: two [64 keys x 64 dims (128 B)] halves of 8 KB
 constexpr int kVHalf = 64 * 128;
+constexpr int kQBlk = 128 * 128;      // one (plane, k-chunk) block of Q: 128 rows x 128 B
 constexpr int kKStage = 4 * kKBlk;    // 32 KB
 constexpr int kVStage = 2 * kVBlk;    // 32 KB
-constexpr int kStages = 3;            // K and V rings
-constexpr int kSmemK = 0;
-constexpr int kSmemV = kSmemK + kStages * kKStage;   // +96 KB
-constexpr int kSmemBar = kSmemV + kStages * kVStage;  // +96 KB = 192 KB
+constexpr int kStages = 2;            // K and V rings
+constexpr int kSmemQ = 0;
+constexpr int kSmemK = kSmemQ + 4 * kQBlk;            // +64 KB
+constexpr int kSmemV = kSmemK + kStages * kKStage;    // +64 KB
+constexpr int kSmemBar = kSmemV + kStages * kVStage;  // +64 KB = 192 KB
 constexpr int kFlashSmem = kSmemBar + 256 + 1024;
-// TMEM columns (512 allocated)
-constexpr uint32_t kTmS = 0;      // S buffers: [0,64), [64,128)
-constexpr uint32_t kTmO = 128;    // O accumulator: 128 fp32 columns
-constexpr uint32_t kTmQ = 256;    // Q as the A operand: hi plane [256,320), lo plane [320,384) (2 bf16 / column)
-constexpr uint32_t kTmP = 384;    // P as the A operand, double-buffered: buffer b at 384 + 64 b = hi 32 cols | lo 32 cols
+constexpr int kFlashThreads = 288;    // 2 consumer warpgroups + 1 producer warp
 
 struct FlashParams {
   CUtensorMap k_map, v_map;
@@ -52,10 +48,18 @@ struct FlashParams {
   long long out_plane, out_batch_stride;
   int out_ld;
   const int* out_rowmap;  // optional: query row (batch * Lq + row) -> output row of a [rows, out_ld] buffer, < 0 = dropped
-  long long* trace;  // optional per-tile clock64 trace of CTA (0,0,0): [role 0..2][tile][8]
 };
 
-__global__ void __launch_bounds__(256, 1) flash_kernel(const __grid_constant__ FlashParams p) {
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+__global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_constant__ FlashParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5;
@@ -64,50 +68,27 @@ __global__ void __launch_bounds__(256, 1) flash_kernel(const __grid_constant__ F
 
   const uint32_t bar = sbase + kSmemBar;
   auto k_full = [&](int s) { return bar + 8u * (0 + s); };
-  auto k_empty = [&](int s) { return bar + 8u * (3 + s); };
-  auto v_full = [&](int s) { return bar + 8u * (6 + s); };
-  auto v_empty = [&](int s) { return bar + 8u * (9 + s); };
-  auto s_full = [&](int s) { return bar + 8u * (12 + s); };
-  auto s_empty = [&](int s) { return bar + 8u * (14 + s); };
-  auto p_full = [&](int b) { return bar + 8u * (16 + b); };   // softmax wrote P_j (buffer j&1) to TMEM
-  auto p_empty = [&](int b) { return bar + 8u * (18 + b); };  // PV_j retired: buffer free, O includes tile j
-  const uint32_t q_ready = bar + 8u * 20;  // Q rows staged in TMEM
-  const uint32_t tmem_slot = bar + 8u * 21;
+  auto k_empty = [&](int s) { return bar + 8u * (2 + s); };
+  auto v_full = [&](int s) { return bar + 8u * (4 + s); };
+  auto v_empty = [&](int s) { return bar + 8u * (6 + s); };
 
   const int n_tiles = (p.mode == 0) ? (p.Lk + 63) / 64 : p.n_glob_tiles + 2;
-  const bool tr = p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-#define FGT_TRACE(role, tile, slot) \
-  if (tr) p.trace[((role) * 64 + ((tile) & 63)) * 8 + (slot)] = clock64()
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(k_full(s), 1);
-      mbar_init(k_empty(s), 1);
+      mbar_init(k_empty(s), 8);  // one arrival per consumer warp
       mbar_init(v_full(s), 1);
-      mbar_init(v_empty(s), 1);
+      mbar_init(v_empty(s), 8);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(s_full(s), 1);
-      mbar_init(s_empty(s), 128);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(p_full(b), 128);
-      mbar_init(p_empty(b), 1);
-    }
-    mbar_init(q_ready, 128);
     fence_mbar_init();
     tma_prefetch_desc(&p.k_map);
     tma_prefetch_desc(&p.v_map);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   // PDL: the prologue above overlapped the previous kernel's tail; nothing before this line touches global data
   pdl_launch_dependents();
   pdl_wait();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem_base) : "r"(tmem_slot));
 
   auto key_row0 = [&](int j) -> int {
     if (p.mode == 0) return j * 64;
@@ -115,33 +96,20 @@ __global__ void __launch_bounds__(256, 1) flash_kernel(const __grid_constant__ F
     return (2 * qt + (j - p.n_glob_tiles)) * 64;
   };
 
-  if (warp == 0) {
-    // ------------------------------------------------------------ K producer
+  if (warp == 8) {
+    // ------------------------------------------------------------ K / V producer
     if (elect_one()) {
       int s = 0;
       uint32_t ph = 0;
       for (int j = 0; j < n_tiles; ++j) {
         const int r0 = key_row0(j);
-        mbar_wait(k_empty(s), ph ^ 1u);
-        FGT_TRACE(0, j, 0);
+        mbar_wait_quiet(k_empty(s), ph ^ 1u);
         mbar_expect_tx(k_full(s), kKStage);
         for (int pl = 0; pl < 2; ++pl)
           for (int kc = 0; kc < 2; ++kc)
             tma_load_4d(sbase + kSmemK + s * kKStage + (pl * 2 + kc) * kKBlk, &p.k_map, k_full(s),
                         head * 128 + kc * 64, r0, batch, pl);
-        if (++s == kStages) { s = 0; ph ^= 1u; }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 6) {
-    // ------------------------------------------------------------ V^T producer
-    if (elect_one()) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int j = 0; j < n_tiles; ++j) {
-        const int r0 = key_row0(j);
-        mbar_wait(v_empty(s), ph ^ 1u);
-        FGT_TRACE(0, j, 1);
+        mbar_wait_quiet(v_empty(s), ph ^ 1u);
         mbar_expect_tx(v_full(s), kVStage);
         for (int pl = 0; pl < 2; ++pl)
           for (int hf = 0; hf < 2; ++hf)
@@ -151,203 +119,144 @@ __global__ void __launch_bounds__(256, 1) flash_kernel(const __grid_constant__ F
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ S = Q K^T issuer
-    if (elect_one()) {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 64);
-      int ks = 0;
-      uint32_t kph = 0;
-      mbar_wait(q_ready, 0);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int sb = j & 1;
-        mbar_wait(k_full(ks), kph);
-        FGT_TRACE(1, j, 0);
-        mbar_wait(s_empty(sb), ((j >> 1) & 1u) ^ 1u);
-        FGT_TRACE(1, j, 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + kTmS + static_cast<uint32_t>(sb * 64);
-        uint32_t acc = 0;
-#pragma unroll
-        for (int kc = 0; kc < 2; ++kc) {
-          const uint64_t b_hi = umma_desc_sw128(sbase + kSmemK + ks * kKStage + (0 * 2 + kc) * kKBlk);
-          const uint64_t b_lo = umma_desc_sw128(sbase + kSmemK + ks * kKStage + (1 * 2 + kc) * kKBlk);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t ko = static_cast<uint64_t>(k * 2);
-            const uint32_t qc = static_cast<uint32_t>((kc * 4 + k) * 8);  // 16 dims = 8 packed columns
-            umma_bf16_ts(d, tmem_base + kTmQ + 64u + qc, b_hi + ko, idesc_s, acc);  // Q_lo * K_hi
-            acc = 1;
-            umma_bf16_ts(d, tmem_base + kTmQ + qc, b_lo + ko, idesc_s, 1u);        // Q_hi * K_lo
-            umma_bf16_ts(d, tmem_base + kTmQ + qc, b_hi + ko, idesc_s, 1u);        // Q_hi * K_hi
-          }
-        }
-        umma_commit(k_empty(ks));
-        umma_commit(s_full(sb));
-        FGT_TRACE(1, j, 2);
-        if (++ks == kStages) { ks = 0; kph ^= 1u; }
-      }
+    return;
+  }
+
+  // -------------------------------------------------------------- consumers (warps 0..7)
+  const int wg = warp >> 2;
+  {
+    // Q tile -> shared memory as the K-major A operand: block (plane, 64-dim chunk) of 128 rows x 128 B, 16-byte chunk c
+    // of row r at c ^ (r & 7) (the 128B swizzle). 256 threads x 16 chunks.
+    uint8_t* sq = smem_raw + (sbase - smem_u32(smem_raw)) + kSmemQ;
+    for (int i = threadIdx.x; i < 2 * 128 * 16; i += 256) {
+      const int pl = i >> 11, r = (i >> 4) & 127, c = i & 15;
+      const int qrow = qt * 128 + r;
+      uint4 v = make_uint4(0u, 0u, 0u, 0u);
+      if (qrow < p.Lq)
+        v = __ldg(reinterpret_cast<const uint4*>(p.q_hi + pl * p.q_plane + batch * p.q_batch_stride +
+                                                 static_cast<long long>(qrow) * p.q_ld + head * 128) + c);
+      const int kc = c >> 3;
+      *reinterpret_cast<uint4*>(sq + (pl * 2 + kc) * kQBlk + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = v;
     }
-    __syncwarp();
-  } else if (warp == 7) {
-    // ------------------------------------------------------------ O += P V issuer
-    if (elect_one()) {
-      const uint32_t idesc_o = umma_idesc_bf16(128, 128) | kIdescBMajorMN;  // B = V tile [keys, d]: d (N) contiguous
-      int vs = 0;
-      uint32_t vph = 0;
-      for (int j = 0; j < n_tiles; ++j) {
-        const int pb = j & 1;
-        mbar_wait(v_full(vs), vph);
-        FGT_TRACE(1, j, 3);
-        mbar_wait(p_full(pb), (j >> 1) & 1u);
-        FGT_TRACE(1, j, 4);
-        tc_fence_after();
-        const uint32_t d = tmem_base + kTmO;
-        const uint32_t pa = tmem_base + kTmP + static_cast<uint32_t>(pb * 64);
-        const uint64_t b_hi = umma_desc_sw128_mn(sbase + kSmemV + vs * kVStage, kVHalf);
-        const uint64_t b_lo = umma_desc_sw128_mn(sbase + kSmemV + vs * kVStage + kVBlk, kVHalf);
+    fence_proxy_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads
+    asm volatile("bar.sync 1, 256;\n" ::: "memory");
+  }
+
+  const int g = lane >> 2, qc = lane & 3;
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_ref[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t q_off = static_cast<uint32_t>(wg) * 64u * 128u;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_tiles; ++j) {
+    int n_valid = 64;  // key columns [0, n_valid) of this tile are live for this warpgroup's rows
+    if (p.mode == 0) {
+      n_valid = min(64, p.Lk - j * 64);
+    } else if (j < p.n_glob_tiles) {
+      n_valid = min(64, p.glob_count - j * 64);
+    } else {
+      n_valid = (wg == j - p.n_glob_tiles) ? 64 : 0;
+    }
+    mbar_wait_quiet(k_full(s), ph);
+    float sv[32];
+    if (n_valid > 0) {
+      fence_regs(sv);
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 2; ++kc) {
+        const uint32_t kb = sbase + kSmemK + s * kKStage;
+        const uint64_t b_hi = gmma_desc_sw128(kb + (0 * 2 + kc) * kKBlk);
+        const uint64_t b_lo = gmma_desc_sw128(kb + (1 * 2 + kc) * kKBlk);
+        const uint64_t a_hi = gmma_desc_sw128(sbase + kSmemQ + (0 * 2 + kc) * kQBlk + q_off);
+        const uint64_t a_lo = gmma_desc_sw128(sbase + kSmemQ + (1 * 2 + kc) * kQBlk + q_off);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          const uint64_t ko = static_cast<uint64_t>(k * 128);  // 16 keys = two 8-row swizzle atoms = 2048 B >> 4
-          const uint32_t pc = static_cast<uint32_t>(k * 8);
-          umma_bf16_ts(d, pa + 32u + pc, b_hi + ko, idesc_o, (j | k) != 0);  // P_lo * V_hi
-          umma_bf16_ts(d, pa + pc, b_lo + ko, idesc_o, 1u);                  // P_hi * V_lo
-          umma_bf16_ts(d, pa + pc, b_hi + ko, idesc_o, 1u);                  // P_hi * V_hi
-        }
-        umma_commit(v_empty(vs));
-        umma_commit(p_empty(pb));
-        FGT_TRACE(1, j, 5);
-        if (++vs == kStages) { vs = 0; vph ^= 1u; }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------ softmax / output warps (2..5)
-    // O stays in TMEM. Exponentials are taken against a reference max m_ref that is only raised (and
-    // O / l rescaled in place) when the running max outgrows it by more than 2^8 — softmax is
-    // shift-invariant, so the result is exact; P values stay <= 256. Q and P are staged in TMEM as
-    // the A operands of the MMAs (no shared-memory round trip, no re-read of Q per instruction).
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    const int qrow = qt * 128 + r;
-    {
-      // this thread's query row: 128 bf16 per plane = 64 packed words -> TMEM columns
-      const __nv_bfloat16* qp = p.q_hi + batch * p.q_batch_stride + static_cast<long long>(qrow) * p.q_ld + head * 128;
-#pragma unroll
-      for (int pl = 0; pl < 2; ++pl) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t w[32];
-          const uint4* src = reinterpret_cast<const uint4*>(qp + pl * p.q_plane + half * 64);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            uint4 v = make_uint4(0u, 0u, 0u, 0u);
-            if (qrow < p.Lq) v = __ldg(src + i);
-            w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
-          }
-          tmem_st32(lane_base + kTmQ + static_cast<uint32_t>(pl * 64 + half * 32), w);
+          const uint64_t ko = static_cast<uint64_t>(k * 2);
+          wgmma_ss<64, false>(sv, a_lo + ko, b_hi + ko, (kc | k) != 0);  // Q_lo * K_hi
+          wgmma_ss<64, false>(sv, a_hi + ko, b_lo + ko, 1u);             // Q_hi * K_lo
+          wgmma_ss<64, false>(sv, a_hi + ko, b_hi + ko, 1u);             // Q_hi * K_hi
         }
       }
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(q_ready);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(sv);
     }
-    float m_ref = -INFINITY, l_run = 0.f;
+    if (lane == 0) mbar_arrive(k_empty(s));
 
-    for (int j = 0; j < n_tiles; ++j) {
-      const int s = j & 1;
-      const bool trs = tr && threadIdx.x == 64;
-      if (trs) p.trace[(2 * 64 + (j & 63)) * 8 + 0] = clock64();
-      mbar_wait(s_full(s), (j >> 1) & 1u);
-      if (trs) p.trace[(2 * 64 + (j & 63)) * 8 + 1] = clock64();
-      tc_fence_after();
-      float sv[64];
-      {
-        uint32_t raw[32];
-        tmem_ld32(lane_base + kTmS + static_cast<uint32_t>(s * 64), raw);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) sv[i] = __uint_as_float(raw[i]);
-        tmem_ld32(lane_base + kTmS + static_cast<uint32_t>(s * 64 + 32), raw);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) sv[32 + i] = __uint_as_float(raw[i]);
-      }
-      tc_fence_before();
-      mbar_arrive(s_empty(s));
-      if (trs) p.trace[(2 * 64 + (j & 63)) * 8 + 2] = clock64();
-
-      int n_valid = 64;  // columns [0, n_valid) are live for this row
-      if (p.mode == 0) {
-        n_valid = min(64, p.Lk - j * 64);
-      } else if (j < p.n_glob_tiles) {
-        n_valid = min(64, p.glob_count - j * 64);
-      } else {
-        n_valid = ((r >> 6) == (j - p.n_glob_tiles)) ? 64 : 0;
-      }
+    uint32_t pa_hi[16], pa_lo[16];
+    if (n_valid > 0) {
+      // thread holds S[row g + 8 h][8 jj + 2 qc + e] in sv[4 jj + 2 h + e]; a row is spread over the 4 lanes of a quad
       if (n_valid != 64) {
 #pragma unroll
-        for (int i = 0; i < 64; ++i) sv[i] = (i < n_valid) ? sv[i] : -INFINITY;
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * jj + 2 * qc + e >= n_valid) sv[4 * jj + e] = sv[4 * jj + 2 + e] = -INFINITY;
       }
-      float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-      for (int i = 0; i < 64; i += 2) {
-        mx0 = fmaxf(mx0, sv[i]);
-        mx1 = fmaxf(mx1, sv[i + 1]);
-      }
-      const float m_tile = fmaxf(mx0, mx1) * p.scale_log2;  // scale > 0
-      const bool grow = m_tile > m_ref + 8.f;               // also true for the first finite maximum
-      const float alpha = grow ? ex2_approx(m_ref - m_tile) : 1.f;  // m_ref = -inf -> 0
-      if (grow) m_ref = m_tile;
-      const float neg_m = (m_ref == -INFINITY) ? 0.f : -m_ref;
-      float ps0 = 0.f, ps1 = 0.f, ps2 = 0.f, ps3 = 0.f;
+      for (int h = 0; h < 2; ++h) {
+        float mx = -INFINITY;
 #pragma unroll
-      for (int i = 0; i < 64; i += 4) {
-        sv[i] = ex2_approx(fmaf(sv[i], p.scale_log2, neg_m));
-        sv[i + 1] = ex2_approx(fmaf(sv[i + 1], p.scale_log2, neg_m));
-        sv[i + 2] = ex2_approx(fmaf(sv[i + 2], p.scale_log2, neg_m));
-        sv[i + 3] = ex2_approx(fmaf(sv[i + 3], p.scale_log2, neg_m));
-        ps0 += sv[i]; ps1 += sv[i + 1]; ps2 += sv[i + 2]; ps3 += sv[i + 3];
-      }
-      l_run = l_run * alpha + ((ps0 + ps1) + (ps2 + ps3));
-      uint32_t phi[32], plo[32];
+        for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * h], sv[4 * jj + 2 * h + 1]));
+        const float m_tile = quad_max(mx) * p.scale_log2;  // scale > 0
+        const bool grow = m_tile > m_ref[h] + 8.f;          // also true for the first finite maximum
+        const float alpha = grow ? ex2_approx(m_ref[h] - m_tile) : 1.f;  // m_ref = -inf -> 0
+        if (grow) m_ref[h] = m_tile;
+        const float neg_m = (m_ref[h] == -INFINITY) ? 0.f : -m_ref[h];
+        float ps = 0.f;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) split_bf16x2(sv[2 * i], sv[2 * i + 1], phi[i], plo[i]);
-
-      // P buffer j&1 is free once PV_{j-2} retired
-      if (trs) p.trace[(2 * 64 + (j & 63)) * 8 + 3] = clock64();
-      mbar_wait(p_empty(s), ((j >> 1) & 1u) ^ 1u);
-      if (trs) p.trace[(2 * 64 + (j & 63)) * 8 + 4] = clock64();
-      tc_fence_after();
-      if (j > 0 && __any_sync(0xffffffffu, grow)) {  // tcgen05.ld/st are warp-collective
-        // rescaling O needs every earlier PV retired: wait for PV_{j-1}
-        mbar_wait(p_empty((j - 1) & 1), ((j - 1) >> 1) & 1u);
-        tc_fence_after();
-        const float a = grow ? alpha : 1.f;
+        for (int jj = 0; jj < 8; ++jj) {
+          sv[4 * jj + 2 * h] = ex2_approx(fmaf(sv[4 * jj + 2 * h], p.scale_log2, neg_m));
+          sv[4 * jj + 2 * h + 1] = ex2_approx(fmaf(sv[4 * jj + 2 * h + 1], p.scale_log2, neg_m));
+          ps += sv[4 * jj + 2 * h] + sv[4 * jj + 2 * h + 1];
+        }
+        l_run[h] = l_run[h] * alpha + ps;
+        if (grow) {
 #pragma unroll
-        for (int c0 = 0; c0 < 128; c0 += 32) {
-          uint32_t raw[32];
-          tmem_ld32(lane_base + kTmO + c0, raw);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) raw[i] = __float_as_uint(__uint_as_float(raw[i]) * a);
-          tmem_st32(lane_base + kTmO + c0, raw);
+          for (int jj = 0; jj < 16; ++jj) {
+            o[4 * jj + 2 * h] *= alpha;
+            o[4 * jj + 2 * h + 1] *= alpha;
+          }
         }
       }
-      tmem_st32(lane_base + kTmP + static_cast<uint32_t>(s * 64), phi);
-      tmem_st32(lane_base + kTmP + static_cast<uint32_t>(s * 64) + 32u, plo);
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(p_full(s));
-      if (trs) p.trace[(2 * 64 + (j & 63)) * 8 + 5] = clock64();
+      // P as the A operand: k16 chunk kk = sv[8 kk .. 8 kk + 7] -> {(g, 2qc), (g + 8, 2qc), (g, 2qc + 8), (g + 8, 2qc + 8)}
+#pragma unroll
+      for (int i = 0; i < 16; ++i) split_bf16x2(sv[2 * i], sv[2 * i + 1], pa_hi[i], pa_lo[i]);
     }
-    // last PV retired -> read the accumulator once, normalise, store split-bf16
-    mbar_wait(p_empty((n_tiles - 1) & 1), ((n_tiles - 1) >> 1) & 1u);
-    tc_fence_after();
-    const float inv = 1.f / l_run;
-    // Output row: in place (batch-strided), or scattered through the row map — the attention then undoes the zone /
-    // window regrouping itself (attention_base.py:100-103, attention_flow.py:165-168) and the output projection is a
-    // plain row-major GEMM over the real tokens only.
+
+    mbar_wait_quiet(v_full(s), ph);
+    if (n_valid > 0) {
+      const uint32_t vb = sbase + kSmemV + s * kVStage;
+      const uint64_t b_hi = gmma_desc_sw128_mn(vb, kVHalf);
+      const uint64_t b_lo = gmma_desc_sw128_mn(vb + kVBlk, kVHalf);
+      fence_regs(o);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t ko = static_cast<uint64_t>(k * 128);  // 16 keys = two 8-row swizzle atoms = 2048 B >> 4
+        const uint32_t ah[4] = {pa_hi[4 * k], pa_hi[4 * k + 1], pa_hi[4 * k + 2], pa_hi[4 * k + 3]};
+        const uint32_t al[4] = {pa_lo[4 * k], pa_lo[4 * k + 1], pa_lo[4 * k + 2], pa_lo[4 * k + 3]};
+        wgmma_rs_bf16_mnb128(o, al, b_hi + ko, 1u);  // P_lo * V_hi
+        wgmma_rs_bf16_mnb128(o, ah, b_lo + ko, 1u);  // P_hi * V_lo
+        wgmma_rs_bf16_mnb128(o, ah, b_hi + ko, 1u);  // P_hi * V_hi
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+    }
+    if (lane == 0) mbar_arrive(v_empty(s));
+    if (++s == kStages) { s = 0; ph ^= 1u; }
+  }
+
+  // normalise, store split-bf16. Output row: in place (batch-strided), or scattered through the row map — the
+  // attention then undoes the zone / window regrouping itself (attention_base.py:100-103, attention_flow.py:165-168)
+  // and the output projection is a plain row-major GEMM over the real tokens only.
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float inv = 1.f / quad_sum(l_run[h]);
+    const int qrow = qt * 128 + wg * 64 + (warp & 3) * 16 + g + 8 * h;
     bool row_ok = qrow < p.Lq;
     long long orow = batch * p.out_batch_stride + static_cast<long long>(qrow) * p.out_ld;
     if (p.out_rowmap && row_ok) {
@@ -355,37 +264,17 @@ __global__ void __launch_bounds__(256, 1) flash_kernel(const __grid_constant__ F
       row_ok = m >= 0;
       orow = static_cast<long long>(m) * p.out_ld;
     }
-    __nv_bfloat16* oh = p.out_hi + orow + head * 128;
-    __nv_bfloat16* ol = oh + p.out_plane;
+    if (!row_ok) continue;
+    __nv_bfloat16* oh = p.out_hi + orow + head * 128 + 2 * qc;
 #pragma unroll
-    for (int c0 = 0; c0 < 128; c0 += 32) {
-      uint32_t raw[32];
-      tmem_ld32(lane_base + kTmO + c0, raw);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t hw[4], lw[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            split_bf16x2(__uint_as_float(raw[c * 8 + 2 * q]) * inv, __uint_as_float(raw[c * 8 + 2 * q + 1]) * inv, hw[q],
-                         lw[q]);
-          reinterpret_cast<uint4*>(oh + c0)[c] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-          reinterpret_cast<uint4*>(ol + c0)[c] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-        }
-      }
+    for (int jj = 0; jj < 16; ++jj) {
+      uint32_t hw, lw;
+      split_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, hw, lw);
+      *reinterpret_cast<uint32_t*>(oh + 8 * jj) = hw;
+      *reinterpret_cast<uint32_t*>(oh + p.out_plane + 8 * jj) = lw;
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
-
-static long long* g_flash_trace = nullptr;  // debugging aid, see fgt_debug_flash_trace()
 
 int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   FGT_REQUIRE(d.head_dim == 128, FGT_ERR_ARG, "attention: head_dim=%d (only 128 supported)", d.head_dim);
@@ -440,7 +329,6 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   p.out_batch_stride = d.out_batch_stride;
   p.out_ld = d.out_ld;
   p.out_rowmap = d.out_rowmap;
-  p.trace = g_flash_trace;
   FGT_REQUIRE((reinterpret_cast<uintptr_t>(d.out_hi) & 15) == 0, FGT_ERR_ARG, "attention: output misaligned");
 
   static bool attr_set = false;
@@ -449,7 +337,7 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid((d.Lq + 127) / 128, d.heads, d.batches);
-  launch_k(flash_kernel, dim3(grid), dim3(256), kFlashSmem, stream, p);
+  launch_k(flash_kernel, dim3(grid), dim3(kFlashThreads), kFlashSmem, stream, p);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }
@@ -459,11 +347,4 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
 extern "C" int fgt_attention(const FgtAttnDesc* desc, fgt_stream_t stream) {
   if (!desc) return fgt::set_err(FGT_ERR_ARG, "fgt_attention: null desc");
   return fgt::attention_launch(*desc, reinterpret_cast<cudaStream_t>(stream));
-}
-
-// Debug aid (not part of the data path): when given a device buffer of 3*64*8 int64, the next
-// fgt_attention launches record clock64 timestamps of CTA (0,0,0) per role / key tile into it.
-extern "C" int fgt_debug_flash_trace(long long* device_buf) {
-  fgt::g_flash_trace = device_buf;
-  return FGT_OK;
 }

@@ -1,17 +1,19 @@
-// Persistent, warp-specialised implicit-GEMM engine for sm_100a.
+// Persistent, warp-specialised implicit-GEMM engine for sm_90a.
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warp 1      : MMA issuer     (one elected thread, tcgen05.mma kind::f16, 3-term split-bf16)
-//   warps 2..5  : epilogue       (tcgen05.ld TMEM -> regs -> bias/act/aux -> 128B-swizzled smem panels ->
-//                                  TMA tile store; rows scattered through a rowmap, transposed / NCHW outputs and
-//                                  launches with two outputs store straight from registers instead)
+//   warps 0..7 : two consumer warpgroups (wgmma.mma_async, 3-term split-bf16 or 1-term fp16, fp32 accumulators in
+//                registers); warpgroup w owns rows [64 w, 64 w + 64) of the 128-row tile and runs the epilogue of
+//                those rows straight from its registers (bias / activation / aux operand, rows scattered through a
+//                rowmap, transposed / NCHW outputs, launches with two outputs)
+//   warp 8     : TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
 //
-// One CTA per SM loops over output tiles (128 output positions x bn channels). The fp32
-// accumulator lives in TMEM in 2..8 buffers (512 columns / tile width) so the epilogue of tile i overlaps the
-// main loops of the following tiles — short-K layers (one or two K iterations per tile) are otherwise bound by
-// the load -> MMA -> epilogue latency chain of a tile, not by bandwidth. Used for every Linear/Conv on the path (see include/fgt_b200.h).
+// One CTA per SM loops over output tiles (128 output positions x bn channels); the producer runs ahead through the
+// stage ring while the consumers finish the previous tile's epilogue. Used for every Linear/Conv on the path (see
+// include/fgt_b200.h).
 #include "common.h"
 #include "ptx.cuh"
+
+#include <mutex>
+#include <unordered_set>
 
 namespace fgt {
 
@@ -19,6 +21,8 @@ constexpr int kMaxAMaps = 18;  // 2 segments x up to 9 stride phases
 constexpr int kMaxTaps = 64;   // up to 7x7 (=49) taps
 constexpr int kBK = 64;        // K elements per pipeline stage (128 bytes of bf16)
 constexpr int kAPlaneBytes = 128 * 128;  // one A plane per stage: 128 rows x 128 B
+constexpr int kGemmThreads = 288;        // 2 consumer warpgroups + 1 producer warp
+constexpr int kProducerWarp = 8;
 
 struct TapDesc {
   int8_t phase;  // which stride-phase view
@@ -34,26 +38,18 @@ struct SegDesc {
 struct GemmParams {
   CUtensorMap a_maps[kMaxAMaps];
   CUtensorMap b_map;
-  CUtensorMap out_map;  // epilogue TMA store: (C, X, Y, Z, plane) bf16 for a split output, (C, X, Y, Z) fp32
-  CUtensorMap aux_map;  // epilogue TMA load of the fp32 aux operand (residual / gate), same geometry as an fp32 out_map
   TapDesc taps[kMaxTaps];
   SegDesc segs[2];
   int num_taps, num_segs, num_maps, k_iters;
   int tiles_x, tiles_y, tiles_z, n_tiles, total_tiles;
-  int bn, bn_p2, stages;
-  int n_acc;    // accumulator buffers in TMEM (power of two, n_acc * bn_p2 <= 512)
-  int planes;   // 2: split-bf16 operands, 3 MMAs per K step; 1: single-plane fp16 operands, 1 MMA per K step
-  int out_half; // the 16-bit output is ONE plane of fp16 (input of a 1-term layer) instead of split-bf16
-  int tma_out;  // epilogue stores through shared memory + TMA (single output, unit channel stride, no rowmap)
-  int aux_tma;    // the aux tile is fetched into the staging panels by TMA (fp32 output launches) instead of per-row loads
-  int stg_slots;  // staging ring of the TMA epilogue: 1, 2 or 4 slots (a slot = the panels of one 64-channel chunk)
-  int stg_slot_bytes;
+  int bn, stages;
   int box_w, box_h, a_rows;
   int N, cout_per_group;
   int out_w, out_h;
   int linear;  // 1: rows on x only (rowmap / lin_batch addressing)
   int lin_batch;
-  int vec_ok;  // 16-byte vector stores allowed
+  int vec_ok;   // channel pairs stored (and aux pairs loaded) as one 8-byte / 4-byte access
+  int aux_vec;  // aux pairs loaded as one access (debugging aid: 0 = per-element loads)
   long long os_z, os_y, os_x, os_c;
   const int* rowmap;
   float* out_f32;
@@ -65,17 +61,8 @@ struct GemmParams {
   const float* bias;
   int act;
   float alpha;
+  int out_half;  // the 16-bit output is ONE plane of fp16 (input of a 1-term layer) instead of split-bf16
 };
-
-__device__ __forceinline__ float apply_act(float v, int act) {
-  switch (act) {
-    case FGT_ACT_LEAKY02: return v > 0.f ? v : 0.2f * v;
-    case FGT_ACT_RELU: return fmaxf(v, 0.f);
-    case FGT_ACT_SIGMOID: return 1.f / (1.f + expf(-v));
-    case FGT_ACT_TANH: return tanhf(v);
-    default: return v;
-  }
-}
 
 // Epilogue parameters hoisted into registers once per CTA.
 struct EpiArgs {
@@ -85,318 +72,161 @@ struct EpiArgs {
   const float* aux2;
   long long out_plane, os_c;
   float alpha;
-  int act, aux_mode, vec_ok, N, out_half;
+  int act, aux_mode, vec_ok, aux_vec, N, out_half;
 };
 
-// kExt = 1 adds the rarely used epilogue modes (pre-activation add, add+ReLU, GRU update, slope-0.01
-// LeakyReLU); keeping them out of the common instantiation keeps it at ~150 registers with no spills.
-template <int NC, int kExt>
-__device__ __forceinline__ void epi_chunk(const EpiArgs& e, const uint32_t (&raw)[NC], const float* sb, long long off,
-                                          int col0) {
-  float v[NC];
-#pragma unroll
-  for (int q = 0; q < NC / 4; ++q) {
-    const float4 b = *reinterpret_cast<const float4*>(sb + 4 * q);
-    v[4 * q] = fmaf(__uint_as_float(raw[4 * q]), e.alpha, b.x);
-    v[4 * q + 1] = fmaf(__uint_as_float(raw[4 * q + 1]), e.alpha, b.y);
-    v[4 * q + 2] = fmaf(__uint_as_float(raw[4 * q + 2]), e.alpha, b.z);
-    v[4 * q + 3] = fmaf(__uint_as_float(raw[4 * q + 3]), e.alpha, b.w);
+__device__ __forceinline__ float act_one(float v, int act) {
+  switch (act) {
+    case FGT_ACT_LEAKY02: return v > 0.f ? v : 0.2f * v;
+    case FGT_ACT_LEAKY001: return v > 0.f ? v : 0.01f * v;
+    case FGT_ACT_RELU: return fmaxf(v, 0.f);
+    case FGT_ACT_SIGMOID: return 1.f / (1.f + expf(-v));
+    case FGT_ACT_TANH: return tanhf(v);
+    default: return v;
   }
-  const bool vec = e.vec_ok && col0 + NC <= e.N;
+}
+
+__device__ __forceinline__ void load_pair(const float* src, long long o0, long long o1, bool two, bool vec, float& x0,
+                                          float& x1) {
+  if (vec) {
+    const float2 a = __ldg(reinterpret_cast<const float2*>(src + o0));
+    x0 = a.x;
+    x1 = a.y;
+  } else {
+    x0 = __ldg(src + o0);
+    x1 = two ? __ldg(src + o1) : 0.f;
+  }
+}
+
+// Output channels (col, col + 1) of one output row at element offset `off`: bias + alpha * acc, activation, aux
+// operand, stores. `two`: col + 1 < N. kExt = 1 adds the rarely used modes (pre-activation add, add+ReLU, GRU
+// updates, slope-0.01 LeakyReLU); keeping them out of the common instantiation keeps its register count down.
+template <int kExt>
+__device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, long long off, int col, bool two) {
+  const bool vec = e.vec_ok && two;  // vec_ok implies a unit channel stride and even element offsets
+  const long long o0 = off + static_cast<long long>(col) * e.os_c;
+  const long long o1 = o0 + e.os_c;
+  const bool avec = vec && e.aux_vec;
+  float a0 = 0.f, a1 = 0.f;
   if (kExt && e.aux_mode == FGT_AUX_ADD_PRE) {  // residual added BEFORE the activation (LAFC edge head)
-    if (vec) {
-      const float4* ap = reinterpret_cast<const float4*>(e.aux + off + col0);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) {
-        const float4 a = __ldg(ap + q);
-        v[4 * q] += a.x; v[4 * q + 1] += a.y; v[4 * q + 2] += a.z; v[4 * q + 3] += a.w;
-      }
-    } else {
-      for (int j = 0; j < NC; ++j)
-        if (col0 + j < e.N) v[j] += __ldg(e.aux + off + static_cast<long long>(col0 + j) * e.os_c);
-    }
+    load_pair(e.aux, o0, o1, two, avec, a0, a1);
+    v0 += a0;
+    v1 += a1;
   }
-  if (e.act == FGT_ACT_LEAKY02) {
-#pragma unroll
-    for (int j = 0; j < NC; ++j) v[j] = v[j] > 0.f ? v[j] : 0.2f * v[j];
-  } else if (kExt && e.act == FGT_ACT_LEAKY001) {
-#pragma unroll
-    for (int j = 0; j < NC; ++j) v[j] = v[j] > 0.f ? v[j] : 0.01f * v[j];
-  } else if (e.act == FGT_ACT_RELU) {
-#pragma unroll
-    for (int j = 0; j < NC; ++j) v[j] = fmaxf(v[j], 0.f);
-  } else if (e.act == FGT_ACT_SIGMOID) {
-#pragma unroll
-    for (int j = 0; j < NC; ++j) v[j] = 1.f / (1.f + expf(-v[j]));
-  } else if (e.act == FGT_ACT_TANH) {
-#pragma unroll
-    for (int j = 0; j < NC; ++j) v[j] = tanhf(v[j]);
+  if (kExt) {
+    v0 = act_one(v0, e.act);
+    v1 = act_one(v1, e.act);
+  } else if (e.act == FGT_ACT_LEAKY02) {
+    v0 = v0 > 0.f ? v0 : 0.2f * v0;
+    v1 = v1 > 0.f ? v1 : 0.2f * v1;
+  } else if (e.act != FGT_ACT_NONE) {
+    v0 = act_one(v0, e.act);
+    v1 = act_one(v1, e.act);
   }
   if (kExt && e.aux_mode == FGT_AUX_GRU_ZR) {  // fused z | r gates: two C-channel outputs (host guarantees vec)
     const int half = e.N >> 1;
-    if (col0 < half) {
-      float4* op = reinterpret_cast<float4*>(e.out_f32 + off + col0);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) op[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    if (col < half) {
+      *reinterpret_cast<float2*>(e.out_f32 + o0) = make_float2(v0, v1);
     } else {
-      const long long o = off + (col0 - half);
-      const float4* ap = reinterpret_cast<const float4*>(e.aux + o);
-      uint4* hp = reinterpret_cast<uint4*>(e.out_hi + o);
-      uint4* lp = reinterpret_cast<uint4*>(e.out_hi + e.out_plane + o);
-#pragma unroll
-      for (int q = 0; q < NC / 8; ++q) {
-        const float4 a0 = __ldg(ap + 2 * q), a1 = __ldg(ap + 2 * q + 1);
-        uint32_t hw[4], lw[4];
-        split_bf16x2(v[8 * q] * a0.x, v[8 * q + 1] * a0.y, hw[0], lw[0]);
-        split_bf16x2(v[8 * q + 2] * a0.z, v[8 * q + 3] * a0.w, hw[1], lw[1]);
-        split_bf16x2(v[8 * q + 4] * a1.x, v[8 * q + 5] * a1.y, hw[2], lw[2]);
-        split_bf16x2(v[8 * q + 6] * a1.z, v[8 * q + 7] * a1.w, hw[3], lw[3]);
-        hp[q] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-        lp[q] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-      }
+      const long long o = off + (col - half);
+      load_pair(e.aux, o, o + 1, true, e.aux_vec != 0, a0, a1);
+      uint32_t hw, lw;
+      split_bf16x2(v0 * a0, v1 * a1, hw, lw);
+      *reinterpret_cast<uint32_t*>(e.out_hi + o) = hw;
+      *reinterpret_cast<uint32_t*>(e.out_hi + e.out_plane + o) = lw;
     }
     return;
   }
+  if (e.aux_mode == FGT_AUX_ADD) {
+    load_pair(e.aux, o0, o1, two, avec, a0, a1);
+    v0 += a0;
+    v1 += a1;
+  } else if (e.aux_mode == FGT_AUX_MUL) {
+    load_pair(e.aux, o0, o1, two, avec, a0, a1);
+    v0 *= a0;
+    v1 *= a1;
+  } else if (kExt && e.aux_mode == FGT_AUX_ADD_RELU) {
+    load_pair(e.aux, o0, o1, two, avec, a0, a1);
+    v0 = fmaxf(v0 + a0, 0.f);
+    v1 = fmaxf(v1 + a1, 0.f);
+  } else if (kExt && e.aux_mode == FGT_AUX_GRU) {  // h' = (1 - z) * h + z * q   (aux = h, aux2 = z, v = q)
+    float z0, z1;
+    load_pair(e.aux, o0, o1, two, avec, a0, a1);
+    load_pair(e.aux2, o0, o1, two, avec, z0, z1);
+    v0 = (1.f - z0) * a0 + z0 * v0;
+    v1 = (1.f - z1) * a1 + z1 * v1;
+  }
   if (vec) {
-    const long long o = off + col0;
-    if (e.aux_mode == FGT_AUX_ADD) {
-      const float4* ap = reinterpret_cast<const float4*>(e.aux + o);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) {
-        const float4 a = __ldg(ap + q);
-        v[4 * q] += a.x; v[4 * q + 1] += a.y; v[4 * q + 2] += a.z; v[4 * q + 3] += a.w;
-      }
-    } else if (e.aux_mode == FGT_AUX_MUL) {
-      const float4* ap = reinterpret_cast<const float4*>(e.aux + o);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) {
-        const float4 a = __ldg(ap + q);
-        v[4 * q] *= a.x; v[4 * q + 1] *= a.y; v[4 * q + 2] *= a.z; v[4 * q + 3] *= a.w;
-      }
-    } else if (kExt && e.aux_mode == FGT_AUX_ADD_RELU) {
-      const float4* ap = reinterpret_cast<const float4*>(e.aux + o);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) {
-        const float4 a = __ldg(ap + q);
-        v[4 * q] = fmaxf(v[4 * q] + a.x, 0.f); v[4 * q + 1] = fmaxf(v[4 * q + 1] + a.y, 0.f);
-        v[4 * q + 2] = fmaxf(v[4 * q + 2] + a.z, 0.f); v[4 * q + 3] = fmaxf(v[4 * q + 3] + a.w, 0.f);
-      }
-    } else if (kExt && e.aux_mode == FGT_AUX_GRU) {  // h' = (1 - z) * h + z * q   (aux = h, aux2 = z, v = q)
-      const float4* hp4 = reinterpret_cast<const float4*>(e.aux + o);
-      const float4* zp4 = reinterpret_cast<const float4*>(e.aux2 + o);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) {
-        const float4 h = __ldg(hp4 + q);
-        const float4 z = __ldg(zp4 + q);
-        v[4 * q] = (1.f - z.x) * h.x + z.x * v[4 * q];
-        v[4 * q + 1] = (1.f - z.y) * h.y + z.y * v[4 * q + 1];
-        v[4 * q + 2] = (1.f - z.z) * h.z + z.z * v[4 * q + 2];
-        v[4 * q + 3] = (1.f - z.w) * h.w + z.w * v[4 * q + 3];
-      }
-    }
-    if (e.out_f32) {
-      float4* op = reinterpret_cast<float4*>(e.out_f32 + o);
-#pragma unroll
-      for (int q = 0; q < NC / 4; ++q) op[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    }
+    if (e.out_f32) *reinterpret_cast<float2*>(e.out_f32 + o0) = make_float2(v0, v1);
     if (e.out_hi && e.out_half) {
-      uint4* hp = reinterpret_cast<uint4*>(e.out_hi + o);
-#pragma unroll
-      for (int q = 0; q < NC / 8; ++q)
-        hp[q] = make_uint4(pack_f16x2(v[8 * q], v[8 * q + 1]), pack_f16x2(v[8 * q + 2], v[8 * q + 3]),
-                           pack_f16x2(v[8 * q + 4], v[8 * q + 5]), pack_f16x2(v[8 * q + 6], v[8 * q + 7]));
+      *reinterpret_cast<uint32_t*>(e.out_hi + o0) = pack_f16x2(v0, v1);
     } else if (e.out_hi) {
-      uint4* hp = reinterpret_cast<uint4*>(e.out_hi + o);
-      uint4* lp = reinterpret_cast<uint4*>(e.out_hi + e.out_plane + o);
-#pragma unroll
-      for (int q = 0; q < NC / 8; ++q) {
-        uint32_t hw[4], lw[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) split_bf16x2(v[8 * q + 2 * t], v[8 * q + 2 * t + 1], hw[t], lw[t]);
-        hp[q] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-        lp[q] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-      }
+      uint32_t hw, lw;
+      split_bf16x2(v0, v1, hw, lw);
+      *reinterpret_cast<uint32_t*>(e.out_hi + o0) = hw;
+      *reinterpret_cast<uint32_t*>(e.out_hi + e.out_plane + o0) = lw;
     }
   } else {
     // generic path: strided channel stores (transposed / NCHW outputs) and N tails
-    for (int j = 0; j < NC; ++j) {
-      if (col0 + j < e.N) {
-        const long long o = off + static_cast<long long>(col0 + j) * e.os_c;
-        float x = v[j];
-        if (e.aux_mode == FGT_AUX_ADD) x += __ldg(e.aux + o);
-        else if (e.aux_mode == FGT_AUX_MUL) x *= __ldg(e.aux + o);
-        else if (kExt && e.aux_mode == FGT_AUX_ADD_RELU) x = fmaxf(x + __ldg(e.aux + o), 0.f);
-        else if (kExt && e.aux_mode == FGT_AUX_GRU) {
-          const float z = __ldg(e.aux2 + o);
-          x = (1.f - z) * __ldg(e.aux + o) + z * x;
-        }
-        if (e.out_f32) e.out_f32[o] = x;
-        if (e.out_hi && e.out_half) {
-          reinterpret_cast<__half*>(e.out_hi)[o] = __float2half_rn(x);
-        } else if (e.out_hi) {
-          __nv_bfloat16 h, l;
-          split_bf16(x, h, l);
-          e.out_hi[o] = h;
-          e.out_hi[e.out_plane + o] = l;
-        }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      if (q == 1 && !two) break;
+      const long long o = q ? o1 : o0;
+      const float x = q ? v1 : v0;
+      if (e.out_f32) e.out_f32[o] = x;
+      if (e.out_hi && e.out_half) {
+        reinterpret_cast<__half*>(e.out_hi)[o] = __float2half_rn(x);
+      } else if (e.out_hi) {
+        __nv_bfloat16 h, l;
+        split_bf16(x, h, l);
+        e.out_hi[o] = h;
+        e.out_hi[e.out_plane + o] = l;
       }
     }
   }
 }
 
-// Register-only part of the epilogue for the TMA-store path (unit channel stride guaranteed): bias, activation and
-// the aux operand for 32 consecutive channels of one output row; channels >= N (N tail) skip their aux loads.
-template <int kExt>
-__device__ __forceinline__ void epi_math(const EpiArgs& e, const uint32_t (&raw)[32], const float* sb, long long off,
-                                         int col0, bool valid, float (&v)[32], uint32_t aux_smem = 0u, uint32_t sw = 0u) {
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    const float4 b = *reinterpret_cast<const float4*>(sb + 4 * q);
-    v[4 * q] = fmaf(__uint_as_float(raw[4 * q]), e.alpha, b.x);
-    v[4 * q + 1] = fmaf(__uint_as_float(raw[4 * q + 1]), e.alpha, b.y);
-    v[4 * q + 2] = fmaf(__uint_as_float(raw[4 * q + 2]), e.alpha, b.z);
-    v[4 * q + 3] = fmaf(__uint_as_float(raw[4 * q + 3]), e.alpha, b.w);
-  }
-  const long long o = off + col0;
-  const bool aux_ok = valid && e.aux_mode != FGT_AUX_NONE;
-  float4 a[8];
-  if (aux_ok && aux_smem) {  // the tile's aux values were fetched by TMA into this thread's swizzled panel row
-#pragma unroll
-    for (int q = 0; q < 8; ++q) a[q] = ld_shared_f4(aux_smem + ((static_cast<uint32_t>(q) ^ sw) << 4));
-  } else if (aux_ok) {
-    const float4* ap = reinterpret_cast<const float4*>(e.aux + o);
-#pragma unroll
-    for (int q = 0; q < 8; ++q)
-      a[q] = (col0 + 4 * q + 4 <= e.N) ? __ldg(ap + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-  } else {
-#pragma unroll
-    for (int q = 0; q < 8; ++q) a[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (kExt && e.aux_mode == FGT_AUX_ADD_PRE) {
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      v[4 * q] += a[q].x; v[4 * q + 1] += a[q].y; v[4 * q + 2] += a[q].z; v[4 * q + 3] += a[q].w;
-    }
-  }
-  if (e.act == FGT_ACT_LEAKY02) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : 0.2f * v[j];
-  } else if (kExt && e.act == FGT_ACT_LEAKY001) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : 0.01f * v[j];
-  } else if (e.act == FGT_ACT_RELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-  } else if (e.act == FGT_ACT_SIGMOID) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 1.f / (1.f + expf(-v[j]));
-  } else if (e.act == FGT_ACT_TANH) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = tanhf(v[j]);
-  }
-  if (e.aux_mode == FGT_AUX_ADD) {
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      v[4 * q] += a[q].x; v[4 * q + 1] += a[q].y; v[4 * q + 2] += a[q].z; v[4 * q + 3] += a[q].w;
-    }
-  } else if (e.aux_mode == FGT_AUX_MUL) {
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      v[4 * q] *= a[q].x; v[4 * q + 1] *= a[q].y; v[4 * q + 2] *= a[q].z; v[4 * q + 3] *= a[q].w;
-    }
-  } else if (kExt && e.aux_mode == FGT_AUX_ADD_RELU) {
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      v[4 * q] = fmaxf(v[4 * q] + a[q].x, 0.f); v[4 * q + 1] = fmaxf(v[4 * q + 1] + a[q].y, 0.f);
-      v[4 * q + 2] = fmaxf(v[4 * q + 2] + a[q].z, 0.f); v[4 * q + 3] = fmaxf(v[4 * q + 3] + a[q].w, 0.f);
-    }
-  } else if (kExt && e.aux_mode == FGT_AUX_GRU) {  // h' = (1 - z) * h + z * q   (aux = h, aux2 = z, v = q)
-    if (valid) {
-      const float4* zp = reinterpret_cast<const float4*>(e.aux2 + o);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 z = (col0 + 4 * q + 4 <= e.N) ? __ldg(zp + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-        v[4 * q] = (1.f - z.x) * a[q].x + z.x * v[4 * q];
-        v[4 * q + 1] = (1.f - z.y) * a[q].y + z.y * v[4 * q + 1];
-        v[4 * q + 2] = (1.f - z.z) * a[q].z + z.z * v[4 * q + 2];
-        v[4 * q + 3] = (1.f - z.w) * a[q].w + z.w * v[4 * q + 3];
-      }
-    }
-  }
-}
-
-// Debugging aid (fgt_debug_gemm_trace): clock64 timeline of one CTA, [role 0 producer | 1 MMA | 2 epilogue][local tile
-// 0..63][4 slots]. Only the kTrace instantiation reads these; the production instantiations are unchanged by it.
-__device__ long long* g_gemm_trace = nullptr;
-__device__ int g_gemm_trace_cta = 0;
-
-template <int kExt, int kTrace = 0>
-__global__ void __launch_bounds__(192, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  long long* trace = nullptr;
-  if (kTrace) trace = (static_cast<int>(blockIdx.x) == g_gemm_trace_cta) ? g_gemm_trace : nullptr;
-#define FGT_GTRACE(role, lt, slot) \
-  if (kTrace && trace && (lt) < 64) trace[((role) * 64 + (lt)) * 4 + (slot)] = clock64()
+// BN: the wgmma N of the launch (>= p.bn; the B tile rows beyond p.bn are never written and their columns are
+// dropped). kF16: single-plane fp16 operands (one MMA per K step) instead of split-bf16 (three).
+template <int BN, bool kF16, int kExt>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atoms.
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  const uint32_t b_plane_bytes = static_cast<uint32_t>(p.bn) * 128u;
-  const uint32_t nplanes = static_cast<uint32_t>(p.planes);
-  const uint32_t stage_bytes = nplanes * (kAPlaneBytes + b_plane_bytes);
-  const uint32_t stg_ring = smem_base + static_cast<uint32_t>(p.stages) * stage_bytes;  // output panels (ring of chunks)
-  const uint32_t bar_base = stg_ring + static_cast<uint32_t>(p.tma_out ? p.stg_slots * p.stg_slot_bytes : 0);
-  // barrier layout: full[stages], empty[stages], acc_full[n_acc], acc_empty[n_acc], tmem slot
-  const int n_acc = p.n_acc;
-  const int acc_shift = 31 - __clz(n_acc);
+  constexpr uint32_t nplanes = kF16 ? 1u : 2u;
+  constexpr uint32_t b_plane_bytes = static_cast<uint32_t>(BN) * 128u;
+  constexpr uint32_t stage_bytes = nplanes * (kAPlaneBytes + b_plane_bytes);
+  const uint32_t bar_base = smem_base + static_cast<uint32_t>(p.stages) * stage_bytes;
+  // barrier layout: full[stages], empty[stages]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  auto accf_bar = [&](int b) { return bar_base + 8u * (2 * p.stages + b); };
-  auto acce_bar = [&](int b) { return bar_base + 8u * (2 * p.stages + n_acc + b); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * p.stages + 2 * n_acc);
-  // per-tile bias slice staged in smem (2 buffers x 256 floats), after the 256-byte barrier block
-  float* sbias_base = reinterpret_cast<float*>(smem_raw + (bar_base - smem_u32(smem_raw)) + 256);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < n_acc; ++b) {
-      mbar_init(accf_bar(b), 1);
-      mbar_init(acce_bar(b), 4);
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
     }
     fence_mbar_init();
     for (int i = 0; i < p.num_maps; ++i) tma_prefetch_desc(&p.a_maps[i]);
     tma_prefetch_desc(&p.b_map);
-    if (p.tma_out) tma_prefetch_desc(&p.out_map);
-    if (p.aux_tma) {
-      tma_prefetch_desc(&p.aux_map);
-      mbar_init(bar_base + 8u * 30, 1);  // aux tile landed (one load in flight at a time)
-      fence_mbar_init();
-    }
   }
-  if (warp == 1) tmem_alloc(tmem_slot, static_cast<uint32_t>(n_acc * p.bn_p2));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem_base) : "r"(tmem_slot));
   // PDL: the prologue above overlapped the previous kernel's tail; nothing before this line touches global data
   pdl_launch_dependents();
   pdl_wait();
 
   const int tiles_per_z = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------------------------------------ TMA producer
     if (elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      const uint32_t tx_bytes = nplanes * (static_cast<uint32_t>(p.a_rows) * 128u + b_plane_bytes);
-      int plt = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++plt) {
+      const uint32_t tx_bytes = nplanes * (static_cast<uint32_t>(p.a_rows) + static_cast<uint32_t>(p.bn)) * 128u;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int nt = tile % p.n_tiles;
         const int mt = tile / p.n_tiles;
         const int z = mt / tiles_per_z;
@@ -407,7 +237,6 @@ __global__ void __launch_bounds__(192, 1) gemm_tc_kernel(const __grid_constant__
         const int n0 = nt * p.bn;
         const int group = n0 / p.cout_per_group;
         int kidx = 0;
-        FGT_GTRACE(0, plt, 0);
         for (int t = 0; t < p.num_taps; ++t) {
           const TapDesc tap = p.taps[t];
           for (int sgi = 0; sgi < p.num_segs; ++sgi) {
@@ -415,8 +244,7 @@ __global__ void __launch_bounds__(192, 1) gemm_tc_kernel(const __grid_constant__
             const CUtensorMap* amap = &p.a_maps[sg.map_base + tap.phase];
             const int c0 = sg.c_base + group * sg.c_per_group;
             for (int ch = 0; ch < sg.chunks; ++ch, ++kidx) {
-              mbar_wait(empty_bar(stage), phase ^ 1u);
-              if (kTrace && kidx == 0) { FGT_GTRACE(0, plt, 1); }
+              mbar_wait_quiet(empty_bar(stage), phase ^ 1u);
               const uint32_t sa = smem_base + stage * stage_bytes;
               const uint32_t sb = sa + nplanes * kAPlaneBytes;
               const uint32_t fb = full_bar(stage);
@@ -432,72 +260,25 @@ __global__ void __launch_bounds__(192, 1) gemm_tc_kernel(const __grid_constant__
             }
           }
         }
-        FGT_GTRACE(0, plt, 2);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t idesc = p.planes == 1 ? umma_idesc_f16(128, p.bn) : umma_idesc_bf16(128, p.bn);
-      int lt = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++lt) {
-        const int buf = lt & (n_acc - 1);
-        const uint32_t aph = (lt >> acc_shift) & 1u;
-        FGT_GTRACE(1, lt, 0);
-        mbar_wait(acce_bar(buf), aph ^ 1u);
-        tc_fence_after();
-        FGT_GTRACE(1, lt, 1);
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(buf * p.bn_p2);
-        for (int it = 0; it < p.k_iters; ++it) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          if (kTrace && it == 0) { FGT_GTRACE(1, lt, 2); }
-          const uint32_t sa = smem_base + stage * stage_bytes;
-          const uint32_t sb = sa + nplanes * kAPlaneBytes;
-          const uint64_t a_hi = umma_desc_sw128(sa);
-          const uint64_t b_hi = umma_desc_sw128(sb);
-          if (nplanes == 2) {
-            const uint64_t a_lo = umma_desc_sw128(sa + kAPlaneBytes);
-            const uint64_t b_lo = umma_desc_sw128(sb + b_plane_bytes);
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) {
-              const uint64_t ko = static_cast<uint64_t>(k * 2);  // 32 bytes >> 4
-              umma_bf16(d_tmem, a_lo + ko, b_hi + ko, idesc, (it | k) != 0);
-              umma_bf16(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-              umma_bf16(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) {
-              const uint64_t ko = static_cast<uint64_t>(k * 2);
-              umma_bf16(d_tmem, a_hi + ko, b_hi + ko, idesc, (it | k) != 0);
-            }
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(accf_bar(buf));
-        FGT_GTRACE(1, lt, 3);
       }
     }
     __syncwarp();
   } else {
-    // ------------------------------------------------------------ epilogue (warps 2..5)
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may read
-    const int r = quarter * 32 + lane;
+    // ------------------------------------------------------------ consumers: MMA + epilogue (warps 0..7)
+    const int wg = warp >> 2;
+    // Both warpgroups issue their MMAs unconditionally, also when all 64 rows of one lie beyond the tile's a_rows (boxes
+    // of <= 64 positions): a branch around wgmma makes ptxas serialise every MMA of the kernel. Rows >= a_rows read
+    // stale shared memory and are never stored.
+    const uint32_t a_off = static_cast<uint32_t>(wg) * 64u * 128u;
     EpiArgs ep;
     ep.out_f32 = p.out_f32; ep.out_hi = p.out_hi; ep.aux = p.aux; ep.aux2 = p.aux2; ep.out_plane = p.out_plane; ep.os_c = p.os_c;
-    ep.alpha = p.alpha; ep.act = p.act; ep.aux_mode = p.aux_mode; ep.vec_ok = p.vec_ok; ep.N = p.N;
+    ep.alpha = p.alpha; ep.act = p.act; ep.aux_mode = p.aux_mode; ep.vec_ok = p.vec_ok; ep.aux_vec = p.aux_vec; ep.N = p.N;
     ep.out_half = p.out_half;
-    const int e_bn = p.bn, e_bn_p2 = p.bn_p2, e_N = p.N;
-    int lt = 0;
-    uint32_t stg_it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++lt) {
-      const int buf = lt & (n_acc - 1);
-      const uint32_t aph = (lt >> acc_shift) & 1u;
+    const int qc = lane & 3;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const int nt = tile % p.n_tiles;
       const int mt = tile / p.n_tiles;
       const int z = mt / tiles_per_z;
@@ -506,163 +287,124 @@ __global__ void __launch_bounds__(192, 1) gemm_tc_kernel(const __grid_constant__
       const int tx = rem - ty * p.tiles_x;
       const int n0 = nt * p.bn;
 
-      // output position of this thread's accumulator row
-      bool valid = r < p.a_rows;
-      long long off = 0;
-      if (p.linear) {
-        int row = tx * p.box_w + r;
-        valid = valid && row < p.out_w;
-        if (valid && p.rowmap) {
-          row = p.rowmap[row];
-          valid = row >= 0;
-        }
-        if (valid) {
-          if (p.lin_batch > 0) {
-            const int zb = row / p.lin_batch;
-            off = zb * p.os_z + static_cast<long long>(row - zb * p.lin_batch) * p.os_x;
+      int prev = -1;
+      for (int it = 0; it < p.k_iters; ++it) {
+        mbar_wait_quiet(full_bar(stage), phase);
+        {
+          const uint32_t sa = smem_base + stage * stage_bytes;
+          const uint32_t sb = sa + nplanes * kAPlaneBytes;
+          const uint64_t a_hi = gmma_desc_sw128(sa + a_off);
+          const uint64_t b_hi = gmma_desc_sw128(sb);
+          fence_regs(acc);
+          wgmma_fence();
+          if (nplanes == 2) {
+            const uint64_t a_lo = gmma_desc_sw128(sa + kAPlaneBytes + a_off);
+            const uint64_t b_lo = gmma_desc_sw128(sb + b_plane_bytes);
+#pragma unroll
+            for (int k = 0; k < kBK / 16; ++k) {
+              const uint64_t ko = static_cast<uint64_t>(k * 2);  // 32 bytes >> 4
+              wgmma_ss<BN, kF16>(acc, a_lo + ko, b_hi + ko, (it | k) != 0);
+              wgmma_ss<BN, kF16>(acc, a_hi + ko, b_lo + ko, 1u);
+              wgmma_ss<BN, kF16>(acc, a_hi + ko, b_hi + ko, 1u);
+            }
           } else {
-            off = static_cast<long long>(row) * p.os_x;
+#pragma unroll
+            for (int k = 0; k < kBK / 16; ++k) {
+              const uint64_t ko = static_cast<uint64_t>(k * 2);
+              wgmma_ss<BN, kF16>(acc, a_hi + ko, b_hi + ko, (it | k) != 0);
+            }
           }
+          wgmma_commit();
+          // the group of the previous stage has retired once at most this one is pending
+          wgmma_wait<1>();
+          fence_regs(acc);
         }
-      } else {
-        const int ry = r / p.box_w;
-        const int oy = ty * p.box_h + ry;
-        const int ox = tx * p.box_w + (r - ry * p.box_w);
-        valid = valid && oy < p.out_h && ox < p.out_w;
-        off = z * p.os_z + oy * p.os_y + ox * p.os_x;
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
       }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (lane == 0) mbar_arrive(empty_bar(prev));
 
-      // stage this tile's bias slice (zeros beyond N / without bias); 128 epilogue threads cooperate
-      float* sbias = sbias_base + (lt & 1) * p.bn;  // two bn-float slices (sized exactly: 3 stages + staging must fit)
-      for (int c = threadIdx.x - 64; c < p.bn; c += 128)
-        sbias[c] = (p.bias && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f;
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");
-
-      if (kTrace && warp == 2 && lane == 0) { FGT_GTRACE(2, lt, 0); }
-      mbar_wait(accf_bar(buf), aph);
-      tc_fence_after();
-      if (kTrace && warp == 2 && lane == 0) { FGT_GTRACE(2, lt, 1); }
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                             static_cast<uint32_t>(buf * e_bn_p2);
-      if (p.tma_out) {
-        // 64 output channels at a time: each thread writes its row into two 128-row x 128-byte panels laid out
-        // with the 128B swizzle (16-byte chunk j of row r at j ^ (r & 7): conflict-free), then one thread hands
-        // the panels to the TMA engine, which writes full 128-byte lines and clips the M / N tails.
-        const bool issuer = threadIdx.x == 64;
-        const int x0 = tx * p.box_w, y0 = p.linear ? 0 : ty * p.box_h, zz = p.linear ? 0 : z;
-        const uint32_t row_off = static_cast<uint32_t>(r) * 128u;
-        const uint32_t sw = static_cast<uint32_t>(r & 7);
-        const uint32_t aux_bar = bar_base + 8u * 30;
-        for (int c0 = 0; c0 < e_bn && n0 + c0 < e_N; c0 += 64, ++stg_it) {
-          // ring of staging slots: this chunk's slot is free once all but the (slots - 1) most recent store groups
-          // have finished reading shared memory
-          const uint32_t stg_base = stg_ring + static_cast<uint32_t>((stg_it & (p.stg_slots - 1)) * p.stg_slot_bytes);
-          if (issuer) {
-            if (p.stg_slots == 1) bulk_wait_read<0>();
-            else if (p.stg_slots == 2) bulk_wait_read<1>();
-            else bulk_wait_read<3>();
-            if (p.aux_tma) {  // fetch this chunk's aux tile (two 32-column fp32 panels) into the slot it will be stored from
-              const bool two = n0 + c0 + 32 < e_N;
-              mbar_expect_tx(aux_bar, static_cast<uint32_t>(p.a_rows) * 128u * (two ? 2u : 1u));
-              tma_load_4d(stg_base, &p.aux_map, aux_bar, n0 + c0, x0, y0, zz);
-              if (two) tma_load_4d(stg_base + kAPlaneBytes, &p.aux_map, aux_bar, n0 + c0 + 32, x0, y0, zz);
-            }
+      // output positions of this thread's two accumulator rows
+      long long off[2];
+      bool valid[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        bool v = r < p.a_rows;
+        long long o = 0;
+        if (p.linear) {
+          int row = tx * p.box_w + r;
+          v = v && row < p.out_w;
+          if (v && p.rowmap) {
+            row = p.rowmap[row];
+            v = row >= 0;
           }
-          if (p.aux_tma) {
-            mbar_wait(aux_bar, stg_it & 1u);  // implies the slot was free: the loads were issued after the read-wait
-          } else {
-            asm volatile("bar.sync 1, 128;\n" ::: "memory");
-          }
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            uint32_t raw[32];
-            tmem_ld32(t_row + c0 + hf * 32, raw);
-            tmem_ld_wait();
-            float v[32];
-            epi_math<kExt>(ep, raw, sbias + c0 + hf * 32, off, n0 + c0 + hf * 32, valid, v,
-                           p.aux_tma ? stg_base + hf * kAPlaneBytes + row_off : 0u, sw);
-            if (ep.out_hi && ep.out_half) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint32_t a = stg_base + row_off + (((static_cast<uint32_t>(hf * 4 + q)) ^ sw) << 4);
-                st_shared_v4(a, pack_f16x2(v[8 * q], v[8 * q + 1]), pack_f16x2(v[8 * q + 2], v[8 * q + 3]),
-                             pack_f16x2(v[8 * q + 4], v[8 * q + 5]), pack_f16x2(v[8 * q + 6], v[8 * q + 7]));
-              }
-            } else if (ep.out_hi) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint32_t hw[4], lw[4];
-#pragma unroll
-                for (int t = 0; t < 4; ++t) split_bf16x2(v[8 * q + 2 * t], v[8 * q + 2 * t + 1], hw[t], lw[t]);
-                const uint32_t a = stg_base + row_off + (((static_cast<uint32_t>(hf * 4 + q)) ^ sw) << 4);
-                st_shared_v4(a, hw[0], hw[1], hw[2], hw[3]);
-                st_shared_v4(a + kAPlaneBytes, lw[0], lw[1], lw[2], lw[3]);
-              }
+          if (v) {
+            if (p.lin_batch > 0) {
+              const int zb = row / p.lin_batch;
+              o = zb * p.os_z + static_cast<long long>(row - zb * p.lin_batch) * p.os_x;
             } else {
+              o = static_cast<long long>(row) * p.os_x;
+            }
+          }
+        } else {
+          const int ry = r / p.box_w;
+          const int oy = ty * p.box_h + ry;
+          const int ox = tx * p.box_w + (r - ry * p.box_w);
+          v = v && oy < p.out_h && ox < p.out_w;
+          o = z * p.os_z + static_cast<long long>(oy) * p.os_y + static_cast<long long>(ox) * p.os_x;
+        }
+        off[h] = o;
+        valid[h] = v;
+      }
 #pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const uint32_t a = stg_base + hf * kAPlaneBytes + row_off + ((static_cast<uint32_t>(q) ^ sw) << 4);
-                st_shared_v4(a, __float_as_uint(v[4 * q]), __float_as_uint(v[4 * q + 1]), __float_as_uint(v[4 * q + 2]),
-                             __float_as_uint(v[4 * q + 3]));
-              }
-            }
-          }
-          fence_proxy_async_smem();
-          asm volatile("bar.sync 1, 128;\n" ::: "memory");
-          if (issuer) {
-            if (ep.out_hi) {
-              tma_store_5d(&p.out_map, stg_base, n0 + c0, x0, y0, zz, 0);
-              if (!ep.out_half) tma_store_5d(&p.out_map, stg_base + kAPlaneBytes, n0 + c0, x0, y0, zz, 1);
-            } else {
-              tma_store_4d(&p.out_map, stg_base, n0 + c0, x0, y0, zz);
-              if (n0 + c0 + 32 < e_N) tma_store_4d(&p.out_map, stg_base + kAPlaneBytes, n0 + c0 + 32, x0, y0, zz);
-            }
-            bulk_commit();
-          }
-        }
-      } else if ((e_bn & 31) == 0) {
-        for (int c0 = 0; c0 < e_bn; c0 += 32) {
-          uint32_t raw[32];
-          tmem_ld32(t_row + c0, raw);
-          tmem_ld_wait();
-          if (valid && n0 + c0 < e_N) epi_chunk<32, kExt>(ep, raw, sbias + c0, off, n0 + c0);
-        }
-      } else {
-        for (int c0 = 0; c0 < e_bn; c0 += 16) {
-          uint32_t raw[16];
-          tmem_ld16(t_row + c0, raw);
-          tmem_ld_wait();
-          if (valid && n0 + c0 < e_N) epi_chunk<16, kExt>(ep, raw, sbias + c0, off, n0 + c0);
+      for (int j = 0; j < BN / 8; ++j) {
+        const int cl = j * 8 + 2 * qc;
+        const int col = n0 + cl;
+        if (cl < p.bn && col < p.N) {
+          const bool two = col + 1 < p.N;
+          const float b0 = p.bias ? __ldg(p.bias + col) : 0.f;
+          const float b1 = (p.bias && two) ? __ldg(p.bias + col + 1) : 0.f;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (valid[h])
+              epi_pair<kExt>(ep, fmaf(acc[4 * j + 2 * h], ep.alpha, b0), fmaf(acc[4 * j + 2 * h + 1], ep.alpha, b1),
+                             off[h], col, two);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acce_bar(buf));
-      if (kTrace && warp == 2 && lane == 0) { FGT_GTRACE(2, lt, 2); }
     }
   }
-#undef FGT_GTRACE
-
-  if (p.tma_out && threadIdx.x == 64) bulk_wait0();  // all tile stores complete before the CTA's smem goes away
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, static_cast<uint32_t>(n_acc * p.bn_p2));
-  }
-}
-
-static int next_pow2_ge32(int v) {
-  int r = 32;
-  while (r < v) r <<= 1;
-  return r;
 }
 
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
-static bool g_gemm_trace_on = false;  // debugging aid, see fgt_debug_gemm_trace()
-static bool g_gemm_direct_epilogue = false;  // debugging aid: force the register-store epilogue (A/B comparisons)
-static bool g_gemm_direct_aux = false;       // debugging aid: aux operand by per-row global loads even on the TMA path
+static bool g_gemm_direct_epilogue = false;  // debugging aid: per-element stores only (A/B comparisons)
+static bool g_gemm_direct_aux = false;       // debugging aid: aux operand by per-element loads on the paired path
+
+// wgmma N of a launch: the tile width itself up to 128 (every multiple of 16 has an instantiation), 256 above.
+static int mma_n(int bn) { return bn <= 128 ? bn : 256; }
+
+// The extended epilogue (kExt = 1) has no 256-wide instantiation: its 128 accumulator registers per thread plus the
+// extended modes' state do not fit the 224-register budget without spilling; the host rejects bn > 128 for those modes.
+template <bool kF16, int kExt>
+static void* gemm_kernel_for(int n) {
+  switch (n) {
+    case 16: return reinterpret_cast<void*>(gemm_tc_kernel<16, kF16, kExt>);
+    case 32: return reinterpret_cast<void*>(gemm_tc_kernel<32, kF16, kExt>);
+    case 48: return reinterpret_cast<void*>(gemm_tc_kernel<48, kF16, kExt>);
+    case 64: return reinterpret_cast<void*>(gemm_tc_kernel<64, kF16, kExt>);
+    case 80: return reinterpret_cast<void*>(gemm_tc_kernel<80, kF16, kExt>);
+    case 96: return reinterpret_cast<void*>(gemm_tc_kernel<96, kF16, kExt>);
+    case 112: return reinterpret_cast<void*>(gemm_tc_kernel<112, kF16, kExt>);
+    case 128: return reinterpret_cast<void*>(gemm_tc_kernel<128, kF16, kExt>);
+    default:
+      if constexpr (kExt != 0) return nullptr;
+      else return reinterpret_cast<void*>(gemm_tc_kernel<256, kF16, kExt>);
+  }
+}
 
 int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   FGT_REQUIRE(d.num_segs >= 1 && d.num_segs <= 2, FGT_ERR_ARG, "gemm_tc: num_segs=%d", d.num_segs);
@@ -762,8 +504,6 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   p.n_tiles = (d.N + d.bn - 1) / d.bn;
   p.total_tiles = p.tiles_x * p.tiles_y * p.tiles_z * p.n_tiles;
   p.bn = d.bn;
-  p.bn_p2 = next_pow2_ge32(d.bn);
-  p.n_acc = 512 / p.bn_p2 < 8 ? 512 / p.bn_p2 : 8;
   p.box_w = d.box_w;
   p.box_h = d.box_h;
   p.a_rows = a_rows;
@@ -783,98 +523,52 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   p.bias = d.bias;
   p.act = d.act;
   p.alpha = d.alpha;
-  // 16-byte vector path: unit channel stride and every address component a multiple of 8 elements
-  auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  p.vec_ok = (d.os_c == 1 && d.os_x % 8 == 0 && d.os_y % 8 == 0 && d.os_z % 8 == 0 && (d.out_half || d.out_plane % 8 == 0) &&
-              al(d.out_f32) && al(d.out_hi) && al(d.aux) && al(d.aux2))
+  // paired channel accesses (8-byte fp32 / 4-byte 16-bit): unit channel stride and every address component even
+  auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7) == 0; };
+  p.vec_ok = (d.os_c == 1 && d.os_x % 2 == 0 && d.os_y % 2 == 0 && d.os_z % 2 == 0 && (d.out_half || d.out_plane % 2 == 0) &&
+              al(d.out_f32) && al(d.out_hi) && al(d.aux) && al(d.aux2) && !g_gemm_direct_epilogue)
                  ? 1
                  : 0;
+  p.aux_vec = g_gemm_direct_aux ? 0 : 1;
 
   // ---- numerics: 3-term split-bf16 (default) or single-plane fp16 operands (1 MMA per K step)
-  p.planes = one_term ? 1 : 2;
+  const int planes = one_term ? 1 : 2;
   p.out_half = d.out_half ? 1 : 0;
   FGT_REQUIRE(!p.out_half || d.out_hi, FGT_ERR_ARG, "gemm_tc: out_half without a 16-bit output");
-  // ---- epilogue through shared memory + TMA tile stores: one output, channels contiguous, plain row order
-  const bool one_out = (d.out_f32 != nullptr) != (d.out_hi != nullptr);
-  p.tma_out = (one_out && p.vec_ok && !d.rowmap && d.lin_batch == 0 && d.bn % 64 == 0 && d.N % 4 == 0 &&
-               d.aux_mode != FGT_AUX_GRU_ZR && !g_gemm_direct_epilogue)
-                  ? 1
-                  : 0;
-  if (p.tma_out) {
-    const bool lin = p.linear != 0;
-    uint64_t dims[5] = {static_cast<uint64_t>(d.N), static_cast<uint64_t>(d.out_w), static_cast<uint64_t>(d.out_h),
-                        static_cast<uint64_t>(d.out_z), p.out_half ? 1u : 2u};
-    const uint64_t es = d.out_hi ? 2 : 4;
-    uint64_t str[4] = {static_cast<uint64_t>(d.os_x) * es, static_cast<uint64_t>(d.os_y) * es,
-                       static_cast<uint64_t>(d.os_z) * es, static_cast<uint64_t>(d.out_plane) * es};
-    if (lin || d.out_h == 1) str[1] = str[0] * dims[1];
-    if (lin || d.out_z == 1) str[2] = str[1] * dims[2];
-    if (p.out_half) str[3] = str[2] * dims[3];
-    uint32_t box[5] = {d.out_hi ? 64u : 32u, static_cast<uint32_t>(d.box_w), static_cast<uint32_t>(d.box_h), 1, 1};
-    int rc = d.out_hi ? encode_map_bf16(&p.out_map, d.out_hi, 5, dims, str, box)
-                      : encode_map_f32(&p.out_map, d.out_f32, 4, dims, str, box);
-    if (rc) return rc;
-    // fp32 output + an aux operand that is a plain fp32 tensor addressed like the output (residual add, gate multiply):
-    // fetch the aux tile by TMA as well — per-row 16-byte loads of a row-per-thread epilogue touch 32 lines per request
-    p.aux_tma = (!d.out_hi && d.aux && !g_gemm_direct_aux &&
-                 (d.aux_mode == FGT_AUX_ADD || d.aux_mode == FGT_AUX_MUL || d.aux_mode == FGT_AUX_ADD_PRE ||
-                  d.aux_mode == FGT_AUX_ADD_RELU))
-                    ? 1
-                    : 0;
-    if (p.aux_tma) {
-      rc = encode_map_f32(&p.aux_map, d.aux, 4, dims, str, box);
-      if (rc) return rc;
-    }
-  }
 
-  const uint32_t stage_bytes = static_cast<uint32_t>(p.planes) * (kAPlaneBytes + static_cast<uint32_t>(d.bn) * 128u);
-  // staging ring of the TMA epilogue: a slot holds one 64-channel chunk (two 16 KB panels; one for an fp16 output).
-  // More slots let the stores of one chunk drain while the next is written — what short-K layers need; long-K
-  // layers keep the shared memory for pipeline stages instead.
-  p.stg_slot_bytes = static_cast<int>(p.out_half ? kAPlaneBytes : 2 * kAPlaneBytes);
-  // alignment slack + barriers + two bias slices of bn floats. Sized exactly: a 128-wide split-bf16 tile with the
-  // TMA epilogue needs 3 x 64 KB stages + 32 KB of panels + this block within the 227 KB limit.
-  const uint32_t base_fixed = 1024u /*align*/ + 256u /*barriers*/ + 2u * static_cast<uint32_t>(d.bn) * 4u /*bias*/;
-  int stages = 0;
-  p.stg_slots = 0;
-  if (p.tma_out) {
-    for (int slots = 4; slots >= 1 && p.stg_slots == 0; slots >>= 1) {
-      const uint32_t fixed = base_fixed + static_cast<uint32_t>(slots * p.stg_slot_bytes);
-      const int st = static_cast<int>((227u * 1024u - fixed) / stage_bytes);
-      const int want = slots == 1 ? 2 : 4;  // extra slots only while at least 4 pipeline stages remain
-      if (st >= want) {
-        p.stg_slots = slots;
-        stages = st;
-      }
-    }
-    if (p.stg_slots == 0) p.tma_out = 0;  // tile too large to also hold the output panels: store from registers
-  }
-  if (!p.tma_out) stages = static_cast<int>((227u * 1024u - base_fixed) / stage_bytes);
+  const int n_mma = mma_n(d.bn);
+  const uint32_t stage_bytes = static_cast<uint32_t>(planes) * (kAPlaneBytes + static_cast<uint32_t>(n_mma) * 128u);
+  const uint32_t fixed = 1024u /*align*/ + 256u /*barriers*/;
+  int stages = static_cast<int>((227u * 1024u - fixed) / stage_bytes);
   if (stages > 6) stages = 6;
   FGT_REQUIRE(stages >= 2, FGT_ERR_ARG, "gemm_tc: tile too large for shared memory");
   p.stages = stages;
-  const size_t smem = static_cast<size_t>(stages) * stage_bytes + base_fixed +
-                      static_cast<size_t>(p.tma_out ? p.stg_slots * p.stg_slot_bytes : 0);
+  const size_t smem = static_cast<size_t>(stages) * stage_bytes + fixed;
 
-  static bool attr_set = false;
-  if (!attr_set) {
-    FGT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    FGT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    FGT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
   const bool ext = d.aux_mode == FGT_AUX_ADD_PRE || d.aux_mode == FGT_AUX_ADD_RELU || d.aux_mode == FGT_AUX_GRU ||
                    d.aux_mode == FGT_AUX_GRU_ZR || d.act == FGT_ACT_LEAKY001;
   if (d.aux_mode == FGT_AUX_GRU_ZR)
     FGT_REQUIRE(d.out_f32 && d.out_hi && p.vec_ok && d.N % 64 == 0 && (d.N / 2) % d.bn == 0 && d.groups == 1, FGT_ERR_ARG,
                 "gemm_tc: FGT_AUX_GRU_ZR needs both outputs, aligned unit-stride channels, N=%d a multiple of 64 and "
                 "bn=%d dividing N/2", d.N, d.bn);
+  FGT_REQUIRE(!ext || d.bn <= 128, FGT_ERR_ARG,
+              "gemm_tc: bn=%d; pre-activation add, add+ReLU, GRU updates and LeakyReLU(0.01) need bn <= 128", d.bn);
+  void* kern = one_term ? (ext ? gemm_kernel_for<true, 1>(n_mma) : gemm_kernel_for<true, 0>(n_mma))
+                        : (ext ? gemm_kernel_for<false, 1>(n_mma) : gemm_kernel_for<false, 0>(n_mma));
+  // raised once per instantiation: the attribute is per kernel
+  static std::mutex attr_mu;
+  static std::unordered_set<void*> attr_done;
+  {
+    std::lock_guard<std::mutex> lk(attr_mu);
+    if (!attr_done.count(kern)) {
+      FGT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_done.insert(kern);
+    }
+  }
   int grid = num_sms();
   if (grid > p.total_tiles) grid = p.total_tiles;
   FGT_REQUIRE(grid >= 1, FGT_ERR_ARG, "gemm_tc: empty problem");
-  if (ext) launch_k(gemm_tc_kernel<1>, dim3(grid), dim3(192), smem, stream, p);
-  else if (g_gemm_trace_on) launch_k(gemm_tc_kernel<0, 1>, dim3(grid), dim3(192), smem, stream, p);
-  else launch_k(gemm_tc_kernel<0>, dim3(grid), dim3(192), smem, stream, p);
+  launch_k(reinterpret_cast<void (*)(GemmParams)>(kern), dim3(grid), dim3(kGemmThreads), smem, stream, p);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }
@@ -886,20 +580,10 @@ extern "C" int fgt_gemm_tc(const FgtGemmDesc* desc, fgt_stream_t stream) {
   return fgt::gemm_tc_launch(*desc, reinterpret_cast<cudaStream_t>(stream));
 }
 
-// Debugging aid (not part of the product interface, like fgt_debug_flash_trace): while buf != NULL, common-epilogue
-// launches use the traced instantiation and CTA `cta` writes its clock64 timeline into buf
-// ([3 roles][64 local tiles][4 slots] int64, device memory): producer {tile start, first stage slot free, last load
-// issued}, MMA {tile start, accumulator buffer free, first operands landed, last MMA committed}, epilogue {tile start,
-// accumulator complete, stores issued}.
+// Debugging aid (not part of the product interface): bit 0 forces per-element epilogue stores, bit 1 per-element aux
+// loads on the paired path; both compute the same arithmetic as the default, so their outputs are bit-identical.
 extern "C" int fgt_debug_gemm_direct_epilogue(int on) {
   fgt::g_gemm_direct_epilogue = (on & 1) != 0;
   fgt::g_gemm_direct_aux = (on & 2) != 0;
-  return FGT_OK;
-}
-
-extern "C" int fgt_debug_gemm_trace(long long* buf, int cta) {
-  FGT_CUDA(cudaMemcpyToSymbol(fgt::g_gemm_trace, &buf, sizeof(buf)));
-  FGT_CUDA(cudaMemcpyToSymbol(fgt::g_gemm_trace_cta, &cta, sizeof(cta)));
-  fgt::g_gemm_trace_on = buf != nullptr;
   return FGT_OK;
 }

@@ -1,5 +1,5 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA/TMEM).
-// Everything here is device-side plumbing shared by gemm_tc.cu and flash.cu.
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA).
+// Everything here is device-side plumbing shared by gemm_tc.cu, flash.cu and conv_tail.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -49,7 +49,18 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a broken pipeline traps (context error) instead of hanging the GPU box.
+// Bounded wait without a diagnostic print, for kernels that issue wgmma: any function call (printf) in such a kernel
+// makes ptxas serialise its warpgroup MMAs. A broken pipeline traps (context error) instead of hanging.
+__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
+#pragma unroll 1
+  for (int i = 0; i < 2048; ++i)
+    if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
+  }
+}
+// Bounded wait: a broken pipeline prints which barrier stalled and traps (context error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 #pragma unroll 1
   for (int i = 0; i < 2048; ++i)
@@ -64,25 +75,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-__device__ __forceinline__ float4 ld_shared_f4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-
 // ---------------------------------------------------------------- fences
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -114,144 +109,46 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// TMA tile stores (shared -> global, bulk async group of the issuing thread). Out-of-range parts of the box
-// are clipped by the hardware, which is what handles M / N tails.
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3,
-                                             int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
-// wait until at most N of this thread's bulk store groups are still reading shared memory
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
-
-// ---------------------------------------------------------------- TMEM
-// Whole-warp collectives. `slot` is the shared-memory word that receives the TMEM base address.
-__device__ __forceinline__ void tmem_alloc(uint32_t slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(slot),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread i <-> lane base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05.mma (kind::f16, bf16 in, f32 acc)
-// Shared-memory matrix descriptor for a K-major tile stored as rows of 128 bytes with the
-// 128B swizzle (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 8-row atoms of 1024 B.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// ---------------------------------------------------------------- wgmma (bf16 / fp16 in, f32 accumulate in registers)
+// Shared-memory matrix descriptor (sm_90 layout) for a K-major tile stored as rows of 128 bytes with the 128B swizzle
+// (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 8-row atoms of 1024 B. Advance K by 16 elements with +2 (32 B >> 4).
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);         // start address  [0,14)
   d |= static_cast<uint64_t>(1) << 16;                         // LBO (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                 // SBO = 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;                         // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                         // layout: SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                         // layout: SWIZZLE_128B
   return d;
 }
-// Same swizzle, MN-major operand (the N/M index is the contiguous one): a [K rows x 64 elements (128 B)] block per
-// 64-wide slice of the MN extent, 8-row atoms of 1024 B along K; `mn_block_bytes` = distance between the slices.
-// Used for V [keys, d] as the B operand of P.V (K = keys, N = d). Advance K by 8 rows per 1024 B.
-__device__ __forceinline__ uint64_t umma_desc_sw128_mn(uint32_t saddr, uint32_t mn_block_bytes) {
+// Same swizzle, MN-major operand (the N index is the contiguous one): a [K rows x 64 elements (128 B)] block per
+// 64-wide slice of the N extent, 8-row atoms of 1024 B along K; `mn_block_bytes` = distance between the slices.
+// Used for V [keys, d] as the B operand of P.V (K = keys, N = d). Advance K by 16 rows with +128 (2048 B >> 4).
+__device__ __forceinline__ uint64_t gmma_desc_sw128_mn(uint32_t saddr, uint32_t mn_block_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);         // start address  [0,14)
-  d |= static_cast<uint64_t>(mn_block_bytes >> 4) << 16;       // LBO: next 64-element slice along MN
+  d |= static_cast<uint64_t>(mn_block_bytes >> 4) << 16;       // LBO: next 64-element slice along N
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                 // SBO: next 8 rows along K
-  d |= static_cast<uint64_t>(1) << 46;                         // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                         // layout: SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                         // layout: SWIZZLE_128B
   return d;
 }
-constexpr uint32_t kIdescBMajorMN = 1u << 16;  // instruction-descriptor bit: B operand is MN-major
-// Instruction descriptor: D=f32, A=B=bf16, both K-major, shape M x N (K = 16 per instruction).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-// Same with A = B = fp16 (operand format code 0).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+// Keeps the compiler from moving reads / writes of accumulator registers across wgmma fences and waits.
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same MMA with the A operand read from tensor memory (rows = TMEM lanes, two bf16 per 32-bit column).
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar)
-      : "memory");
-}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], A and B from shared memory (K-major descriptors). Accumulator fragment of
+// thread t of the warpgroup: d[4 j + 2 h + e] = D[16 (t / 32) + (t % 32) / 4 + 8 h][8 j + 2 (t % 4) + e].
+// kF16: fp16 operands instead of bf16. Specialisations for every N the engines use are in wgmma.cuh.
+template <int N, bool kF16>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d);
 
 // ---------------------------------------------------------------- split-bf16 helpers
 // A float v is carried as hi = bf16(v), lo = bf16(v - hi): hi + lo reproduces v to ~2^-17 relative.
@@ -284,3 +181,5 @@ __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b
 }
 
 }  // namespace fgt
+
+#include "wgmma.cuh"

@@ -1,4 +1,4 @@
-"""B200-native FGT generator behind the reference's nn.Module interface.
+"""H100-native FGT generator behind the reference's nn.Module interface.
 
 Drop-in for /root/reference/FGT/models/model.py: `Model(config).forward(frames, flows, masks)`
 with the same constructor dict, forward signature, output shape ([b*t,3,H,W]) and state_dict
@@ -6,7 +6,7 @@ keys/shapes (SURVEY.md Appendix B), so `load_state_dict(state["model_state_dict"
 checkpoint works (tool/video_inpainting.py:217-230, call site :724).
 
 The nn.Modules below only HOLD parameters under the reference's names; forward() never calls
-them. All arithmetic runs in libfgt_sm100a.so (tcgen05 implicit-GEMM engine, fused flash
+them. All arithmetic runs in libfgt_sm90a.so (wgmma implicit-GEMM engine, fused flash
 attention, HBM-bound helpers) through fgt_b200.lib. There is no CPU / PyTorch fallback.
 """
 import math
@@ -163,10 +163,10 @@ def _pick_bn(n_per_group, groups, name=""):
     return 128
 
 
-def _fill_sms(bn, n_total, m_positions, groups=1, n_sms=148):
+def _fill_sms(bn, n_total, m_positions, groups=1, n_sms=132):
     """Short windows (a frame-sharded rank's 1-3 frames, the driver's t = 6 window) leave most SMs without a tile when
     the channel tile is 128 wide, and a sub-wave GEMM takes as long as its one tile: halve the tile while the launch
-    covers at most half a wave (down to 64, the narrowest tile of the TMA-store epilogue)."""
+    covers at most half a wave (down to 64)."""
     m_tiles = -(-m_positions // 128)
     while (bn > 64 and bn % 32 == 0 and 2 * m_tiles * -(-n_total // bn) <= n_sms   # at most half a wave
            and (groups == 1 or (n_total // groups) % (bn // 2) == 0)):
@@ -175,7 +175,7 @@ def _fill_sms(bn, n_total, m_positions, groups=1, n_sms=148):
 
 
 class FGT(nn.Module):
-    """Parameter layout of FGT (model.py:196-246) + the sm_100a forward schedule (model.py:249-283)."""
+    """Parameter layout of FGT (model.py:196-246) + the sm_90a forward schedule (model.py:249-283)."""
 
     def __init__(self, t_groupSize, s_windowSize, g_downSize, input_resolution, in_channels, cnum, flow_inChannel,
                  flow_cnum, frame_hidden, flow_hidden, passmask, numBlocks, kernel_size, stride, padding, num_heads,
@@ -561,7 +561,7 @@ class FGT(nn.Module):
     def _out_proj(self, g, P, name, att, x):
         """x += output_linear(att) (attention_base.py:105, attention_flow.py:170; residual of model.py:127 / 146). The
         attention kernel has already undone the zone / window regrouping in its store (out_rowmap), so this is a plain
-        row-major GEMM over the real tokens with the residual in its epilogue and a TMA tile store."""
+        row-major GEMM over the real tokens with the residual in its epilogue."""
         rows = g.bt * g.n
         self._linear([lib.ASeg(att, self.d, rows)], P[name + ".o"], rows, aux=x, aux_mode=lib.AUX_ADD, out_f32=x)
 
@@ -645,7 +645,7 @@ class FGT(nn.Module):
         att = self._buf(g, "att_tok", (rows, d), dev, split=True)         # attention output in token order
         # flow re-weighting gate: f' = f * sigmoid(W_r [x; f] + b_r)   (attention_flow.py:126-128)
         self._linear([lib.ASeg(xs, d, rows), lib.ASeg(fs, df, rows)], P[name + ".gate"], rows, act=lib.ACT_SIGMOID,
-                     aux=f, aux_mode=lib.AUX_MUL, out_f32=fp, bn=64 if rows <= 128 * 74 else None)  # 114 -> 228 tiles
+                     aux=f, aux_mode=lib.AUX_MUL, out_f32=fp, bn=64 if rows <= 128 * 66 else None)  # <= half a wave of 128-wide tiles -> 64 wide
         # pooled global tokens (attention_flow.py:135,145) and the LayerNorm statistics of window rows and pooled
         # rows (attention_flow.py:142-143,154): one launch
         nl = g.nwp * 64
@@ -669,7 +669,7 @@ class FGT(nn.Module):
 
     def forward(self, masked_frames, flows, masks):
         if not masked_frames.is_cuda:
-            raise RuntimeError("fgt_b200.FGT runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+            raise RuntimeError("fgt_b200.FGT runs on a CUDA (sm_90a) device only; there is no CPU fallback")
         fs = getattr(self, "_fshard", None)
         graph_ok = fs is None or fs["exchange"] == "p2p"  # NCCL calls are not captured; the P2P exchange is kernels only
         if getattr(self, "_graphed", None) is not None and self.capture is None and graph_ok:

@@ -11,7 +11,7 @@ def warp(feat, flow, mode):
     if mode not in ("forward", "backward"):
         raise AssertionError("Invalid mode: {}".format(mode))
     if not feat.is_cuda:
-        raise RuntimeError("fgt_b200.flow_warp runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+        raise RuntimeError("fgt_b200.flow_warp runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     b, c, h, w = feat.shape
     if tuple(flow.shape) != (b, 2, h, w):
         raise ValueError(f"flow_warp: flow {tuple(flow.shape)} does not match features {tuple(feat.shape)}")

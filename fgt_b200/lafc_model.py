@@ -1,9 +1,9 @@
-"""B200-native LAFC flow-completion network behind the reference's nn.Module interface.
+"""H100-native LAFC flow-completion network behind the reference's nn.Module interface.
 
 Drop-in for /root/reference/LAFC/models/lafc.py: `Model(config).forward(flows, masks, edges=None)`
 -> (flow [b,2,H,W], edge [b,1,H,W]) with the same constructor dict and state_dict keys
 (tool/video_inpainting.py:200-214, call site :378). The nn.Modules only hold parameters; every
-convolution runs on the tcgen05 implicit-GEMM engine (P3D (1,k,k) convs as per-frame 2-D taps,
+convolution runs on the wgmma implicit-GEMM engine (P3D (1,k,k) convs as per-frame 2-D taps,
 (3,1,1) temporal convs as z-taps with TMA zero fill, dilated convs as tap offsets, skip concats as
 K-segments), the input gather and nearest upsampling on HBM-bound helper kernels. No CPU fallback.
 """
@@ -236,7 +236,7 @@ class P3DNet(nn.Module):
         if edges is not None:
             raise ValueError("fgt_b200 LAFC: the `edges` input is unused by the shipped driver (always None)")
         if not flows.is_cuda:
-            raise RuntimeError("fgt_b200 LAFC runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+            raise RuntimeError("fgt_b200 LAFC runs on a CUDA (sm_90a) device only; there is no CPU fallback")
         if getattr(self, "_graphed", None) is not None:
             return self._graphed(flows.float().contiguous(), masks.float().contiguous())
         return self._forward_impl(flows, masks)

@@ -1,4 +1,4 @@
-"""ctypes binding of libfgt_sm100a.so (the C-ABI in include/fgt_b200.h).
+"""ctypes binding of libfgt_sm90a.so (the C-ABI in include/fgt_b200.h).
 
 PyTorch is used here only to own device memory and the CUDA stream; all arithmetic on the path
 is done by the kernels in the shared library. There is no CPU fallback: if the library is missing
@@ -10,7 +10,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libfgt_sm100a.so")
+LIB_PATH = os.path.join(_HERE, "libfgt_sm90a.so")
 
 ACT_NONE, ACT_LEAKY02, ACT_RELU, ACT_SIGMOID, ACT_TANH, ACT_LEAKY001 = 0, 1, 2, 3, 4, 5
 AUX_NONE, AUX_ADD, AUX_MUL, AUX_ADD_PRE, AUX_ADD_RELU, AUX_GRU, AUX_GRU_ZR = 0, 1, 2, 3, 4, 5, 6

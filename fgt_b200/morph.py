@@ -12,7 +12,7 @@ from . import lib
 def _dev(device):
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if dev.type != "cuda":
-        raise RuntimeError("fgt_b200.morph runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+        raise RuntimeError("fgt_b200.morph runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     return dev
 
 

@@ -28,7 +28,7 @@ def pick_bn(n_per_group, groups=1):
     return 128
 
 
-def fill_sms(bn, n_total, m_positions, groups=1, n_sms=148):
+def fill_sms(bn, n_total, m_positions, groups=1, n_sms=132):
     """Small-M problems (RAFT's 1/8-resolution update block: 51 tiles of 128 positions) leave most SMs idle
     with 128-wide channel tiles; halve the tile while that raises the number of busy SMs."""
     m_tiles = -(-m_positions // 128)

@@ -257,7 +257,7 @@ class GpuBackend:
 
     def __init__(self, raft, lafc, fgt, device=None, raft_batch=4):
         if not torch.cuda.is_available():
-            raise RuntimeError("fgt_b200.pipeline.GpuBackend needs a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("fgt_b200.pipeline.GpuBackend needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.raft, self.lafc, self.fgt = raft, lafc, fgt
         self.fgt_model = fgt          # the callable the FGT stage evaluates per window (ShardedBackend swaps it)

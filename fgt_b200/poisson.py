@@ -20,7 +20,7 @@ MAX_ITERS = None      # None: scipy's own limit iter_lim = 2*H*W (then istop = 7
 def _dev(device):
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if dev.type != "cuda":
-        raise RuntimeError("fgt_b200 Poisson blending runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+        raise RuntimeError("fgt_b200 Poisson blending runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     return dev
 
 

@@ -1,4 +1,4 @@
-"""B200-native flow-guided gradient propagation behind the reference's function signature.
+"""H100-native flow-guided gradient propagation behind the reference's function signature.
 
 Drop-in for /root/reference/tool/get_flowNN_gradient.py: `get_flowNN_gradient(args, gradient_x,
 gradient_y, mask_RGB, mask, videoFlowF, videoFlowB, None, None) -> (gradient_x, gradient_y,
@@ -21,7 +21,7 @@ def get_flowNN_gradient(args, gradient_x, gradient_y, mask_RGB, mask, videoFlowF
     if getattr(args, "Nonlocal", False):
         raise ValueError("fgt_b200 implements Nonlocal=False (the driver's setting, video_inpainting.py:796)")
     if not torch.cuda.is_available():
-        raise RuntimeError("fgt_b200 get_flowNN_gradient needs a CUDA (sm_100a) device; there is no CPU fallback")
+        raise RuntimeError("fgt_b200 get_flowNN_gradient needs a CUDA (sm_90a) device; there is no CPU fallback")
     L = lib.load()
     dev = torch.device(device)
     H, W, N = mask.shape

@@ -1,13 +1,13 @@
-"""B200-native RAFT (basic model) behind the reference's nn.Module interface.
+"""H100-native RAFT (basic model) behind the reference's nn.Module interface.
 
 Drop-in for /root/reference/RAFT/raft.py: `RAFT(args).forward(image1, image2, iters=12,
 flow_init=None, upsample=True, test_mode=False)` with the reference's state_dict keys (179 tensors of
 raft-things.pth; survives the driver's DataParallel wrap/unwrap, tool/video_inpainting.py:186-197,
-call site :263). Parameter holders only; arithmetic runs in libfgt_sm100a.so:
+call site :263). Parameter holders only; arithmetic runs in libfgt_sm90a.so:
 
   * feature / context encoders: implicit-GEMM convs; InstanceNorm = fgt_chan_stats + fgt_instnorm_act,
     eval-mode BatchNorm folded into the conv weights at pack time;
-  * all-pairs correlation: one tcgen05 GEMM fmap1 x fmap2^T (alpha = 1/sqrt(256)) + fgt_avgpool2 pyramid;
+  * all-pairs correlation: one wgmma GEMM fmap1 x fmap2^T (alpha = 1/sqrt(256)) + fgt_avgpool2 pyramid;
   * per iteration: fgt_corr_lookup -> motion encoder convs -> SepConvGRU (z, r*h, and the
     (1-z)h+zq update fused in GEMM epilogues) -> flow head -> fgt_raft_flow_update;
   * mask head + fgt_convex_upsample only where the result is consumed (last iteration in test_mode;
@@ -241,7 +241,7 @@ class RAFT(nn.Module):
     # ------------------------------------------------------------------ forward
     def _forward_batch(self, im1, im2, iters, flow_init, test_mode, P, dev):
         """RAFT.forward (raft.py:86-148) on n image pairs at once: every kernel of the update loop covers
-        the n*h*w positions of all pairs, which is what fills the 148 SMs (one 1/8-resolution pair is 51 tiles)."""
+        the n*h*w positions of all pairs, which is what fills the 132 SMs (one 1/8-resolution pair is 51 tiles)."""
         n, _, H, W = im1.shape
         if H % 8 or W % 8:
             raise ValueError(f"RAFT input {H}x{W} must be divisible by 8 (the reference crashes otherwise, "
@@ -344,7 +344,7 @@ class RAFT(nn.Module):
 
     def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False):
         if not image1.is_cuda:
-            raise RuntimeError("fgt_b200 RAFT runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+            raise RuntimeError("fgt_b200 RAFT runs on a CUDA (sm_90a) device only; there is no CPU fallback")
         if getattr(self, "_graphs", None) is not None and flow_init is None:
             from .graphs import GraphedCall
             key = (iters, bool(test_mode))

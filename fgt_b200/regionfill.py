@@ -18,7 +18,7 @@ def regionfill_batch(images, masks, tol=1e-12, device=None, return_iters=False, 
     harmonic fill inside each mask, the image unchanged outside."""
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if dev.type != "cuda":
-        raise RuntimeError("fgt_b200 regionfill runs on a CUDA (sm_100a) device only; there is no CPU fallback")
+        raise RuntimeError("fgt_b200 regionfill runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     img = torch.as_tensor(images).to(dev, torch.float64).contiguous()
     msk = (torch.as_tensor(masks).to(dev) != 0).to(torch.uint8).contiguous()
     if img.dim() != 3 or img.shape != msk.shape:

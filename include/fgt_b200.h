@@ -1,18 +1,18 @@
-/* fgt_b200 — C-ABI of the B200-native (sm_100a) kernels behind FGT's flow-guided-attention
+/* fgt_b200 — C-ABI of the H100-native (sm_90a) kernels behind FGT's flow-guided-attention
  * inference path. Plain pointers and sizes only; every pointer is a DEVICE pointer unless the
  * name ends in _host. All work is enqueued on the stream passed by the caller; the library never
  * allocates or frees device memory and never synchronises unless stated.
  *
  * Every entry point returns 0 on success or a negative FGT_ERR_* code; fgt_last_error() gives the
- * message (thread-local). There is no CPU fallback: without an sm_100 device the calls fail.
+ * message (thread-local). There is no CPU fallback: without an sm_90 device the calls fail.
  *
  * Data carried between tensor-core kernels uses the "split-bf16" format: a logical fp32 tensor is
  * stored as two bf16 planes, hi = bf16(v) and lo = bf16(v - hi), the lo plane `plane` elements
- * after the hi plane. Three bf16 tcgen05 MMAs (hi*hi + hi*lo + lo*hi, fp32 accumulate in TMEM)
+ * after the hi plane. Three bf16 wgmma MMAs (hi*hi + hi*lo + lo*hi, fp32 accumulate in registers)
  * reproduce the fp32 product to ~2^-16 relative, which is what lets the path meet the 1e-3
  * end-to-end tolerance against the fp32 reference.
  *
- * Reference interfaces replaced (all under /root/reference, see INTEGRATION.md for the bindings):
+ * Reference interfaces replaced (paths in the original FGT project, see INTEGRATION.md for the bindings):
  *   fgt_gemm_tc      : every nn.Linear / nn.Conv2d / nn.Conv3d on the inference path —
  *                      FGT/models/model.py:33-50,206-215,95-96; transformer_base/attention_flow.py:
  *                      33-36,44-48,51-54; attention_base.py:38-41; ffn_base.py:39-46;
@@ -39,7 +39,7 @@ enum {
   FGT_OK = 0,
   FGT_ERR_ARG = -1,     /* bad shape / alignment / unsupported geometry */
   FGT_ERR_CUDA = -2,    /* CUDA runtime or driver call failed */
-  FGT_ERR_DEVICE = -3   /* no sm_100 device / driver entry point missing */
+  FGT_ERR_DEVICE = -3   /* no sm_90 device / driver entry point missing */
 };
 
 enum { FGT_ACT_NONE = 0, FGT_ACT_LEAKY02 = 1, FGT_ACT_RELU = 2, FGT_ACT_SIGMOID = 3, FGT_ACT_TANH = 4,
@@ -56,7 +56,7 @@ int fgt_version(void);
 const char* fgt_last_error(void);
 
 /* ------------------------------------------------------------------------------------------
- * fgt_gemm_tc: implicit-GEMM convolution / linear layer on tcgen05 tensor cores.
+ * fgt_gemm_tc: implicit-GEMM convolution / linear layer on the tensor cores (wgmma).
  *
  *   D[m, n] = act(alpha * sum_{tap, seg, c} A_seg[c, x(m)+dx(tap), y(m)+dy(tap), z(m)+dz(tap)]
  *                                          * W[n, tap, seg, c]  + bias[n])   (then aux add / mul)
@@ -92,7 +92,8 @@ typedef struct {
   int groups;
   int out_w, out_h, out_z;   /* output extents along x, y, z */
   int box_w, box_h;          /* output tile = box_w x box_h positions (<=128, multiple of 8) */
-  int bn;                    /* output-channel tile (multiple of 16, <= 256, divides N/groups if groups>1) */
+  int bn;                    /* output-channel tile (multiple of 16, <= 256, divides N/groups if groups>1;
+                                <= 128 with FGT_AUX_ADD_PRE / ADD_RELU / GRU / GRU_ZR or FGT_ACT_LEAKY001) */
   /* epilogue */
   const float* bias;         /* [N] or NULL */
   float alpha;               /* scale applied to the accumulator before bias */
@@ -118,7 +119,7 @@ int fgt_gemm_tc(const FgtGemmDesc* desc, fgt_stream_t stream);
  * fgt_attention: fused softmax(Q K^T * scale) V (flash-style, scores never leave the SM).
  * Q, K, V: split-bf16 row-major [batch, rows, heads*128] with their own leading dimensions, so one
  * fused QKV projection buffer [rows, 3*heads*128] can feed all three (V is consumed as an MN-major
- * tcgen05 B operand; no transposed copy). Output: split-bf16 [batch, Lq, heads*128].
+ * wgmma B operand; no transposed copy). Output: split-bf16 [batch, Lq, heads*128].
  *   mode 0 (dense)   : every query row attends to keys [0, Lk)            (TMHSA zones)
  *   mode 1 (windowed): query tile i (=two 64-token windows) attends to its own two 64-key tiles
  *                      (block-diagonal) plus the shared keys [glob_start, glob_start+glob_count)
@@ -141,14 +142,6 @@ typedef struct {
 } FgtAttnDesc;
 
 int fgt_attention(const FgtAttnDesc* desc, fgt_stream_t stream);
-
-/* Debug aid (not on the data path): with a device buffer of 3*64*8 int64, subsequent fgt_attention
- * launches record clock64() of CTA (0,0,0) per role (TMA / MMA / softmax) and key tile; NULL disables. */
-int fgt_debug_flash_trace(long long* device_buf);
-/* Debug aid (not on the data path): with a device buffer of 3*64*4 int64, subsequent common-epilogue fgt_gemm_tc
- * launches use a traced instantiation in which CTA `cta` records clock64() per role (TMA producer / MMA issuer /
- * epilogue) and local tile (see tools/trace_gemm.py for the slots); NULL disables. */
-int fgt_debug_gemm_trace(long long* device_buf, int cta);
 
 /* ------------------------------------------------------------------------------------------
  * HBM-bound helpers (coalesced / vectorised CUDA-core kernels). "split" outputs are split-bf16.
@@ -344,7 +337,7 @@ int fgt_resize_bilinear_f32(const float* in, int B, int H, int W, int C, int OH,
                             float scale_c1, float* out, fgt_stream_t stream);
 
 /* 3x3 convolution (zero padding 1, stride 1) with cout <= 3 output channels + bias + activation in one kernel: the
- * nine taps become the N dimension of a tcgen05 GEMM over the input positions (activation read once) and are summed
+ * nine taps become the N dimension of a wgmma GEMM over the input positions (activation read once) and are summed
  * per output pixel in shared memory — the decoder's final conv + tanh (FGT/models/model.py:185-193). x: NHWC
  * split-bf16 [n,H,W,cin], cin a multiple of 64 (<= 256); w: split-bf16 [32, cin], row tap*cout + c = W[c,:,ty,tx]
  * (zero rows up to 32); out: fp32 with element strides (os_n, os_c, os_y, os_x). Replaces fgt_gemm_tc "taps as N" +

@@ -7,4 +7,4 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) GPU; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU; run with -m gpu on a machine that has one")

@@ -1,4 +1,4 @@
-"""GPU parity of the full FGT forward (fgt_b200.fgt_model.Model, every op an sm_100a kernel behind
+"""GPU parity of the full FGT forward (fgt_b200.fgt_model.Model, every op an sm_90a kernel behind
 the C-ABI) against (a) the CPU oracle on the same seeded inputs and (b) the committed golden
 outputs of the unmodified reference. Tolerance: north_star's 1e-3 relative (rel-L2 and max/max)."""
 import pytest

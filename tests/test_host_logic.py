@@ -182,8 +182,8 @@ def test_fill_sms_tile_choice():
     """Channel-tile width by wave fill (fgt_model._fill_sms): 128 wide when the launch covers more than half a wave,
     halved (never below 64, never across a group boundary) when it does not."""
     from fgt_b200.fgt_model import _fill_sms
-    assert _fill_sms(128, 512, 7200) == 128             # 57 x 4 = 228 tiles: > half a wave of 148 SMs
-    assert _fill_sms(128, 512, 1440) == 64              # 12 x 4 = 48 tiles: 2 x 48 <= 148 -> 64 wide (96 tiles)
+    assert _fill_sms(128, 512, 7200) == 128             # 57 x 4 = 228 tiles: > half a wave of 132 SMs
+    assert _fill_sms(128, 512, 1440) == 64              # 12 x 4 = 48 tiles: 2 x 48 <= 132 -> 64 wide (96 tiles)
     assert _fill_sms(128, 512, 128) == 64               # a single row tile still stops at 64
     assert _fill_sms(64, 512, 128) == 64
     assert _fill_sms(128, 1536, 2160) == 128            # 17 x 12 = 204 tiles

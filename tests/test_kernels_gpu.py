@@ -1,4 +1,4 @@
-"""GPU parity of the individual sm_100a kernels, called through the C-ABI (fgt_b200.lib), against
+"""GPU parity of the individual sm_90a kernels, called through the C-ABI (fgt_b200.lib), against
 fp64 PyTorch restatements of the same op on the same seeded inputs."""
 
 import pytest
@@ -42,34 +42,35 @@ def test_conv(kw):
 
 
 @pytest.mark.parametrize("kw", [
-    dict(M=7200, N=1960, K=512, bn=128),                                              # fp32 only, N tail clipped by TMA
+    dict(M=7200, N=1960, K=512, bn=128),                                              # fp32 only, N tail (partial tile)
     dict(M=1000, N=520, K=1960, bn=128, act=2, split_only=True, aux_mode=1),          # split only, M and N tails, residual
     dict(M=7200, N=1536, K=512, bn=128, split_only=True),
     dict(M=333, N=256, K=320, bn=256, split_only=True, act=3, aux_mode=2),
     dict(M=7200, N=256, K=768, bn=128, terms=1, split_only=True),                     # fp16 operands, fp16 output
     dict(M=1000, N=192, K=576, bn=64, terms=1, act=1),                                # fp16 operands, fp32 output
     dict(M=2000, N=256, K=6272, bn=128, terms=1, split_out=True),                     # f_patch2vec: fp32 + split outputs
-    dict(M=70000, N=64, K=64, bn=64, split_only=True, act=1),                         # one K iteration per tile (8 TMEM buffers)
+    dict(M=70000, N=64, K=64, bn=64, split_only=True, act=1),                         # one K iteration per tile
 ])
-def test_linear_tma_epilogue_and_one_term(kw):
-    """Launches with a single, channel-contiguous output store through shared memory + TMA tile stores; terms=1 uses
-    single-plane fp16 operands (the flow branch)."""
+def test_linear_tails_and_one_term(kw):
+    """Linear launches with M / N tails, one or two outputs, aux operands, a 256-wide tile and one K iteration per tile;
+    terms=1 uses single-plane fp16 operands (the flow branch)."""
     from tools import diag_gemm as D
     assert D.linear_case(**kw)
 
 
 @pytest.mark.parametrize("kw", [
-    dict(n=2, h=61, w=107, cin=64, cout=128, k=3, stride=2, bn=128, split_only=True),  # edge tiles clipped by the TMA store
+    dict(n=2, h=61, w=107, cin=64, cout=128, k=3, stride=2, bn=128, split_only=True),  # partial output boxes at the right / bottom edges
     dict(n=2, h=60, w=108, cin=128, cout=128, k=3, bn=128, terms=1, split_only=True),
     dict(n=1, h=30, w=54, cin=192, cout=192, k=3, dil=4, bn=64, split_only=True),
 ])
-def test_conv_tma_epilogue_and_one_term(kw):
+def test_conv_edge_tiles_and_one_term(kw):
     from tools import diag_gemm as D
     assert D.conv_case(**kw)
 
 
-def test_tma_epilogue_bit_equal_to_register_epilogue():
-    """The two epilogue paths run the same arithmetic: identical bits."""
+def test_paired_epilogue_bit_equal_to_per_element_epilogue():
+    """The paired-access epilogue (8-byte fp32 / 4-byte 16-bit stores and aux loads) and the per-element one run the same
+    arithmetic: identical bits."""
     import ctypes
     lib = _lib()
     from fgt_b200 import packing
@@ -83,7 +84,7 @@ def test_tma_epilogue_bit_equal_to_register_epilogue():
     L = lib.load()
     L.fgt_debug_gemm_direct_epilogue.argtypes = [ctypes.c_int]
     outs = []
-    for direct in (0, 1, 2):   # 0: TMA epilogue + TMA-fetched aux tile, 1: register epilogue, 2: TMA epilogue + per-row aux loads
+    for direct in (0, 1, 2):   # 0: paired stores + paired aux loads, 1: per-element stores and loads, 2: paired stores + per-element aux loads
         L.fgt_debug_gemm_direct_epilogue(direct)
         try:
             o32 = torch.zeros(M, N, device=dev)

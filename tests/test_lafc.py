@@ -1,4 +1,4 @@
-"""LAFC flow completion (SURVEY §8 row a8): oracle vs reference goldens (CPU) and the sm_100a path
+"""LAFC flow completion (SURVEY §8 row a8): oracle vs reference goldens (CPU) and the sm_90a path
 vs oracle + goldens (GPU)."""
 import pytest
 import torch

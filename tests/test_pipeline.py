@@ -93,8 +93,8 @@ def test_gpu_pipeline_vs_reference_driver():
     import scipy.ndimage
     far = ~np.stack([scipy.ndimage.binary_dilation(h, iterations=args.frame_dilates) for h in hole0])
     assert (comp[far] == g["comp"][far]).all()
-    # measured on B200: flows 2.3e-3 px mean / 1.8e-2 px max error at 11 px mean magnitude (incl. the golden's fp16
-    # storage), propagation mask identical, final frames 8e-4 levels mean, max 1 level
+    # bounds: flow error relative to the mean flow magnitude (incl. the golden's fp16 storage), propagation mask
+    # identical, final frames within 1 level
     for k in ("flow_f", "flow_b", "done_f", "done_b"):
         assert rep[k][0] < 2e-3 * rep[k][2] and rep[k][1] < 1e-2 * rep[k][2], (k, rep[k])
     assert rep["mask_gradient_mismatch"] < 1e-3, rep

@@ -55,9 +55,6 @@ def test_kernel_target_logic_on_host_matches_oracle(mode):
     assert np.abs(out - FO.flow_prop(feat, flow, mode).numpy()).max() < 1e-5
 
 
-# (The file name sorts last on purpose: should the not-yet-executed kernel fault, no other GPU test shares its fate.)
-# Written after this round's GPU budget was spent: the kernel compiles for sm_100a but has not run on hardware yet, so the
-# expectation is recorded without being allowed to turn the suite red; the mark goes away with the first run in round 2.
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", ["forward", "backward"])
 def test_gpu_flow_warp_vs_golden_and_oracle(mode):

@@ -1,4 +1,4 @@
-"""GPU bring-up diagnostic for the tcgen05 GEMM engine: runs cases from trivial to complex and
+"""GPU bring-up diagnostic for the wgmma GEMM engine: runs cases from trivial to complex and
 prints error statistics (and error structure for the first failure). Run under gpurun."""
 import sys
 import os
@@ -130,7 +130,7 @@ def main():
         lambda: linear_case(7200, 1536, 512, bn=256, aux_mode=lib.AUX_ADD),
         lambda: linear_case(300, 48, 200, bn=48, act=lib.ACT_SIGMOID, aux_mode=lib.AUX_MUL),
         lambda: linear_case(40000, 512, 512, bn=128, scale=3.0),
-        lambda: linear_case(7200, 1960, 512, bn=128),                                  # N tail through the TMA store
+        lambda: linear_case(7200, 1960, 512, bn=128),                                  # N tail (partial tile)
         lambda: linear_case(1000, 520, 1960, bn=128, act=lib.ACT_RELU, split_only=True, aux_mode=lib.AUX_ADD),
         lambda: linear_case(7200, 1536, 512, bn=128, split_only=True),
         lambda: linear_case(333, 256, 320, bn=256, split_only=True, act=lib.ACT_SIGMOID, aux_mode=lib.AUX_MUL),

@@ -1,4 +1,4 @@
-"""GPU bring-up diagnostic for RAFT: compares the sm_100a path with the CPU oracle per iteration count."""
+"""GPU bring-up diagnostic for RAFT: compares the sm_90a path with the CPU oracle per iteration count."""
 import argparse
 import os
 import sys
