@@ -186,8 +186,8 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
   }
 }
 
-// BN: the wgmma N of the launch (>= p.bn; the B tile rows beyond p.bn are never written and their columns are
-// dropped). kF16: single-plane fp16 operands (one MMA per K step) instead of split-bf16 (three).
+// BN: the wgmma N of the launch (== p.bn). kF16: single-plane fp16 operands (one MMA per K step) instead of
+// split-bf16 (three).
 template <int BN, bool kF16, int kExt>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -364,7 +364,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       for (int j = 0; j < BN / 8; ++j) {
         const int cl = j * 8 + 2 * qc;
         const int col = n0 + cl;
-        if (cl < p.bn && col < p.N) {
+        if (col < p.N) {
           const bool two = col + 1 < p.N;
           const float b0 = p.bias ? __ldg(p.bias + col) : 0.f;
           const float b1 = (p.bias && two) ? __ldg(p.bias + col + 1) : 0.f;
@@ -384,11 +384,19 @@ static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b
 static bool g_gemm_direct_epilogue = false;  // debugging aid: per-element stores only (A/B comparisons)
 static bool g_gemm_direct_aux = false;       // debugging aid: aux operand by per-element loads on the paired path
 
-// wgmma N of a launch: the tile width itself up to 128 (every multiple of 16 has an instantiation), 256 above.
-static int mma_n(int bn) { return bn <= 128 ? bn : 256; }
+// Widest channel tile. A 256-wide tile leaves room for only two 96 KB stages of the split-bf16 ring, too shallow to
+// hide the TMA loads behind the MMAs on H100 (DESIGN.md 4.1).
+constexpr int kMaxBN = 128;
 
-// The extended epilogue (kExt = 1) has no 256-wide instantiation: its 128 accumulator registers per thread plus the
-// extended modes' state do not fit the 224-register budget without spilling; the host rejects bn > 128 for those modes.
+// Channel tile of a launch: the requested bn, or, above kMaxBN, the widest multiple of 16 <= kMaxBN that divides it, so
+// a requested tile runs as bn / tile equal tiles and never straddles a group boundary the request respects.
+static int tile_bn(int bn) {
+  int t = bn < kMaxBN ? bn : kMaxBN;
+  while (bn % t) t -= 16;
+  return t;
+}
+
+// wgmma N of a launch = its channel tile (every multiple of 16 up to kMaxBN has an instantiation).
 template <bool kF16, int kExt>
 static void* gemm_kernel_for(int n) {
   switch (n) {
@@ -400,9 +408,7 @@ static void* gemm_kernel_for(int n) {
     case 96: return reinterpret_cast<void*>(gemm_tc_kernel<96, kF16, kExt>);
     case 112: return reinterpret_cast<void*>(gemm_tc_kernel<112, kF16, kExt>);
     case 128: return reinterpret_cast<void*>(gemm_tc_kernel<128, kF16, kExt>);
-    default:
-      if constexpr (kExt != 0) return nullptr;
-      else return reinterpret_cast<void*>(gemm_tc_kernel<256, kF16, kExt>);
+    default: return nullptr;
   }
 }
 
@@ -425,6 +431,7 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   FGT_REQUIRE(d.aux_mode != FGT_AUX_GRU || d.aux2, FGT_ERR_ARG, "gemm_tc: FGT_AUX_GRU needs aux2");
   FGT_REQUIRE((reinterpret_cast<uintptr_t>(d.w_hi) & 15) == 0 && d.k_pad % 64 == 0, FGT_ERR_ARG,
               "gemm_tc: weights misaligned / k_pad=%d", d.k_pad);
+  const int bn = tile_bn(d.bn);
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
@@ -492,7 +499,7 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
     uint64_t dims[3] = {static_cast<uint64_t>(d.k_pad), static_cast<uint64_t>(d.N), one_term ? 1u : 2u};
     uint64_t strides[2] = {static_cast<uint64_t>(d.k_pad) * 2, static_cast<uint64_t>(d.w_plane) * 2};
     if (one_term) strides[1] = strides[0] * dims[1];
-    uint32_t box[3] = {kBK, static_cast<uint32_t>(d.bn), 1};
+    uint32_t box[3] = {kBK, static_cast<uint32_t>(bn), 1};
     int rc = encode_map_bf16(&p.b_map, d.w_hi, 3, dims, strides, box);
     if (rc) return rc;
   }
@@ -501,9 +508,9 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   p.tiles_x = (d.out_w + d.box_w - 1) / d.box_w;
   p.tiles_y = (d.out_h + d.box_h - 1) / d.box_h;
   p.tiles_z = d.out_z;
-  p.n_tiles = (d.N + d.bn - 1) / d.bn;
+  p.n_tiles = (d.N + bn - 1) / bn;
   p.total_tiles = p.tiles_x * p.tiles_y * p.tiles_z * p.n_tiles;
-  p.bn = d.bn;
+  p.bn = bn;
   p.box_w = d.box_w;
   p.box_h = d.box_h;
   p.a_rows = a_rows;
@@ -536,8 +543,7 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   p.out_half = d.out_half ? 1 : 0;
   FGT_REQUIRE(!p.out_half || d.out_hi, FGT_ERR_ARG, "gemm_tc: out_half without a 16-bit output");
 
-  const int n_mma = mma_n(d.bn);
-  const uint32_t stage_bytes = static_cast<uint32_t>(planes) * (kAPlaneBytes + static_cast<uint32_t>(n_mma) * 128u);
+  const uint32_t stage_bytes = static_cast<uint32_t>(planes) * (kAPlaneBytes + static_cast<uint32_t>(bn) * 128u);
   const uint32_t fixed = 1024u /*align*/ + 256u /*barriers*/;
   int stages = static_cast<int>((227u * 1024u - fixed) / stage_bytes);
   if (stages > 6) stages = 6;
@@ -551,10 +557,9 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
     FGT_REQUIRE(d.out_f32 && d.out_hi && p.vec_ok && d.N % 64 == 0 && (d.N / 2) % d.bn == 0 && d.groups == 1, FGT_ERR_ARG,
                 "gemm_tc: FGT_AUX_GRU_ZR needs both outputs, aligned unit-stride channels, N=%d a multiple of 64 and "
                 "bn=%d dividing N/2", d.N, d.bn);
-  FGT_REQUIRE(!ext || d.bn <= 128, FGT_ERR_ARG,
-              "gemm_tc: bn=%d; pre-activation add, add+ReLU, GRU updates and LeakyReLU(0.01) need bn <= 128", d.bn);
-  void* kern = one_term ? (ext ? gemm_kernel_for<true, 1>(n_mma) : gemm_kernel_for<true, 0>(n_mma))
-                        : (ext ? gemm_kernel_for<false, 1>(n_mma) : gemm_kernel_for<false, 0>(n_mma));
+  void* kern = one_term ? (ext ? gemm_kernel_for<true, 1>(bn) : gemm_kernel_for<true, 0>(bn))
+                        : (ext ? gemm_kernel_for<false, 1>(bn) : gemm_kernel_for<false, 0>(bn));
+  FGT_REQUIRE(kern, FGT_ERR_ARG, "gemm_tc: no instantiation for a %d-wide tile", bn);
   // raised once per instantiation: the attribute is per kernel
   static std::mutex attr_mu;
   static std::unordered_set<void*> attr_done;

@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 
 from . import lib
+from .ops import pick_box
 from .packing import fold_layernorm, pack_weight, pack_weight_im2col
 
 LN_EPS = 1e-5
@@ -127,16 +128,6 @@ class _Decoder(nn.Module):
         self.final = _ConvHolder(c // 2, cout, 3)
 
 
-def _pick_box(ow, oh):
-    """Output tile (box_w x box_h <= 128 positions) minimising padded work for an ow x oh map."""
-    best = None
-    for bw, bh in ((16, 8), (32, 4), (8, 16), (64, 2), (128, 1)):
-        tiles = -(-ow // bw) * -(-oh // bh)
-        if best is None or tiles < best[0]:
-            best = (tiles, bw, bh)
-    return best[1], best[2]
-
-
 # MMA terms of the flow branch (flow encoder + f_patch2vec). 1 = single-plane fp16 operands and activations (one MMA per
 # K step instead of three, half the activation bytes): the flow features only steer the spatial attention's gate and
 # Q/K, the flow tokens themselves stay within 1e-3 of the fp32 reference (fp16 has three more mantissa bits than bf16)
@@ -144,14 +135,7 @@ def _pick_box(ow, oh):
 # layer class needs the 3-term split product: each costs 2e-4..7e-4 end to end on its own even in fp16.
 _FLOW_TERMS = int(os.environ.get("FGT_FLOW_TERMS", "1"))
 
-# Layers whose output-channel tile is 256 instead of 128 (measured: only the 640->512 grouped encoder
-# conv gains, 0.443 -> 0.403 ms; smaller problems lose to wave quantisation). Tuning knob for experiments.
-_BN256 = os.environ.get("FGT_BN256", "enc10").split(",")
-
-
-def _pick_bn(n_per_group, groups, name=""):
-    if n_per_group % 256 == 0 and name in _BN256:
-        return 256
+def _pick_bn(n_per_group, groups):
     if n_per_group % 128 == 0:
         return 128
     if n_per_group <= 128:
@@ -438,14 +422,14 @@ class FGT(nn.Module):
             cpg = [c if groups > 1 else 0 for c in seg_counts]
             segs = [lib.ASeg(x, cin, w, h, n, c_per_group=cpg[0], c_count=seg_counts[0]),
                     lib.ASeg(x2, cin2, w, h, n, c_per_group=cpg[1], c_count=seg_counts[1])]
-        bw, bh = _pick_box(ow, oh)
+        bw, bh = pick_box(ow, oh)
         if nchw_out:
             strides = dict(os_z=N * oh * ow, os_y=ow, os_x=1, os_c=oh * ow)
         else:
             strides = dict(os_z=oh * ow * N, os_y=ow * N, os_x=N, os_c=1)
         lib.gemm_tc(segs, wp["w"], N, kx=k, ky=k, stride=stride, pad_x=pad, pad_y=pad, groups=groups, out_w=ow,
                     out_h=oh, out_z=n, box_w=bw, box_h=bh,
-                    bn=_fill_sms(_pick_bn(N // groups, groups, wp["name"]), N, n * oh * ow, groups), bias=wp["b"], act=act,
+                    bn=_fill_sms(_pick_bn(N // groups, groups), N, n * oh * ow, groups), bias=wp["b"], act=act,
                     out_f32=out_f32, out_split=out_split, out_f16=out_f16, tag=wp["name"], terms=terms, alg_k=alg_k,
                     **strides)
         return oh, ow
@@ -453,26 +437,25 @@ class FGT(nn.Module):
     @staticmethod
     def _deconv(x, cin, n, h, w, P, name, out_split):
         """nearest-x2 + 3x3 conv + LeakyReLU as four 2x2 phase convs writing the interleaved [n,2h,2w,N] output."""
-        bw, bh = _pick_box(w, h)
+        bw, bh = pick_box(w, h)
         for py in (0, 1):
             for px in (0, 1):
                 wp = P[f"{name}.p{py}{px}"]
                 N = wp["N"]
                 lib.gemm_tc([lib.ASeg(x, cin, w, h, n)], wp["w"], N, kx=2, ky=2, pad_x=1 - px, pad_y=1 - py, out_w=w,
-                            out_h=h, out_z=n, box_w=bw, box_h=bh, bn=_pick_bn(N, 1, name), bias=wp["b"],
+                            out_h=h, out_z=n, box_w=bw, box_h=bh, bn=_pick_bn(N, 1), bias=wp["b"],
                             act=lib.ACT_LEAKY02, out_split=out_split, out_elem_offset=(py * 2 * w + px) * N,
                             os_z=4 * h * w * N, os_y=4 * w * N, os_x=2 * N, os_c=1, tag=wp["name"])
 
     @staticmethod
     def _linear(segs, wp, rows, bn=None, **kw):
         lib.gemm_tc(segs, wp["w"], wp["N"], out_w=rows,
-                    bn=bn or _fill_sms(_pick_bn(wp["N"], 1, wp["name"]), wp["N"], rows), bias=wp["b"], tag=wp["name"], **kw)
+                    bn=bn or _fill_sms(_pick_bn(wp["N"], 1), wp["N"], rows), bias=wp["b"], tag=wp["name"], **kw)
 
     def _ffn(self, g, P, name, x, xs, dev, need_split=True):
         """x += FusionFeedForward(LN(x)) (ffn_base.py:53-77, model.py:128-129 / 147-148). need_split: whether the next
         consumer reads the split-bf16 copy of x (a spatial block's gate GEMM, vec2patch); when it does not (a temporal
-        block or the positional embedding follows: they read the fp32 x), the second GEMM has a single output and stores
-        through the TMA epilogue."""
+        block or the positional embedding follows: they read the fp32 x), the second GEMM writes the fp32 x alone."""
         with lib.scope("ffn"):
             self._ffn_impl(g, P, name, x, xs if need_split else None, dev)
 
@@ -546,9 +529,9 @@ class FGT(nn.Module):
         # rows were written by this rank's own LayerNorm launch (stream order), so the Q projection runs BEFORE the
         # barrier and hides the time the peers' rows need to arrive over NVLink.
         wq = P[name + ".q"]
-        bw, bh = _pick_box(Lzl, g.zones)
+        bw, bh = pick_box(Lzl, g.zones)
         lib.gemm_tc([lib.ASeg(s_all, d, Lzl, g.zones, 1, sx=d, sy=Lz * d, elem_offset=off * zl * d)], wq["w"], d,
-                    out_w=Lzl, out_h=g.zones, box_w=bw, box_h=bh, bn=_pick_bn(d, 1, wq["name"]), bias=wq["b"],
+                    out_w=Lzl, out_h=g.zones, box_w=bw, box_h=bh, bn=_pick_bn(d, 1), bias=wq["b"],
                     out_split=q, os_x=d, os_y=Lzl * d, tag=wq["name"])
         pg.barrier()  # every peer's rows of this layer are in s_all
         self._linear([lib.ASeg(s_all, d, g.zones * Lz)], P[name + ".kv"], g.zones * Lz, out_split=kv)

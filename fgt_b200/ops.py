@@ -1,17 +1,24 @@
 """Launch helpers shared by the LAFC / RAFT host modules: NHWC split-bf16 convolutions on the
 tensor-core engine (fgt_gemm_tc), with the tile heuristics in one place."""
+import functools
+
 from . import lib
 from .packing import pack_weight, pack_weight_im2col
 
+# Output boxes the GEMM engine takes: box_w x box_h <= 128 positions, a multiple of 8 (the 8-row swizzle atom of the
+# A tile). Five 128-position boxes come first and the rest by size, so a tie in tile count keeps the larger box.
+_FIRST = ((16, 8), (32, 4), (8, 16), (64, 2), (128, 1))
+_BOXES = _FIRST + tuple(sorted(((bw, bh) for bh in range(1, 129) for bw in range(1, 128 // bh + 1)
+                                if bw * bh % 8 == 0 and (bw, bh) not in _FIRST),
+                               key=lambda b: (-b[0] * b[1], -b[0])))
 
+
+@functools.lru_cache(maxsize=None)
 def pick_box(ow, oh):
-    """Output tile (box_w x box_h <= 128 positions) minimising padded work for an ow x oh map."""
-    best = None
-    for bw, bh in ((16, 8), (32, 4), (8, 16), (64, 2), (128, 1)):
-        tiles = -(-ow // bw) * -(-oh // bh)
-        if best is None or tiles < best[0]:
-            best = (tiles, bw, bh)
-    return best[1], best[2]
+    """Output box (box_w, box_h) for an ow x oh map: the fewest tiles, since every tile runs 128 MMA rows whatever its
+    box holds (the 20 x 36 token grid: 12 x 10, 6 tiles instead of 9 with 16 x 8). The box may be wider or taller than
+    the map."""
+    return min(_BOXES, key=lambda b: -(-ow // b[0]) * -(-oh // b[1]))
 
 
 def pick_bn(n_per_group, groups=1):

@@ -92,8 +92,9 @@ typedef struct {
   int groups;
   int out_w, out_h, out_z;   /* output extents along x, y, z */
   int box_w, box_h;          /* output tile = box_w x box_h positions (<=128, multiple of 8) */
-  int bn;                    /* output-channel tile (multiple of 16, <= 256, divides N/groups if groups>1;
-                                <= 128 with FGT_AUX_ADD_PRE / ADD_RELU / GRU / GRU_ZR or FGT_ACT_LEAKY001) */
+  int bn;                    /* output-channel tile (multiple of 16, <= 256, divides N/groups if groups>1); a
+                                request wider than 128 runs as bn/t tiles of t channels, t the widest multiple
+                                of 16 <= 128 dividing bn, so tiles never straddle a group boundary */
   /* epilogue */
   const float* bias;         /* [N] or NULL */
   float alpha;               /* scale applied to the accumulator before bias */
