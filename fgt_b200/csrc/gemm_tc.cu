@@ -7,8 +7,9 @@
 //   warp 8     : TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
 //
 // One CTA per SM loops over output tiles (128 output positions x bn channels); the producer runs ahead through the
-// stage ring while the consumers finish the previous tile's epilogue. Used for every Linear/Conv on the path (see
-// include/fgt_b200.h).
+// stage ring while the consumers finish the previous tile's epilogue. The epilogue loads its bias / aux operands in
+// batches before the accumulators are final, and up to bn = 64 the consumers issue the next tile's first K stage before
+// it. Used for every Linear/Conv on the path (see include/fgt_b200.h).
 #include "common.h"
 #include "ptx.cuh"
 
@@ -50,6 +51,7 @@ struct GemmParams {
   int lin_batch;
   int vec_ok;   // channel pairs stored (and aux pairs loaded) as one 8-byte / 4-byte access
   int aux_vec;  // aux pairs loaded as one access (debugging aid: 0 = per-element loads)
+  int vec4_ok;  // 4-channel accesses (16-byte fp32 / 8-byte 16-bit) are aligned: the batched epilogue may run
   long long os_z, os_y, os_x, os_c;
   const int* rowmap;
   float* out_f32;
@@ -186,9 +188,91 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
   }
 }
 
+// ---- Batched epilogue (kExt = 0, whole tile inside N, unit channel stride, 16-byte aligned rows: `vec4_ok`).
+// The operands that do not depend on the accumulators (bias, aux) are loaded for a chunk of JC column groups j at once,
+// before the accumulators are final, so the tile waits for global memory once per chunk instead of once per column
+// pair. The quad of threads (qc = 0..3) that holds rows (r, r + 8) x channels [8 j, 8 j + 8) swaps pairs with
+// `shfl_xor(1)` so that thread qc owns row r + 8 (qc & 1), channels [8 j + 4 (qc >> 1), + 4): one 16-byte fp32 store,
+// 8 bytes per 16-bit plane. Each element gets exactly the arithmetic of epi_pair (bias fma, activation, aux), so the
+// bits are the same. In-place residual (aux == out_f32): every element is read by the thread that writes it, before
+// it writes it.
+template <int JC>
+struct EpiPre {
+  float b[JC][2];  // bias of this thread's accumulator pair (channels 8 j + 2 qc, + 1)
+  float4 a[JC];    // aux of the 4 channels this thread stores
+};
+
+__device__ __forceinline__ bool aux_loaded(int aux_mode) { return aux_mode == FGT_AUX_ADD || aux_mode == FGT_AUX_MUL; }
+
+template <int JC>
+__device__ __forceinline__ void epi_prefetch(EpiPre<JC>& pre, const EpiArgs& e, const float* bias, int j0, int n0,
+                                             int qc, long long off, bool valid) {
+#pragma unroll
+  for (int jj = 0; jj < JC; ++jj) {
+    const int col = n0 + (j0 + jj) * 8 + 2 * qc;
+    pre.b[jj][0] = bias ? __ldg(bias + col) : 0.f;
+    pre.b[jj][1] = bias ? __ldg(bias + col + 1) : 0.f;
+  }
+  if (aux_loaded(e.aux_mode)) {
+    const float* src = e.aux + off + n0 + 4 * (qc >> 1);
+#pragma unroll
+    for (int jj = 0; jj < JC; ++jj)
+      pre.a[jj] = valid ? __ldg(reinterpret_cast<const float4*>(src + (j0 + jj) * 8)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
+// kAct: 0 = none, 1 = LeakyReLU(0.2), 2 = any other kExt = 0 activation (act_one).
+template <int kAct>
+__device__ __forceinline__ float epi_act(float v, int act) {
+  if (kAct == 1) return v > 0.f ? v : 0.2f * v;
+  if (kAct == 2) return act_one(v, act);
+  return v;
+}
+
+template <int kAct, int JC, int R>
+__device__ __forceinline__ void epi_chunk(const EpiArgs& e, const float (&acc)[R], const EpiPre<JC>& pre, int j0,
+                                          int n0, int qc, long long off, bool valid) {
+  const bool odd = qc & 1;
+  const long long ob = off + n0 + 4 * (qc >> 1);
+#pragma unroll
+  for (int jj = 0; jj < JC; ++jj) {
+    const int j = j0 + jj;
+    const float b0 = pre.b[jj][0], b1 = pre.b[jj][1];
+    const float v00 = fmaf(acc[4 * j], e.alpha, b0), v01 = fmaf(acc[4 * j + 1], e.alpha, b1);
+    const float v10 = fmaf(acc[4 * j + 2], e.alpha, b0), v11 = fmaf(acc[4 * j + 3], e.alpha, b1);
+    // keep the pair of row (qc & 1), trade the other row's pair with the neighbour qc ^ 1
+    const float r0 = __shfl_xor_sync(0xffffffffu, odd ? v00 : v10, 1);
+    const float r1 = __shfl_xor_sync(0xffffffffu, odd ? v01 : v11, 1);
+    float x[4];
+    x[0] = odd ? r0 : v00;
+    x[1] = odd ? r1 : v01;
+    x[2] = odd ? v10 : r0;
+    x[3] = odd ? v11 : r1;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) x[q] = epi_act<kAct>(x[q], e.act);
+    if (e.aux_mode == FGT_AUX_ADD) {
+      x[0] += pre.a[jj].x; x[1] += pre.a[jj].y; x[2] += pre.a[jj].z; x[3] += pre.a[jj].w;
+    } else if (e.aux_mode == FGT_AUX_MUL) {
+      x[0] *= pre.a[jj].x; x[1] *= pre.a[jj].y; x[2] *= pre.a[jj].z; x[3] *= pre.a[jj].w;
+    }
+    if (!valid) continue;
+    const long long o = ob + j * 8;
+    if (e.out_f32) *reinterpret_cast<float4*>(e.out_f32 + o) = make_float4(x[0], x[1], x[2], x[3]);
+    if (e.out_hi && e.out_half) {
+      *reinterpret_cast<uint2*>(e.out_hi + o) = make_uint2(pack_f16x2(x[0], x[1]), pack_f16x2(x[2], x[3]));
+    } else if (e.out_hi) {
+      uint32_t h0, l0, h1, l1;
+      split_bf16x2(x[0], x[1], h0, l0);
+      split_bf16x2(x[2], x[3], h1, l1);
+      *reinterpret_cast<uint2*>(e.out_hi + o) = make_uint2(h0, h1);
+      *reinterpret_cast<uint2*>(e.out_hi + e.out_plane + o) = make_uint2(l0, l1);
+    }
+  }
+}
+
 // BN: the wgmma N of the launch (== p.bn). kF16: single-plane fp16 operands (one MMA per K step) instead of
-// split-bf16 (three).
-template <int BN, bool kF16, int kExt>
+// split-bf16 (three). kSerial: the previous schedule (no early K stage, per-pair epilogue), kept for A/B comparisons.
+template <int BN, bool kF16, int kExt, bool kSerial>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atoms.
@@ -277,8 +361,50 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
     const int qc = lane & 3;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    int prev = -1;  // ring stage of the newest issued MMA group; released once a later group has been waited past
+    // Schedule: after a tile's last K stage, each warpgroup issues the first K stage of its next tile into the other
+    // accumulator array and runs the tile's epilogue while the tensor cores work on it. Stage release, the wgmma group
+    // count and the MMA order are those of back-to-back tiles; only the issue point moves. The early stage is issued
+    // unconditionally (a runtime trip count around a wgmma makes ptxas serialise all of them); without a next tile it
+    // is a dummy stage that waits on no barrier and whose result is never read. Two accumulator arrays fit in the 168
+    // registers a thread has at 288 threads (allocated as 12 warps) up to BN = 64.
+    constexpr int early = (!kSerial && BN <= 64) ? 1 : 0;  // K stages of a tile issued before the previous epilogue
+    // Registers cannot be indexed dynamically: the tile loop runs pairs of tiles with the two arrays in swapped roles.
+    float acc0[BN / 2], acc1[BN / 2];
+
+    // Issues the MMAs of K stage `it` of a tile into `acc` (the caller commits the group).
+    auto mma_stage = [&](float (&acc)[BN / 2], int it, bool loaded) {
+      if (loaded) mbar_wait_quiet(full_bar(stage), phase);
+      const uint32_t sa = smem_base + stage * stage_bytes;
+      const uint32_t sb = sa + nplanes * kAPlaneBytes;
+      const uint64_t a_hi = gmma_desc_sw128(sa + a_off);
+      const uint64_t b_hi = gmma_desc_sw128(sb);
+      fence_regs(acc);
+      wgmma_fence();
+      if (nplanes == 2) {
+        const uint64_t a_lo = gmma_desc_sw128(sa + kAPlaneBytes + a_off);
+        const uint64_t b_lo = gmma_desc_sw128(sb + b_plane_bytes);
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k) {
+          const uint64_t ko = static_cast<uint64_t>(k * 2);  // 32 bytes >> 4
+          wgmma_ss<BN, kF16>(acc, a_lo + ko, b_hi + ko, (it | k) != 0);
+          wgmma_ss<BN, kF16>(acc, a_hi + ko, b_lo + ko, 1u);
+          wgmma_ss<BN, kF16>(acc, a_hi + ko, b_hi + ko, 1u);
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k) {
+          const uint64_t ko = static_cast<uint64_t>(k * 2);
+          wgmma_ss<BN, kF16>(acc, a_hi + ko, b_hi + ko, (it | k) != 0);
+        }
+      }
+    };
+    auto advance = [&]() {
+      if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+    };
+
+    // One tile: its remaining K stages into `cur`, the first stage of `next_tile` into `nxt`, the epilogue from `cur`.
+    auto run_tile = [&](float (&cur)[BN / 2], float (&nxt)[BN / 2], int tile, int next_tile) {
       const int nt = tile % p.n_tiles;
       const int mt = tile / p.n_tiles;
       const int z = mt / tiles_per_z;
@@ -287,45 +413,16 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       const int tx = rem - ty * p.tiles_x;
       const int n0 = nt * p.bn;
 
-      int prev = -1;
-      for (int it = 0; it < p.k_iters; ++it) {
-        mbar_wait_quiet(full_bar(stage), phase);
-        {
-          const uint32_t sa = smem_base + stage * stage_bytes;
-          const uint32_t sb = sa + nplanes * kAPlaneBytes;
-          const uint64_t a_hi = gmma_desc_sw128(sa + a_off);
-          const uint64_t b_hi = gmma_desc_sw128(sb);
-          fence_regs(acc);
-          wgmma_fence();
-          if (nplanes == 2) {
-            const uint64_t a_lo = gmma_desc_sw128(sa + kAPlaneBytes + a_off);
-            const uint64_t b_lo = gmma_desc_sw128(sb + b_plane_bytes);
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) {
-              const uint64_t ko = static_cast<uint64_t>(k * 2);  // 32 bytes >> 4
-              wgmma_ss<BN, kF16>(acc, a_lo + ko, b_hi + ko, (it | k) != 0);
-              wgmma_ss<BN, kF16>(acc, a_hi + ko, b_lo + ko, 1u);
-              wgmma_ss<BN, kF16>(acc, a_hi + ko, b_hi + ko, 1u);
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) {
-              const uint64_t ko = static_cast<uint64_t>(k * 2);
-              wgmma_ss<BN, kF16>(acc, a_hi + ko, b_hi + ko, (it | k) != 0);
-            }
-          }
-          wgmma_commit();
-          // the group of the previous stage has retired once at most this one is pending
-          wgmma_wait<1>();
-          fence_regs(acc);
-        }
+      for (int it = early; it < p.k_iters; ++it) {
+        mma_stage(cur, it, true);
+        wgmma_commit();
+        // the group of the previous stage has retired once at most this one is pending
+        wgmma_wait<1>();
+        fence_regs(cur);
         if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         prev = stage;
-        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+        advance();
       }
-      wgmma_wait<0>();
-      fence_regs(acc);
-      if (lane == 0) mbar_arrive(empty_bar(prev));
 
       // output positions of this thread's two accumulator rows
       long long off[2];
@@ -360,22 +457,86 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
         off[h] = o;
         valid[h] = v;
       }
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int cl = j * 8 + 2 * qc;
-        const int col = n0 + cl;
-        if (col < p.N) {
-          const bool two = col + 1 < p.N;
-          const float b0 = p.bias ? __ldg(p.bias + col) : 0.f;
-          const float b1 = (p.bias && two) ? __ldg(p.bias + col + 1) : 0.f;
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            if (valid[h])
-              epi_pair<kExt>(ep, fmaf(acc[4 * j + 2 * h], ep.alpha, b0), fmaf(acc[4 * j + 2 * h + 1], ep.alpha, b1),
-                             off[h], col, two);
+      // The batched epilogue stores row (qc & 1) of the quad's two rows. Its first load batch goes out while the tile's
+      // last MMA group runs.
+      const bool batched = kExt == 0 && !kSerial && p.vec4_ok && n0 + BN <= p.N;
+      const long long off_q = (qc & 1) ? off[1] : off[0];
+      const bool valid_q = (qc & 1) ? valid[1] : valid[0];
+      // column groups per load batch, as registers allow: 4 at BN = 64 next to two accumulator arrays, half the tile
+      // above BN = 96
+      constexpr int JC = (early && BN == 64) ? 4 : BN >= 112 ? BN / 16 : BN / 8;
+      EpiPre<JC> pre;
+      if (batched) epi_prefetch<JC>(pre, ep, p.bias, 0, n0, qc, off_q, valid_q);
+
+      // The next tile's first stage goes to the tensor cores before this tile's epilogue.
+      const int last = prev;
+      const bool has_next = next_tile < p.total_tiles;
+      prev = -1;
+      for (int e = 0; e < early; ++e) {
+        mma_stage(nxt, 0, has_next);
+        if (has_next) {
+          prev = stage;
+          advance();
         }
       }
+      // retire every group of `cur` with a count fixed at compile time (the commit is unconditional: a commit on a
+      // divergent path, or a wait ptxas cannot prove covers `cur`, makes it serialise the MMAs)
+      if constexpr (early) {
+        wgmma_commit();
+        wgmma_wait<1>();
+      } else {
+        wgmma_wait<0>();
+      }
+      fence_regs(cur);
+      if (lane == 0) mbar_arrive(empty_bar(last));
+
+      if (batched) {
+        const int act_kind = ep.act == FGT_ACT_NONE ? 0 : ep.act == FGT_ACT_LEAKY02 ? 1 : 2;
+#pragma unroll
+        for (int j0 = 0; j0 < BN / 8; j0 += JC) {
+          if (j0 > 0) epi_prefetch<JC>(pre, ep, p.bias, j0, n0, qc, off_q, valid_q);
+          if (act_kind == 0) epi_chunk<0>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
+          else if (act_kind == 1) epi_chunk<1>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
+          else epi_chunk<2>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int cl = j * 8 + 2 * qc;
+          const int col = n0 + cl;
+          if (col < p.N) {
+            const bool two = col + 1 < p.N;
+            const float b0 = p.bias ? __ldg(p.bias + col) : 0.f;
+            const float b1 = (p.bias && two) ? __ldg(p.bias + col + 1) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              if (valid[h])
+                epi_pair<kExt>(ep, fmaf(cur[4 * j + 2 * h], ep.alpha, b0), fmaf(cur[4 * j + 2 * h + 1], ep.alpha, b1),
+                               off[h], col, two);
+          }
+        }
+      }
+    };
+
+    const int step = gridDim.x;
+    int tile = blockIdx.x;  // grid <= total_tiles: every CTA has a tile
+    if constexpr (early) {
+      mma_stage(acc0, 0, true);
+      wgmma_commit();
+      prev = stage;
+      advance();
     }
+    if constexpr (early) {
+      for (; tile < p.total_tiles; tile += 2 * step) {
+        run_tile(acc0, acc1, tile, tile + step);
+        if (tile + step >= p.total_tiles) break;
+        run_tile(acc1, acc0, tile + step, tile + 2 * step);
+      }
+    } else {
+      // one array: a second one behind the pair loop's exit stays live (spills) and makes ptxas serialise the MMAs
+      for (; tile < p.total_tiles; tile += step) run_tile(acc0, acc0, tile, tile + step);
+    }
+    wgmma_wait<0>();
   }
 }
 
@@ -383,6 +544,7 @@ static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b
 
 static bool g_gemm_direct_epilogue = false;  // debugging aid: per-element stores only (A/B comparisons)
 static bool g_gemm_direct_aux = false;       // debugging aid: aux operand by per-element loads on the paired path
+static bool g_gemm_serial = false;           // debugging aid: the previous tile schedule (A/B timing)
 
 // Widest channel tile. A 256-wide tile leaves room for only two 96 KB stages of the split-bf16 ring, too shallow to
 // hide the TMA loads behind the MMAs on H100 (DESIGN.md 4.1).
@@ -397,17 +559,17 @@ static int tile_bn(int bn) {
 }
 
 // wgmma N of a launch = its channel tile (every multiple of 16 up to kMaxBN has an instantiation).
-template <bool kF16, int kExt>
+template <bool kF16, int kExt, bool kSerial>
 static void* gemm_kernel_for(int n) {
   switch (n) {
-    case 16: return reinterpret_cast<void*>(gemm_tc_kernel<16, kF16, kExt>);
-    case 32: return reinterpret_cast<void*>(gemm_tc_kernel<32, kF16, kExt>);
-    case 48: return reinterpret_cast<void*>(gemm_tc_kernel<48, kF16, kExt>);
-    case 64: return reinterpret_cast<void*>(gemm_tc_kernel<64, kF16, kExt>);
-    case 80: return reinterpret_cast<void*>(gemm_tc_kernel<80, kF16, kExt>);
-    case 96: return reinterpret_cast<void*>(gemm_tc_kernel<96, kF16, kExt>);
-    case 112: return reinterpret_cast<void*>(gemm_tc_kernel<112, kF16, kExt>);
-    case 128: return reinterpret_cast<void*>(gemm_tc_kernel<128, kF16, kExt>);
+    case 16: return reinterpret_cast<void*>(gemm_tc_kernel<16, kF16, kExt, kSerial>);
+    case 32: return reinterpret_cast<void*>(gemm_tc_kernel<32, kF16, kExt, kSerial>);
+    case 48: return reinterpret_cast<void*>(gemm_tc_kernel<48, kF16, kExt, kSerial>);
+    case 64: return reinterpret_cast<void*>(gemm_tc_kernel<64, kF16, kExt, kSerial>);
+    case 80: return reinterpret_cast<void*>(gemm_tc_kernel<80, kF16, kExt, kSerial>);
+    case 96: return reinterpret_cast<void*>(gemm_tc_kernel<96, kF16, kExt, kSerial>);
+    case 112: return reinterpret_cast<void*>(gemm_tc_kernel<112, kF16, kExt, kSerial>);
+    case 128: return reinterpret_cast<void*>(gemm_tc_kernel<128, kF16, kExt, kSerial>);
     default: return nullptr;
   }
 }
@@ -537,6 +699,11 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
                  ? 1
                  : 0;
   p.aux_vec = g_gemm_direct_aux ? 0 : 1;
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  p.vec4_ok = (p.vec_ok && p.aux_vec && d.os_x % 4 == 0 && d.os_y % 4 == 0 && d.os_z % 4 == 0 &&
+               (d.out_half || d.out_plane % 4 == 0) && al16(d.out_f32) && al16(d.aux))
+                  ? 1
+                  : 0;
 
   // ---- numerics: 3-term split-bf16 (default) or single-plane fp16 operands (1 MMA per K step)
   const int planes = one_term ? 1 : 2;
@@ -557,8 +724,11 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
     FGT_REQUIRE(d.out_f32 && d.out_hi && p.vec_ok && d.N % 64 == 0 && (d.N / 2) % d.bn == 0 && d.groups == 1, FGT_ERR_ARG,
                 "gemm_tc: FGT_AUX_GRU_ZR needs both outputs, aligned unit-stride channels, N=%d a multiple of 64 and "
                 "bn=%d dividing N/2", d.N, d.bn);
-  void* kern = one_term ? (ext ? gemm_kernel_for<true, 1>(bn) : gemm_kernel_for<true, 0>(bn))
-                        : (ext ? gemm_kernel_for<false, 1>(bn) : gemm_kernel_for<false, 0>(bn));
+  void* kern = g_gemm_serial
+                   ? (one_term ? (ext ? gemm_kernel_for<true, 1, true>(bn) : gemm_kernel_for<true, 0, true>(bn))
+                               : (ext ? gemm_kernel_for<false, 1, true>(bn) : gemm_kernel_for<false, 0, true>(bn)))
+                   : (one_term ? (ext ? gemm_kernel_for<true, 1, false>(bn) : gemm_kernel_for<true, 0, false>(bn))
+                               : (ext ? gemm_kernel_for<false, 1, false>(bn) : gemm_kernel_for<false, 0, false>(bn)));
   FGT_REQUIRE(kern, FGT_ERR_ARG, "gemm_tc: no instantiation for a %d-wide tile", bn);
   // raised once per instantiation: the attribute is per kernel
   static std::mutex attr_mu;
@@ -590,5 +760,13 @@ extern "C" int fgt_gemm_tc(const FgtGemmDesc* desc, fgt_stream_t stream) {
 extern "C" int fgt_debug_gemm_direct_epilogue(int on) {
   fgt::g_gemm_direct_epilogue = (on & 1) != 0;
   fgt::g_gemm_direct_aux = (on & 2) != 0;
+  return FGT_OK;
+}
+
+// Debugging aid (not part of the product interface): nonzero selects the previous tile schedule for launches that
+// follow: no K stage of the next tile before a tile's epilogue, and the per-pair epilogue with its loads interleaved with
+// the stores. Same MMAs in the same order, so the outputs are bit-identical; one build can time both schedules.
+extern "C" int fgt_debug_gemm_serial_epilogue(int on) {
+  fgt::g_gemm_serial = on != 0;
   return FGT_OK;
 }
