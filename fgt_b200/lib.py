@@ -127,6 +127,17 @@ def load():
     for fn in (lib.fgt_binary_dilate, lib.fgt_fill_holes_init, lib.fgt_fill_holes_pass, lib.fgt_fill_holes_finish,
                lib.fgt_resize_nearest_u8, lib.fgt_resize_bilinear_f32):
         fn.restype = ctypes.c_int
+    lib.fgt_inpaint_telea_workspace.argtypes = [ci, ci, ci]
+    lib.fgt_inpaint_telea_workspace.restype = cll
+    lib.fgt_inpaint_telea.argtypes = [_c_p, _c_p, ci, ci, ci, ci, cll, cd_, _c_p, cll, _c_p, _c_p]
+    lib.fgt_inpaint_telea_plan.argtypes = [_c_p, ci, ci, ci, cd_, _c_p, cll, _c_p]
+    lib.fgt_inpaint_telea_fill.argtypes = [_c_p, ci, ci, ci, ci, ci, cd_, _c_p, cll, _c_p, _c_p]
+    lib.fgt_inpaint_telea_host.argtypes = [_c_p, _c_p, ci, ci, ci, cd_, _c_p]
+    lib.fgt_grad_prep_pre.argtypes = [_c_p, _c_p, ci, ci, ci, _c_p, _c_p]
+    lib.fgt_grad_prep_post.argtypes = [_c_p, _c_p, ci, ci, ci, _c_p, _c_p, _c_p]
+    for fn in (lib.fgt_inpaint_telea, lib.fgt_inpaint_telea_plan, lib.fgt_inpaint_telea_fill, lib.fgt_inpaint_telea_host,
+               lib.fgt_grad_prep_pre, lib.fgt_grad_prep_post):
+        fn.restype = ctypes.c_int
     lib.fgt_conv_tail.argtypes = [_c_p, cll, ci, ci, ci, ci, _c_p, cll, ci, ci, _c_p, ci, _c_p, cll, cll, cll, cll, _c_p]
     lib.fgt_conv_tail.restype = ctypes.c_int
     lib.fgt_swin_prep.argtypes = [_c_p, _c_p, ci, ci, ci, ci, ci, _c_p, ci, ci, ci, ci, ci, _c_p, _c_p, _c_p, _c_p, _c_p,

@@ -4,10 +4,12 @@ instead of directories, with every heavy stage on the GPU:
     frames, masks ──► RAFT flows (batched pairs) ──► flow diffusion (batched CG) + LAFC completion
                  ──► gradient propagation ──► Poisson blending (batched LSQR) ──► FGT windows + compositing
 
-Host-side remain exactly the calls the reference makes to third-party image code — `F.interpolate` of the input
-frames (:478-483), `cv2.resize` of flows and masks (:264-267,:544-546), `scipy.ndimage.binary_dilation /
-binary_fill_holes` (:549-561,:637-640) and `cv2.inpaint` (TELEA, :591-599,:663-671) — SURVEY §8f rank 3 lists
-their GPU equivalents as the next step. The stage implementations come from a backend object; `GpuBackend`
+The calls the reference makes to third-party image code run as device kernels when the backend provides them
+(`GpuBackend` does): `cv2.resize` of flows and masks (:264-267,:544-546), `scipy.ndimage.binary_dilation /
+binary_fill_holes` (:549-561,:637-640), and — with `GpuBackend(..., host_inpaint=False)` — `cv2.inpaint` (TELEA,
+:316-320,:591-599,:663-671, byte-identical, fgt_b200/inpaint.py) with the gradient preparation around it. By default
+TELEA stays on the host pool, where it is faster; the `F.interpolate` of the input frames (:478-483) is host-side
+too. The stage implementations come from a backend object; `GpuBackend`
 (default) binds the fgt_b200 modules, and the parity tests plug the CPU oracle into the same glue, so the glue
 itself is verified against a full run of the unmodified reference driver (tests/golden/pipeline_*.npz).
 There is no CPU fallback in this module: GpuBackend raises without a CUDA device.
@@ -23,6 +25,9 @@ import torch
 import torch.nn.functional as F
 
 HOST_THREADS = max(1, min(8, os.cpu_count() or 1))   # per-frame host work (TELEA, differences) runs on a small pool
+# GpuBackend keeps cv2.inpaint on the host pool unless built with host_inpaint=False: the device TELEA is byte-identical
+# but its serial planning made it slower than 8 cv2 threads at the driver's sizes on an H100 (DESIGN §8)
+HOST_INPAINT_DEFAULT = True
 
 
 def _frame_major(n, h, w, c=None, dtype=np.float32):
@@ -91,10 +96,11 @@ def load_clip(frames_u8, args, masks_u8=None):
     return torch.cat(video, 0), torch.cat(video_flow, 0)
 
 
-def extrapolate(video, flow_f, flow_b, h_scale, w_scale):
+def extrapolate(video, flow_f, flow_b, h_scale, w_scale, backend=None):
     """extrapolation (:286-335): a canvas H_scale x W_scale as large (rounded down to multiples of 4) with the clip in
-    the middle; the border is the hole. The frames are TELEA-inpainted into the border right away, the flows are
-    zero there. Returns (video, flow_f, flow_b, flow_mask [H',W'] bool, mask_dilated [H',W'] bool)."""
+    the middle; the border is the hole. The frames are TELEA-inpainted into the border right away (all frames in one
+    device batch with one shared mask when the backend has `inpaint_telea`), the flows are zero there.
+    Returns (video, flow_f, flow_b, flow_mask [H',W'] bool, mask_dilated [H',W'] bool)."""
     H, W, _, N = video.shape
     He, We = int(h_scale * H), int(w_scale * W)
     He, We = He - He % 4, We - We % 4
@@ -108,7 +114,12 @@ def extrapolate(video, flow_f, flow_b, h_scale, w_scale):
         big[:, :, :, i] = cv2.inpaint((big[:, :, :, i] * 255).astype(np.uint8), flow_mask.astype(np.uint8), 3,
                                       cv2.INPAINT_TELEA).astype(np.float32) / 255.0
 
-    _per_frame(fill, N)
+    if backend is not None and hasattr(backend, "inpaint_telea"):
+        frames = np.moveaxis(big, -1, 0)                                  # [N,He,We,3] view
+        done = backend.inpaint_telea((frames * 255).astype(np.uint8), flow_mask.astype(np.uint8))
+        frames[...] = done.astype(np.float32) / 255.0
+    else:
+        _per_frame(fill, N)
     ff = np.zeros((He, We, 2, N - 1), dtype=np.float32)
     fb = np.zeros((He, We, 2, N - 1), dtype=np.float32)
     ff[y0:y0 + H, x0:x0 + W] = flow_f
@@ -180,9 +191,12 @@ def complete_flows(backend, flows, flow_mask, mode, num_flows, flow_interval):
     return np.ascontiguousarray(np.transpose(out, (2, 3, 1, 0)))
 
 
-def prepare_gradients(video, mask, mask_dilated):
+def prepare_gradients(video, mask, mask_dilated, backend=None):
     """:583-614 — zero the hole (in place, like the driver), TELEA-inpaint it for a plausible initialisation, take
-    forward differences and zero them wherever they touch the hole. video [H,W,3,N] float32 (BGR, 0..1)."""
+    forward differences and zero them wherever they touch the hole. video [H,W,3,N] float32 (BGR, 0..1). A backend
+    with `prepare_gradients` runs the whole stage on the device (bit-identical)."""
+    if backend is not None and hasattr(backend, "prepare_gradients"):
+        return backend.prepare_gradients(video, mask, mask_dilated)
     H, W, _, N = video.shape
     gx = _frame_major(N, H, W, 3)                      # last column / row stay zero (:601-606)
     gy = _frame_major(N, H, W, 3)
@@ -233,13 +247,19 @@ def blend_frames(backend, video, gx, gy, mask, mask_gradient):
                 except Exception:  # noqa: BLE001
                     blends.append((video[:, :, :, i].astype(np.float64), mask[:, :, i].copy()))
     slot = {i: k for k, i in enumerate(todo)}
+    filled = None
+    if todo and hasattr(backend, "inpaint_telea"):       # every frame's leftover TELEA in one device batch
+        filled = backend.inpaint_telea(np.stack([(np.clip(b, 0, 1.0) * 255).astype(np.uint8) for b, _ in blends], 0),
+                                       np.stack([u.astype(np.uint8) for _, u in blends], 0))
 
     def finish(i):
         if i not in slot:
             return video[:, :, :, i]
         blend, unfilled = blends[slot[i]]
         blend = np.clip(blend, 0, 1.0)
-        tmp = cv2.inpaint((blend * 255).astype(np.uint8), unfilled.astype(np.uint8), 3, cv2.INPAINT_TELEA).astype(np.float32) / 255.0
+        u8 = filled[slot[i]] if filled is not None else \
+            cv2.inpaint((blend * 255).astype(np.uint8), unfilled.astype(np.uint8), 3, cv2.INPAINT_TELEA)
+        tmp = u8.astype(np.float32) / 255.0
         blend[unfilled, :] = tmp[unfilled, :]
         video[:, :, :, i] = blend
         mask[:, :, i] = unfilled
@@ -255,13 +275,15 @@ class GpuBackend:
     """Stage implementations on the fgt_b200 kernels. raft / lafc / fgt are the drop-in modules (already on the
     device, weights loaded); lafc_config provides num_flows / flow_interval like the driver's LAFC yaml."""
 
-    def __init__(self, raft, lafc, fgt, device=None, raft_batch=4):
+    def __init__(self, raft, lafc, fgt, device=None, raft_batch=4, host_inpaint=HOST_INPAINT_DEFAULT):
         if not torch.cuda.is_available():
             raise RuntimeError("fgt_b200.pipeline.GpuBackend needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.raft, self.lafc, self.fgt = raft, lafc, fgt
         self.fgt_model = fgt          # the callable the FGT stage evaluates per window (ShardedBackend swaps it)
         self.raft_batch = raft_batch
+        if not host_inpaint:          # opt-in: TELEA and the gradient preparation on the device (byte-identical)
+            self.inpaint_telea, self.prepare_gradients = self._inpaint_telea, self._prepare_gradients
 
     def raft_pairs(self, img1, img2, iters):
         outs = []
@@ -296,6 +318,15 @@ class GpuBackend:
         x = torch.as_tensor(flows).to(self.dev).permute(0, 2, 3, 1).contiguous()
         return morph.resize_bilinear(x, (H, W), channel_scale=(float(W) / float(w), float(H) / float(h)),
                                      device=self.dev).cpu().numpy()
+
+    def _inpaint_telea(self, images, masks):
+        """cv2.inpaint(..., 3, INPAINT_TELEA) of uint8 [B,H,W,3] with masks [B,H,W] or one [H,W] -> numpy uint8."""
+        from . import inpaint
+        return inpaint.inpaint_telea(images, masks, 3, device=self.dev).cpu().numpy()
+
+    def _prepare_gradients(self, video, mask, mask_dilated):
+        from . import inpaint
+        return inpaint.prepare_gradients(video, mask, mask_dilated, device=self.dev)
 
     def lafc_complete(self, flows, masks, diffused, triplets, pivot):
         fl, mk, df = (torch.from_numpy(a).to(self.dev).unsqueeze(0) for a in (flows, masks, diffused))   # [1,c,t,H,W]
@@ -360,7 +391,8 @@ class ShardedBackend:
 
     def __getattr__(self, name):
         # the mask / resize glue kernels are cheap and run replicated on every rank: delegate when the inner backend has them
-        if name in ("resize_masks", "dilate_masks", "fill_holes", "resize_flows") and hasattr(self.inner, name):
+        if name in ("resize_masks", "dilate_masks", "fill_holes", "resize_flows", "inpaint_telea", "prepare_gradients") \
+                and hasattr(self.inner, name):
             return getattr(self.inner, name)
         raise AttributeError(name)
 
@@ -487,14 +519,14 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
     assert video.dtype == np.float32
     if args.mode == "video_extrapolation":
         N = video.shape[3]
-        video, flow_f, flow_b, fm2, md2 = extrapolate(video, flow_f, flow_b, args.H_scale, args.W_scale)
+        video, flow_f, flow_b, fm2, md2 = extrapolate(video, flow_f, flow_b, args.H_scale, args.W_scale, backend)
         tile = lambda m: np.moveaxis(np.repeat(m[None], N, 0), 0, -1)           # the same mask for every frame (:531-535)
         mask, mask_dilated, flow_mask = tile(fm2), tile(md2), tile(fm2)
     else:
         mask, mask_dilated, flow_mask = prepare_masks(masks_u8, args, backend)
     done_f = complete_flows(backend, flow_f, flow_mask, "forward", num_flows, flow_interval)
     done_b = complete_flows(backend, flow_b, flow_mask, "backward", num_flows, flow_interval)
-    gx, gy = prepare_gradients(video, mask, mask_dilated)
+    gx, gy = prepare_gradients(video, mask, mask_dilated, backend)
     gx, gy, mask_gradient = backend.propagate(args, gx, gy, mask, mask_dilated, done_f, done_b)
     frame_blends = blend_frames(backend, video, gx, gy, mask, np.array(mask_gradient, dtype=bool))
     comp = backend.fgt_stage(frame_blends, mask, done_f, args.step, args.num_ref, args.neighbor_stride)

@@ -49,7 +49,8 @@ def models(H, W, seeds=(31, 32, 33), dev=dev):
     lafc = LAFCModel(dict(synth.CFG_LAFC)); lafc.load_state_dict(sds["lafc"]); lafc = lafc.to(dev)
     raft = RAFT(argparse.Namespace(small=False, mixed_precision=False, alternate_corr=False))
     raft.load_state_dict(sds["raft"]); raft = raft.to(dev).eval()
-    return PL.GpuBackend(raft, lafc, fgt, device=dev), sds
+    # --device-inpaint: the opt-in device TELEA and gradient preparation instead of cv2 on the host pool (A/B runs)
+    return PL.GpuBackend(raft, lafc, fgt, device=dev, host_inpaint="--device-inpaint" not in sys.argv), sds
 
 
 def run(N, H, W, reps):
