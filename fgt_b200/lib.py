@@ -138,6 +138,12 @@ def load():
     for fn in (lib.fgt_inpaint_telea, lib.fgt_inpaint_telea_plan, lib.fgt_inpaint_telea_fill, lib.fgt_inpaint_telea_host,
                lib.fgt_grad_prep_pre, lib.fgt_grad_prep_post):
         fn.restype = ctypes.c_int
+    lib.fgt_native_workspace.argtypes = [ci, ci, ci, ci]
+    lib.fgt_native_workspace.restype = cll
+    lib.fgt_native_count.argtypes = [_c_p, ci, ci, ci, ci, _c_p, cll, _c_p]
+    lib.fgt_native_composite.argtypes = [_c_p, ci, ci, ci, _c_p, ci, ci, ci, ci, ci, _c_p, cll, _c_p, _c_p]
+    for fn in (lib.fgt_native_count, lib.fgt_native_composite):
+        fn.restype = ctypes.c_int
     lib.fgt_conv_tail.argtypes = [_c_p, cll, ci, ci, ci, ci, _c_p, cll, ci, ci, _c_p, ci, _c_p, cll, cll, cll, cll, _c_p]
     lib.fgt_conv_tail.restype = ctypes.c_int
     lib.fgt_swin_prep.argtypes = [_c_p, _c_p, ci, ci, ci, ci, ci, _c_p, ci, ci, ci, ci, ci, _c_p, _c_p, _c_p, _c_p, _c_p,

@@ -13,6 +13,7 @@ too. The stage implementations come from a backend object; `GpuBackend`
 (default) binds the fgt_b200 modules, and the parity tests plug the CPU oracle into the same glue, so the glue
 itself is verified against a full run of the unmodified reference driver (tests/golden/pipeline_*.npz).
 There is no CPU fallback in this module: GpuBackend raises without a CUDA device.
+With `native=True` the result is returned at the input frames' size instead of the working size (fgt_b200/native.py).
 """
 import argparse
 import os
@@ -328,6 +329,12 @@ class GpuBackend:
         from . import inpaint
         return inpaint.prepare_gradients(video, mask, mask_dilated, device=self.dev)
 
+    def composite_native(self, comp, frames, masks, frame_dilates):
+        """The working-resolution result pasted into the input frames at their size (fgt_b200/native.py) -> numpy
+        uint8 [N,h,w,3]."""
+        from . import native
+        return native.composite_native(comp, frames, masks, frame_dilates, device=self.dev).cpu().numpy()
+
     def lafc_complete(self, flows, masks, diffused, triplets, pivot):
         fl, mk, df = (torch.from_numpy(a).to(self.dev).unsqueeze(0) for a in (flows, masks, diffused))   # [1,c,t,H,W]
         out = []
@@ -391,8 +398,8 @@ class ShardedBackend:
 
     def __getattr__(self, name):
         # the mask / resize glue kernels are cheap and run replicated on every rank: delegate when the inner backend has them
-        if name in ("resize_masks", "dilate_masks", "fill_holes", "resize_flows", "inpaint_telea", "prepare_gradients") \
-                and hasattr(self.inner, name):
+        if name in ("resize_masks", "dilate_masks", "fill_holes", "resize_flows", "inpaint_telea", "prepare_gradients",
+                    "composite_native") and hasattr(self.inner, name):
             return getattr(self.inner, name)
         raise AttributeError(name)
 
@@ -502,15 +509,45 @@ class ShardedBackend:
 
 
 # ------------------------------------------------------------------------------------------------ driver
-def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_interval=3, return_stages=False):
+def _check_native(frames_u8, masks_u8, backend, args):
+    if args.mode == "video_extrapolation":
+        raise ValueError("native=True: video_extrapolation has no original frame to paste the result into")
+    if not hasattr(backend, "composite_native"):
+        raise TypeError(f"native=True needs a backend with composite_native ({type(backend).__name__} has none)")
+    sizes = {np.asarray(f).shape[:2] for f in frames_u8}
+    if len(sizes) != 1:
+        raise ValueError(f"native=True needs frames of one size (got {sorted(sizes)})")
+    (hw,) = sizes
+    bad = [np.asarray(m).shape for m in masks_u8 if np.asarray(m).shape[:2] != hw]
+    if bad or len(masks_u8) != len(frames_u8):
+        raise ValueError(f"native=True: {len(masks_u8)} masks for {len(frames_u8)} frames of {hw}"
+                         + (f"; mask sizes {bad[:3]}" if bad else ""))
+
+
+def composite_native(backend, comp, frames_u8, masks_u8, args):
+    """The working-resolution frames `comp` upscaled to the input size and pasted into the input frames as given (with
+    the watermark in watermark_removal) inside a feathered band around the mask (fgt_b200/native.py). Returns a list of
+    N uint8 RGB frames [h,w,3]."""
+    out = backend.composite_native(np.stack(comp), np.stack([np.asarray(f) for f in frames_u8]),
+                                   np.stack([np.asarray(m) for m in masks_u8]), args.frame_dilates)
+    return list(np.asarray(out))
+
+
+def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_interval=3, return_stages=False,
+                     native=False):
     """The driver on arrays: frames_u8 [N,h,w,3] RGB uint8 (the PNGs the driver reads), masks_u8 [N,h,w] (non-zero =
     remove; ignored by video_extrapolation) -> list of N uint8 RGB frames (what the driver writes to result.mp4).
     `args`: make_args(...), `args.mode` one of object_removal (default), watermark_removal (frames are masked before
     resizing, :454-473), video_extrapolation (the clip is placed in a larger canvas whose border is inpainted,
-    :516-537); num_flows / flow_interval are the LAFC config entries the driver reads (:352)."""
+    :516-537); num_flows / flow_interval are the LAFC config entries the driver reads (:352).
+    native=True returns the frames at the input size h x w instead of imgH x imgW: the result is upscaled and pasted
+    into the input frames around the mask by `backend.composite_native` (object and watermark removal; every frame and
+    mask of one size). With return_stages the working-resolution frames are then in stages["comp"]."""
     args = args or make_args()
     if args.mode not in MODES:
         raise ValueError(f"Accepted modes: {MODES}, but input is {args.mode}")
+    if native:
+        _check_native(frames_u8, masks_u8, backend, args)
     video, video_flow = load_clip(frames_u8, args, masks_u8 if args.mode == "watermark_removal" else None)
     flow_f = compute_flows(backend, video_flow, args, "forward")
     flow_b = compute_flows(backend, video_flow, args, "backward")
@@ -530,10 +567,14 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
     gx, gy, mask_gradient = backend.propagate(args, gx, gy, mask, mask_dilated, done_f, done_b)
     frame_blends = blend_frames(backend, video, gx, gy, mask, np.array(mask_gradient, dtype=bool))
     comp = backend.fgt_stage(frame_blends, mask, done_f, args.step, args.num_ref, args.neighbor_stride)
+    out = composite_native(backend, comp, frames_u8, masks_u8, args) if native else comp
     if return_stages:
-        return comp, dict(flow_f=flow_f, flow_b=flow_b, done_f=done_f, done_b=done_b, mask_gradient=mask_gradient,
-                          frame_blends=np.stack(frame_blends), mask=mask)
-    return comp
+        stages = dict(flow_f=flow_f, flow_b=flow_b, done_f=done_f, done_b=done_b, mask_gradient=mask_gradient,
+                      frame_blends=np.stack(frame_blends), mask=mask)
+        if native:
+            stages["comp"] = np.stack(comp)
+        return out, stages
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ command line
@@ -582,12 +623,17 @@ def main(argv=None):
     ap.add_argument("--lafc_ckpts", default="../LAFC/checkpoint")
     ap.add_argument("--fgt_ckpts", default="../FGT/checkpoint")
     ap.add_argument("--gpu", type=int, default=0)
+    ap.add_argument("--native", action="store_true",
+                    help="write the frames at the input size: the result is upscaled and pasted into the input frames "
+                         "around the mask (object_removal, watermark_removal)")
     for k, v in DEFAULTS.items():
         if k == "mode":
             ap.add_argument("--mode", default=v, choices=list(MODES))
         elif k not in ("Nonlocal", "raft_iters"):
             ap.add_argument("--" + k, type=type(v), default=v)
     ns = ap.parse_args(argv)
+    if ns.native and ns.mode == "video_extrapolation":
+        ap.error("--native: video_extrapolation has no original frame to paste the result into")
     dev = torch.device("cuda", ns.gpu)
     backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev)
     args = make_args(**{k: getattr(ns, k) for k in DEFAULTS if hasattr(ns, k)})
@@ -595,7 +641,8 @@ def main(argv=None):
     masks = IO.read_masks(ns.path_mask, rgb=ns.mode == "watermark_removal") if ns.mode != "video_extrapolation" else [None] * len(frames)
     if len(frames) != len(masks):
         raise ValueError(f"{len(frames)} frames but {len(masks)} masks")
-    comp = video_inpainting(frames, masks, backend, args, lafc_cfg["num_flows"], lafc_cfg["flow_interval"])
+    comp = video_inpainting(frames, masks, backend, args, lafc_cfg["num_flows"], lafc_cfg["flow_interval"],
+                            native=ns.native)
     written = IO.write_frames(ns.outroot, comp)
     print(f"Done, {len(comp)} frames written to {ns.outroot} ({len(written)} files)")
     return comp

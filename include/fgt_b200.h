@@ -375,6 +375,27 @@ int fgt_grad_prep_pre(const float* video, const unsigned char* mask, int B, int 
 int fgt_grad_prep_post(const unsigned char* u8, const unsigned char* mask_dilated, int B, int H, int W, float* gx,
                        float* gy, fgt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Native-resolution output (definition: oracle/native_oracle.py; bit-identical to it, integer arithmetic only). The
+ * pipeline's working-resolution result comp uint8 [B,cH,cW,3] is upscaled to the frames' size H x W with cv2's
+ * fixed-point INTER_LINEAR and blended into the original frames uint8 [B,H,W,3] with weight c / A, where c counts the
+ * pixels of the dilated hole D in the (2k+1) x (2k+1) window around the pixel (the edge replicated outside the image)
+ * and A = (2k+1)^2,
+ * k = ceil(max(H / cH, W / cW)). D is the hole cross-dilated r + 2k times (fgt_binary_dilate).
+ *   fgt_native_workspace  bytes of workspace for the counts of n_masks masks of H x W (negative FGT_ERR_* when a size
+ *                         is empty or A does not fit the uint16 count, i.e. k outside [1, 127]).
+ *   fgt_native_count      c of the dilated masks [n_masks,H,W] (0 / non-zero) into the workspace: two separable box sums.
+ *   fgt_native_composite  out uint8 [B,H,W,3] from comp, frames and the counts in the workspace: one count per frame, or
+ *                         count 0 for every frame when shared_mask != 0. C must be 3; k must be the window of comp's
+ *                         size and the frames' size; out must not alias comp or frames.
+ * ------------------------------------------------------------------------------------------ */
+long long fgt_native_workspace(int n_masks, int H, int W, int k);
+int fgt_native_count(const unsigned char* dilated, int n_masks, int H, int W, int k, void* workspace,
+                     long long workspace_bytes, fgt_stream_t stream);
+int fgt_native_composite(const unsigned char* comp, int B, int cH, int cW, const unsigned char* frames, int H, int W,
+                         int C, int shared_mask, int k, const void* workspace, long long workspace_bytes,
+                         unsigned char* out, fgt_stream_t stream);
+
 /* 3x3 convolution (zero padding 1, stride 1) with cout <= 3 output channels + bias + activation in one kernel: the
  * nine taps become the N dimension of a wgmma GEMM over the input positions (activation read once) and are summed
  * per output pixel in shared memory — the decoder's final conv + tanh (FGT/models/model.py:185-193). x: NHWC
