@@ -88,6 +88,10 @@ __device__ __forceinline__ float act_one(float v, int act) {
   }
 }
 
+// Nearest fp16 value, as fp32. Mixed-precision RAFT (out_half): the fp32 copy of an output equals its fp16 output, as
+// autocast's fp16 tensors do.
+__device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
+
 __device__ __forceinline__ void load_pair(const float* src, long long o0, long long o1, bool two, bool vec, float& x0,
                                           float& x1) {
   if (vec) {
@@ -115,6 +119,10 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
     v0 += a0;
     v1 += a1;
   }
+  if (kExt && e.out_half) {  // mixed precision: the conv's output is an fp16 tensor before its activation (autocast)
+    v0 = round_f16(v0);
+    v1 = round_f16(v1);
+  }
   if (kExt) {
     v0 = act_one(v0, e.act);
     v1 = act_one(v1, e.act);
@@ -125,10 +133,19 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
     v0 = act_one(v0, e.act);
     v1 = act_one(v1, e.act);
   }
+  if (kExt && e.out_half && (e.aux_mode == FGT_AUX_GRU_ZR || e.aux_mode == FGT_AUX_GRU)) {
+    // mixed-precision GRU (update.py:45-60 under autocast): the gates z, r and the candidate q are fp16
+    v0 = round_f16(v0);
+    v1 = round_f16(v1);
+  }
   if (kExt && e.aux_mode == FGT_AUX_GRU_ZR) {  // fused z | r gates: two C-channel outputs (host guarantees vec)
     const int half = e.N >> 1;
     if (col < half) {
       *reinterpret_cast<float2*>(e.out_f32 + o0) = make_float2(v0, v1);
+    } else if (e.out_half) {  // r * h as the fp16 operand of the q conv
+      const long long o = off + (col - half);
+      load_pair(e.aux, o, o + 1, true, e.aux_vec != 0, a0, a1);
+      *reinterpret_cast<uint32_t*>(e.out_hi + o) = pack_f16x2(v0 * a0, v1 * a1);
     } else {
       const long long o = off + (col - half);
       load_pair(e.aux, o, o + 1, true, e.aux_vec != 0, a0, a1);
@@ -149,14 +166,27 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
     v1 *= a1;
   } else if (kExt && e.aux_mode == FGT_AUX_ADD_RELU) {
     load_pair(e.aux, o0, o1, two, avec, a0, a1);
+    if (e.out_half) {  // mixed precision: act(v) is an fp16 tensor before the residual add (RAFT/extractor.py:55-56)
+      v0 = round_f16(v0);
+      v1 = round_f16(v1);
+    }
     v0 = fmaxf(v0 + a0, 0.f);
     v1 = fmaxf(v1 + a1, 0.f);
   } else if (kExt && e.aux_mode == FGT_AUX_GRU) {  // h' = (1 - z) * h + z * q   (aux = h, aux2 = z, v = q)
     float z0, z1;
     load_pair(e.aux, o0, o1, two, avec, a0, a1);
     load_pair(e.aux2, o0, o1, two, avec, z0, z1);
-    v0 = (1.f - z0) * a0 + z0 * v0;
-    v1 = (1.f - z1) * a1 + z1 * v1;
+    if (e.out_half) {  // mixed precision: each of the four fp16 tensor ops of update.py:52,58 rounds to fp16
+      v0 = round_f16(round_f16(round_f16(1.f - z0) * a0) + round_f16(z0 * v0));
+      v1 = round_f16(round_f16(round_f16(1.f - z1) * a1) + round_f16(z1 * v1));
+    } else {
+      v0 = (1.f - z0) * a0 + z0 * v0;
+      v1 = (1.f - z1) * a1 + z1 * v1;
+    }
+  }
+  if (kExt && e.out_half) {  // the fp32 copy (a residual or GRU-state operand) holds the same fp16 value as the 16-bit output
+    v0 = round_f16(v0);
+    v1 = round_f16(v1);
   }
   if (vec) {
     if (e.out_f32) *reinterpret_cast<float2*>(e.out_f32 + o0) = make_float2(v0, v1);
@@ -718,8 +748,10 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   p.stages = stages;
   const size_t smem = static_cast<size_t>(stages) * stage_bytes + fixed;
 
+  // out_half with an fp32 copy (mixed-precision RAFT): the fp16 rounding before the activation and of the fp32 copy lives
+  // in the kExt = 1 epilogue, so the common instantiation keeps the previous code
   const bool ext = d.aux_mode == FGT_AUX_ADD_PRE || d.aux_mode == FGT_AUX_ADD_RELU || d.aux_mode == FGT_AUX_GRU ||
-                   d.aux_mode == FGT_AUX_GRU_ZR || d.act == FGT_ACT_LEAKY001;
+                   d.aux_mode == FGT_AUX_GRU_ZR || d.act == FGT_ACT_LEAKY001 || (d.out_half && d.out_f32);
   if (d.aux_mode == FGT_AUX_GRU_ZR)
     FGT_REQUIRE(d.out_f32 && d.out_hi && p.vec_ok && d.N % 64 == 0 && (d.N / 2) % d.bn == 0 && d.groups == 1, FGT_ERR_ARG,
                 "gemm_tc: FGT_AUX_GRU_ZR needs both outputs, aligned unit-stride channels, N=%d a multiple of 64 and "

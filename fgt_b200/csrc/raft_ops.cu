@@ -66,7 +66,9 @@ __global__ void __launch_bounds__(512) chan_stats_kernel(const float* __restrict
   }
 }
 
-// y = (x - mean) * rstd ; optional ReLU ; optional residual: y = relu(y + res). fp32 and/or split out.
+// y = (x - mean) * rstd ; optional ReLU ; optional residual: y = relu(y + res). fp32 and/or 16-bit out: split-bf16,
+// or single-plane fp16 rows when plane == 0 (mixed-precision RAFT: the fp32 copy then holds the same fp16 values, the
+// residual operand of a later block being an fp16 tensor under autocast).
 // grid.y = image; per-channel scale / shift are derived once per block from the double statistics.
 __global__ void instnorm_act_kernel(const float* __restrict__ x, const double* __restrict__ stats, int HW, int C,
                                     float eps, int relu, const float* __restrict__ res, float* __restrict__ out,
@@ -99,13 +101,24 @@ __global__ void instnorm_act_kernel(const float* __restrict__ x, const double* _
 #pragma unroll
       for (int j = 0; j < 4; ++j) o[j] = fmaxf(o[j], 0.f);
     }
+    const bool f16 = hi && plane == 0;
     if (res) {
+      if (f16) {  // relu(norm(x)) is an fp16 tensor before the residual add (extractor.py:55-56)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) o[j] = __half2float(__float2half_rn(o[j]));
+      }
       const float4 r = __ldg(reinterpret_cast<const float4*>(res + off));
       o[0] = fmaxf(o[0] + r.x, 0.f); o[1] = fmaxf(o[1] + r.y, 0.f);
       o[2] = fmaxf(o[2] + r.z, 0.f); o[3] = fmaxf(o[3] + r.w, 0.f);
     }
+    if (f16) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) o[j] = __half2float(__float2half_rn(o[j]));
+    }
     if (out) *reinterpret_cast<float4*>(out + off) = make_float4(o[0], o[1], o[2], o[3]);
-    if (hi) {
+    if (f16) {
+      *reinterpret_cast<uint2*>(hi + off) = make_uint2(pack_f16x2(o[0], o[1]), pack_f16x2(o[2], o[3]));
+    } else if (hi) {
       uint32_t h0, l0, h1, l1;
       split_bf16x2(o[0], o[1], h0, l0);
       split_bf16x2(o[2], o[3], h1, l1);
@@ -139,7 +152,7 @@ __global__ void avgpool2_kernel(const float* __restrict__ in, long long rows, in
 // coords/2^level with zero padding and align_corners=True pixel coordinates. All window points share
 // the fractional offset, so a (2r+2)^2 patch is staged once per (pixel, level) in shared memory.
 // Window index a (first) offsets x, b (second) offsets y — the reference's meshgrid(dy, dx) stacking.
-// Output: split-bf16 [n_pix, out_pitch], channel = level*(2r+1)^2 + a*(2r+1) + b.
+// Output: split-bf16 [n_pix, out_pitch], channel = level*(2r+1)^2 + a*(2r+1) + b; single-plane fp16 when plane == 0.
 // ------------------------------------------------------------------------------------------
 struct LookupLevels {
   const float* ptr[4];
@@ -180,11 +193,15 @@ __global__ void corr_lookup_kernel(LookupLevels lv, int levels, int radius, cons
       const int a = o / win, b = o - a * win;  // a -> x offset, b -> y offset
       const float v = w00 * patch[b * pw + a] + w01 * patch[b * pw + a + 1] + w10 * patch[(b + 1) * pw + a] +
                       w11 * patch[(b + 1) * pw + a + 1];
-      __nv_bfloat16 hh, ll;
-      split_bf16(v, hh, ll);
       const long long off = static_cast<long long>(p) * out_pitch + l * win * win + o;
-      hi[off] = hh;
-      hi[plane + off] = ll;
+      if (plane == 0) {  // single-plane fp16 row (input of a 1-term convc1)
+        reinterpret_cast<__half*>(hi)[off] = __float2half_rn(v);
+      } else {
+        __nv_bfloat16 hh, ll;
+        split_bf16(v, hh, ll);
+        hi[off] = hh;
+        hi[plane + off] = ll;
+      }
     }
     __syncwarp();
   }
@@ -193,26 +210,36 @@ __global__ void corr_lookup_kernel(LookupLevels lv, int levels, int radius, cons
 // ------------------------------------------------------------------------------------------
 // coords1 += delta (raft.py:132); emits flow = coords1 - coords0 (coords0 = pixel grid, raft.py:64-71)
 // as NCHW fp32 (input of the 7x7 flow conv) and as the last two channels of the GRU input buffer x.
+// x_plane == 0: x is single-plane fp16 (mixed precision), the flow channels are stored as fp16. delta_f16: delta is
+// the flow head's output, an fp16 tensor under autocast, so it is rounded to fp16 before the fp32 add (raft.py:132).
 // ------------------------------------------------------------------------------------------
-__global__ void flow_update_kernel(float* __restrict__ coords, const float* __restrict__ delta, int n_img, int h,
-                                   int w, float* __restrict__ flow_nchw, __nv_bfloat16* __restrict__ x_hi,
+__device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
+
+__global__ void flow_update_kernel(float* __restrict__ coords, const float* __restrict__ delta, int delta_f16, int n_img,
+                                   int h, int w, float* __restrict__ flow_nchw, __nv_bfloat16* __restrict__ x_hi,
                                    long long x_plane, int x_pitch, int x_chan) {
   pdl_launch_dependents();
   pdl_wait();
   const int n = h * w;
+  const bool f16 = x_hi && x_plane == 0;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n_img * n; p += gridDim.x * blockDim.x) {
     const int img = p / n, q = p - img * n;
     float cx = coords[2 * p], cy = coords[2 * p + 1];
     if (delta) {
-      cx += delta[2 * p];
-      cy += delta[2 * p + 1];
+      const float dx = delta[2 * p], dy = delta[2 * p + 1];
+      cx += delta_f16 ? round_f16(dx) : dx;
+      cy += delta_f16 ? round_f16(dy) : dy;
       coords[2 * p] = cx;
       coords[2 * p + 1] = cy;
     }
     const float fx = cx - static_cast<float>(q % w), fy = cy - static_cast<float>(q / w);
     flow_nchw[static_cast<long long>(img) * 2 * n + q] = fx;
     flow_nchw[static_cast<long long>(img) * 2 * n + n + q] = fy;
-    if (x_hi) {
+    if (f16) {
+      __half* xh = reinterpret_cast<__half*>(x_hi) + static_cast<long long>(p) * x_pitch + x_chan;
+      xh[0] = __float2half_rn(fx);
+      xh[1] = __float2half_rn(fy);
+    } else if (x_hi) {
       __nv_bfloat16 h0, l0, h1, l1;
       split_bf16(fx, h0, l0);
       split_bf16(fy, h1, l1);
@@ -220,6 +247,31 @@ __global__ void flow_update_kernel(float* __restrict__ coords, const float* __re
       x_hi[off] = h0; x_hi[off + 1] = h1;
       x_hi[x_plane + off] = l0; x_hi[x_plane + off + 1] = l1;
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// fp16 -> split-bf16, exactly: an fp16 value has 11 significant bits, bf16 hi takes the top 8 and the residual (at most
+// 4 bits, far above bf16's smallest normal) is exact in bf16 lo. Mixed-precision RAFT stores the feature net's output as
+// fp16, as autocast does, and the 3-term correlation GEMM then computes the reference's fp32 correlation of those values
+// (fmap.float(), raft.py:103-104). 8 elements per thread, 16-byte accesses.
+// ------------------------------------------------------------------------------------------
+__global__ void f16_to_split_kernel(const __half* __restrict__ src, long long n8, __nv_bfloat16* __restrict__ hi,
+                                    long long plane) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(src) + i);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t hw[4], lw[4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[t]));
+      split_bf16x2(f.x, f.y, hw[t], lw[t]);
+    }
+    reinterpret_cast<uint4*>(hi)[i] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+    reinterpret_cast<uint4*>(hi + plane)[i] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
   }
 }
 
@@ -330,11 +382,24 @@ extern "C" int fgt_corr_lookup(const float* const* level_ptrs_host, const int* l
   return FGT_OK;
 }
 
-extern "C" int fgt_raft_flow_update(float* coords, const float* delta, int n, int h, int w, float* flow_nchw,
-                                    void* x_hi, long long x_plane, int x_pitch, int x_chan, fgt_stream_t stream) {
+extern "C" int fgt_raft_flow_update(float* coords, const float* delta, int delta_f16, int n, int h, int w,
+                                    float* flow_nchw, void* x_hi, long long x_plane, int x_pitch, int x_chan,
+                                    fgt_stream_t stream) {
   FGT_REQUIRE(coords && flow_nchw && n >= 1, FGT_ERR_ARG, "raft_flow_update: null argument");
+  FGT_REQUIRE(delta_f16 == 0 || delta_f16 == 1, FGT_ERR_ARG, "raft_flow_update: delta_f16=%d (0 or 1)", delta_f16);
   launch_k(flow_update_kernel, dim3(grid_cap(static_cast<long long>(n) * h * w, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      coords, delta, n, h, w, flow_nchw, reinterpret_cast<__nv_bfloat16*>(x_hi), x_plane, x_pitch, x_chan);
+      coords, delta, delta_f16, n, h, w, flow_nchw, reinterpret_cast<__nv_bfloat16*>(x_hi), x_plane, x_pitch, x_chan);
+  FGT_CUDA(cudaGetLastError());
+  return FGT_OK;
+}
+
+extern "C" int fgt_f16_to_split(const void* src, long long n, void* out_hi, long long out_plane, fgt_stream_t stream) {
+  const auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  FGT_REQUIRE(src && out_hi && n >= 0 && n % 8 == 0 && out_plane % 8 == 0 && out_plane >= n && al16(src) && al16(out_hi),
+              FGT_ERR_ARG, "f16_to_split: n=%lld plane=%lld (multiples of 8, 16-byte aligned buffers)", n, out_plane);
+  if (n == 0) return FGT_OK;
+  launch_k(f16_to_split_kernel, dim3(grid_cap(n / 8, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
+      reinterpret_cast<const __half*>(src), n / 8, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }

@@ -164,10 +164,11 @@ def load():
     lib.fgt_avgpool2.argtypes = [_c_p, cll, ci, ci, _c_p, _c_p]
     lib.fgt_corr_lookup.argtypes = [ctypes.POINTER(_c_p), ctypes.POINTER(ci), ctypes.POINTER(ci), ci, ci, _c_p, ci,
                                     ci, _c_p, cll, _c_p]
-    lib.fgt_raft_flow_update.argtypes = [_c_p, _c_p, ci, ci, ci, _c_p, _c_p, cll, ci, ci, _c_p]
+    lib.fgt_raft_flow_update.argtypes = [_c_p, _c_p, ci, ci, ci, ci, _c_p, _c_p, cll, ci, ci, _c_p]
     lib.fgt_convex_upsample.argtypes = [_c_p, _c_p, ci, ci, ci, _c_p, _c_p]
+    lib.fgt_f16_to_split.argtypes = [_c_p, cll, _c_p, cll, _c_p]
     for fn in (lib.fgt_chan_stats, lib.fgt_instnorm_act, lib.fgt_avgpool2, lib.fgt_corr_lookup,
-               lib.fgt_raft_flow_update, lib.fgt_convex_upsample):
+               lib.fgt_raft_flow_update, lib.fgt_convex_upsample, lib.fgt_f16_to_split):
         fn.restype = ctypes.c_int
     lib.fgt_prop_step.argtypes = [_c_p, _c_p, _c_p, ci, ci, ci, ci, cd, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]
     lib.fgt_prop_gather.argtypes = [_c_p, _c_p, _c_p, _c_p, ci, ci, ci, ci, _c_p, _c_p, _c_p]
@@ -518,11 +519,17 @@ def chan_stats(x, n, HW, C, stats, tag=""):
         check(load().fgt_chan_stats(_dp(x), n, HW, C, _dp(stats), stream_ptr()), "fgt_chan_stats")
 
 
+def _plane16(t):
+    """Plane offset of a 16-bit kernel output: 0 selects single-plane fp16 (a torch.float16 tensor), otherwise the
+    split-bf16 lo-plane offset."""
+    return 0 if t is None or t.dtype == torch.float16 else plane_elems(t)
+
+
 def instnorm_act(x, stats, n, HW, C, *, relu=True, res=None, out=None, out_split=None, eps=1e-5, tag=""):
+    """out_split: split-bf16 [2, ...] or a plain fp16 tensor (single-plane rows of a 1-term layer)."""
     with _Prof("instnorm_act", tag, 0, 4.0 * n * HW * C * (3 if res is not None else 2)):
         check(load().fgt_instnorm_act(_dp(x), _dp(stats), n, HW, C, eps, 1 if relu else 0, _dp(res), _dp(out),
-                                      _dp(out_split), plane_elems(out_split) if out_split is not None else 0,
-                                      stream_ptr()), "fgt_instnorm_act")
+                                      _dp(out_split), _plane16(out_split), stream_ptr()), "fgt_instnorm_act")
 
 
 def avgpool2(src, rows, h, w, dst, tag=""):
@@ -531,7 +538,7 @@ def avgpool2(src, rows, h, w, dst, tag=""):
 
 
 def corr_lookup(levels, coords, n_pix, radius, out_split, tag=""):
-    """levels: list of fp32 tensors [n_pix, h_l, w_l]; out_split: [2, n_pix, pitch]."""
+    """levels: list of fp32 tensors [n_pix, h_l, w_l]; out_split: split-bf16 [2, n_pix, pitch] or fp16 [n_pix, pitch]."""
     nl = len(levels)
     ptrs = (_c_p * nl)(*[t.data_ptr() for t in levels])
     hs = (ctypes.c_int * nl)(*[t.shape[1] for t in levels])
@@ -539,13 +546,15 @@ def corr_lookup(levels, coords, n_pix, radius, out_split, tag=""):
     win = 2 * radius + 1
     with _Prof("corr_lookup", tag, 0, 4.0 * n_pix * nl * ((win + 1) ** 2 + win * win)):
         check(load().fgt_corr_lookup(ptrs, hs, ws, nl, radius, _dp(coords), n_pix, out_split.shape[-1],
-                                     _dp(out_split), plane_elems(out_split), stream_ptr()), "fgt_corr_lookup")
+                                     _dp(out_split), _plane16(out_split), stream_ptr()), "fgt_corr_lookup")
 
 
-def raft_flow_update(coords, delta, h, w, flow_nchw, x_split=None, x_chan=0, n=1, tag=""):
+def raft_flow_update(coords, delta, h, w, flow_nchw, x_split=None, x_chan=0, n=1, delta_f16=False, tag=""):
+    """x_split: split-bf16 GRU input, or fp16 for the mixed-precision path; delta_f16: round delta to fp16 first."""
     with _Prof("raft_flow_update", tag, 0, 32.0 * n * h * w):
-        check(load().fgt_raft_flow_update(_dp(coords), _dp(delta), n, h, w, _dp(flow_nchw), _dp(x_split),
-                                          plane_elems(x_split) if x_split is not None else 0,
+        check(load().fgt_raft_flow_update(_dp(coords), _dp(delta), 1 if delta_f16 else 0, n, h, w, _dp(flow_nchw),
+                                          _dp(x_split),
+                                          _plane16(x_split),
                                           x_split.shape[-1] if x_split is not None else 0, x_chan, stream_ptr()),
               "fgt_raft_flow_update")
 
@@ -554,3 +563,10 @@ def convex_upsample(mask, flow_nchw, h, w, out, n=1, tag=""):
     with _Prof("convex_upsample", tag, 0, 4.0 * n * h * w * (576 + 128)):
         check(load().fgt_convex_upsample(_dp(mask), _dp(flow_nchw), n, h, w, _dp(out), stream_ptr()),
               "fgt_convex_upsample")
+
+
+def f16_to_split(src, out_split, tag=""):
+    """fp16 tensor -> split-bf16 [2, ...] of the same element count (exact)."""
+    with _Prof("f16_to_split", tag, 0, 6.0 * src.numel()):
+        check(load().fgt_f16_to_split(_dp(src), src.numel(), _dp(out_split), plane_elems(out_split), stream_ptr()),
+              "fgt_f16_to_split")

@@ -44,22 +44,26 @@ def fill_sms(bn, n_total, m_positions, groups=1, n_sms=132):
     return bn
 
 
-def packed(name, weight, bias, dev, seg_counts=None, im2col_pad=None):
-    """Weight record consumed by conv()/linear(): split-bf16 packed weight + fp32 bias."""
+def packed(name, weight, bias, dev, seg_counts=None, im2col_pad=None, half=False):
+    """Weight record consumed by conv()/linear(): split-bf16 packed weight + fp32 bias. half=True: a 1-term layer,
+    fp16 packed weight (its A operands and 16-bit outputs are single-plane fp16 tensors)."""
     if im2col_pad is not None:
-        w = pack_weight_im2col(weight, im2col_pad)
+        w = pack_weight_im2col(weight, im2col_pad, half=half)
     else:
-        w = pack_weight(weight, seg_counts)
-    return dict(w=w.to(dev), b=bias.detach().float().contiguous().to(dev), N=weight.shape[0], name=name)
+        w = pack_weight(weight, seg_counts, half=half)
+    rec = dict(w=w.to(dev), b=bias.detach().float().contiguous().to(dev), N=weight.shape[0], name=name)
+    if half:
+        rec["terms"] = 1
+    return rec
 
 
 def conv(xs, wp, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad_y=0, pad_z=0, out_z=None, act=lib.ACT_LEAKY02,
          out_split=None, out_f32=None, aux=None, aux_mode=lib.AUX_NONE, groups=1, seg_counts=None, nchw_out=False,
-         alpha=1.0, aux2=None, out_c_total=None, out_c_offset=0):
-    """xs: list of (split tensor [2, Z, Y, X, C], C) sharing Z/Y/X. Output NHWC [Z', Y', X', N]
-    (or NCHW fp32 when nchw_out). Returns (oz, oy, ox)."""
+         alpha=1.0, aux2=None, out_c_total=None, out_c_offset=0, out_f16=None):
+    """xs: list of (split tensor [2, Z, Y, X, C], C) sharing Z/Y/X, or of fp16 tensors [Z, Y, X, C] for a 1-term
+    layer (wp["terms"] == 1). Output NHWC [Z', Y', X', N] (or NCHW fp32 when nchw_out). Returns (oz, oy, ox)."""
     x0, c0 = xs[0]
-    Z, Y, X = x0.shape[1], x0.shape[2], x0.shape[3]
+    Z, Y, X = x0.shape[-4], x0.shape[-3], x0.shape[-2]
     oy = (Y + 2 * pad_y - dil * (ky - 1) - 1) // stride + 1
     ox = (X + 2 * pad_x - dil * (kx - 1) - 1) // stride + 1
     oz = (Z + 2 * pad_z - (kz - 1)) if out_z is None else out_z
@@ -78,12 +82,13 @@ def conv(xs, wp, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad_y=0, pad_z=0
                 groups=groups, out_w=ox, out_h=oy, out_z=oz, box_w=bw, box_h=bh,
                 bn=fill_sms(pick_bn(N // groups, groups), N, ox * oy * oz, groups),
                 bias=wp["b"], alpha=alpha, act=act, aux=aux, aux_mode=aux_mode, aux2=aux2, out_f32=out_f32, out_split=out_split,
-                tag=wp["name"], **strides)
+                tag=wp["name"], terms=wp.get("terms", 3), out_f16=out_f16, **strides)
     return oz, oy, ox
 
 
 def linear(segs, wp, rows, **kw):
-    """segs: list of (split tensor [2, rows, C], C). Row-major [rows, N] outputs."""
+    """segs: list of (split tensor [2, rows, C], C), or of fp16 [rows, C] for a 1-term layer. Row-major [rows, N]
+    outputs."""
     asegs = [lib.ASeg(t, c, rows) for t, c in segs]
     lib.gemm_tc(asegs, wp["w"], wp["N"], out_w=rows, bn=fill_sms(pick_bn(wp["N"], 1), wp["N"], rows),
-                bias=wp["b"], tag=wp["name"], **kw)
+                bias=wp["b"], tag=wp["name"], terms=wp.get("terms", 3), **kw)

@@ -578,10 +578,11 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
 
 
 # ------------------------------------------------------------------------------------------------ command line
-def load_models(raft_model, lafc_ckpts, fgt_ckpts, device):
+def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False):
     """initialize_RAFT / initialize_LAFC / initialize_FGT (:186-230) with the drop-in modules: the same checkpoint
     layout (a `module.`-prefixed RAFT state dict; directories holding one *.tar with `model_state_dict` and one
-    *.yaml config). Returns (GpuBackend, lafc_config)."""
+    *.yaml config). mixed_precision: RAFT's fp16 mode (the reference's --mixed_precision). Returns
+    (GpuBackend, lafc_config)."""
     import glob
     import os
 
@@ -598,7 +599,8 @@ def load_models(raft_model, lafc_ckpts, fgt_ckpts, device):
         with open(yamls[0]) as fh:
             return torch.load(tars[0], map_location="cpu")["model_state_dict"], yaml.full_load(fh)
 
-    raft = torch.nn.DataParallel(RAFT(argparse.Namespace(small=False, mixed_precision=False, alternate_corr=False)))
+    raft = torch.nn.DataParallel(RAFT(argparse.Namespace(small=False, mixed_precision=bool(mixed_precision),
+                                                         alternate_corr=False)))
     raft.load_state_dict(torch.load(raft_model, map_location="cpu"))
     raft = raft.module.to(device).eval()
     lafc_sd, lafc_cfg = ckpt_dir(lafc_ckpts)
@@ -626,6 +628,9 @@ def main(argv=None):
     ap.add_argument("--native", action="store_true",
                     help="write the frames at the input size: the result is upscaled and pasted into the input frames "
                          "around the mask (object_removal, watermark_removal)")
+    ap.add_argument("--mixed_precision", action="store_true",
+                    help="run RAFT with fp16 tensor-core operands, as the reference's autocast mode (faster, not "
+                         "fp32-accurate)")
     for k, v in DEFAULTS.items():
         if k == "mode":
             ap.add_argument("--mode", default=v, choices=list(MODES))
@@ -635,7 +640,7 @@ def main(argv=None):
     if ns.native and ns.mode == "video_extrapolation":
         ap.error("--native: video_extrapolation has no original frame to paste the result into")
     dev = torch.device("cuda", ns.gpu)
-    backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev)
+    backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev, ns.mixed_precision)
     args = make_args(**{k: getattr(ns, k) for k in DEFAULTS if hasattr(ns, k)})
     frames = IO.read_frames(ns.path)
     masks = IO.read_masks(ns.path_mask, rgb=ns.mode == "watermark_removal") if ns.mode != "video_extrapolation" else [None] * len(frames)

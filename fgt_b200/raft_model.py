@@ -12,6 +12,13 @@ call site :263). Parameter holders only; arithmetic runs in libfgt_sm90a.so:
     (1-z)h+zq update fused in GEMM epilogues) -> flow head -> fgt_raft_flow_update;
   * mask head + fgt_convex_upsample only where the result is consumed (last iteration in test_mode;
     the reference computes and discards the other 19, RAFT/raft.py:134-143).
+
+Precision follows `args.mixed_precision`, read on every forward like the reference (raft.py:100,111,128):
+  * False (default): every conv is a 3-term split-bf16 GEMM (fp32-grade).
+  * True: the convs of the three autocast regions (feature net, context net, update block) are 1-term fp16 GEMMs on
+    fp16 weights and fp16 activation rows; the correlation volume and its lookup stay fp32 (raft.py:103-104), and the
+    coordinates are fp32 (DESIGN.md section 2 lists where the rounding points differ from autocast).
+The two paths keep separate packed weights, workspaces and CUDA graphs.
 """
 import torch
 import torch.nn as nn
@@ -96,8 +103,11 @@ class RAFT(nn.Module):
             for m in net.modules():
                 if isinstance(m, nn.Conv2d):
                     nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
-        self._packed = None
+        self._packed = {}
         self._bufs = {}
+
+    def _mixed(self):
+        return bool(getattr(self.args, "mixed_precision", False))
 
     def _drop_graphs(self):
         """Captured CUDA graphs hold the addresses of the packed weights / workspaces they were recorded with."""
@@ -105,20 +115,23 @@ class RAFT(nn.Module):
             self._graphs.clear()
 
     def _apply(self, fn, *a, **k):
-        self._packed = None
+        self._packed = {}
         self._bufs = {}
         self._drop_graphs()
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, *a, **k):
-        self._packed = None
+        self._packed = {}
         self._drop_graphs()
         return super().load_state_dict(*a, **k)
 
     # ------------------------------------------------------------------ weight packing
-    def _pack(self, dev):
+    def _pack(self, dev, half=False):
+        """half: the mixed-precision set, every conv as a 1-term fp16 layer with fp16-rounded weights and biases (the
+        casts autocast applies to a conv's parameters)."""
         sd = {k: v.detach().float() for k, v in self.state_dict().items() if v.dtype.is_floating_point}
         P = {}
+        rnd = (lambda t: t.half()) if half else (lambda t: t.float())  # noqa: E731
 
         def wb(key, bn=None):
             w, b = sd[key + ".weight"], sd[key + ".bias"]
@@ -126,13 +139,15 @@ class RAFT(nn.Module):
                 g, be = sd[bn + ".weight"].double(), sd[bn + ".bias"].double()
                 mu, var = sd[bn + ".running_mean"].double(), sd[bn + ".running_var"].double()
                 s = g / torch.sqrt(var + 1e-5)
-                w = (w.double() * s[:, None, None, None]).float()
-                b = ((b.double() - mu) * s + be).float()
+                w = rnd(w.double() * s[:, None, None, None])  # folded in fp64, rounded once
+                b = rnd((b.double() - mu) * s + be)
+            elif half:
+                w, b = w.half(), b.half()
             return w, b
 
         def put(name, key, bn=None, segs=None, im2col=None):
             w, b = wb(key, bn)
-            P[name] = ops.packed(name, w, b, dev, segs, im2col)
+            P[name] = ops.packed(name, w, b, dev, segs, im2col, half=half)
 
         for net, isbn in (("fnet", False), ("cnet", True)):
             put(f"{net}.conv1", f"{net}.conv1", f"{net}.norm1" if isbn else None, im2col=192)
@@ -147,7 +162,7 @@ class RAFT(nn.Module):
         u = "update_block."
         w, b = wb(u + "encoder.convc1")
         w = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, 384 - 324))  # lookup rows are 384 wide (324 + zero pad)
-        P["convc1"] = ops.packed("convc1", w, b, dev)
+        P["convc1"] = ops.packed("convc1", w, b, dev, half=half)
         put("convc2", u + "encoder.convc2")
         put("convf1", u + "encoder.convf1", im2col=128)
         put("convf2", u + "encoder.convf2")
@@ -155,15 +170,19 @@ class RAFT(nn.Module):
         for s in "12":
             put(f"gru.q{s}", u + f"gru.convq{s}", segs=[128, 256])
             (wz, bz), (wr, br) = wb(u + f"gru.convz{s}", None), wb(u + f"gru.convr{s}", None)
-            P[f"gru.zr{s}"] = ops.packed(f"gru.zr{s}", torch.cat([wz, wr], 0), torch.cat([bz, br], 0), dev, [128, 256])
+            P[f"gru.zr{s}"] = ops.packed(f"gru.zr{s}", torch.cat([wz, wr], 0), torch.cat([bz, br], 0), dev, [128, 256],
+                                         half=half)
         put("fh1", u + "flow_head.conv1")
         put("fh2", u + "flow_head.conv2")
-        w2 = sd[u + "flow_head.conv2.weight"]
-        P["fh2t"] = ops.packed("fh2t", lib.pack_taps_as_n(w2), torch.zeros(32), dev)
+        w2 = rnd(sd[u + "flow_head.conv2.weight"])
+        P["fh2t"] = ops.packed("fh2t", lib.pack_taps_as_n(w2), torch.zeros(32), dev, half=half)
         put("mask0", u + "mask.0")
         put("mask2", u + "mask.2")
         P["mask2"]["b"] = P["mask2"]["b"] * 0.25  # mask = 0.25 * conv(x) (update.py:135): alpha scales W x
-        self._packed = P
+        cw = P["cnet.conv2"]  # net | inp halves of the context net's output conv (raft.py:113)
+        P["cnet.net"] = dict(cw, w=cw["w"][..., :128, :].contiguous(), b=cw["b"][:128].contiguous(), N=128, name="cnet.net")
+        P["cnet.inp"] = dict(cw, w=cw["w"][..., 128:, :].contiguous(), b=cw["b"][128:].contiguous(), N=128, name="cnet.inp")
+        self._packed[half] = P
         return P
 
     def _buf(self, key, name, shape, dev, split=True, zero=False, dtype=None):
@@ -177,69 +196,88 @@ class RAFT(nn.Module):
         return d[name]
 
     # ------------------------------------------------------------------ encoders
-    def _encoder(self, img, net, P, dev, n):
-        """BasicEncoder.forward (extractor.py:168-192) on `n` raw [0,255] images [n,3,H,W] -> NHWC features."""
+    def _encoder(self, img, net, P, dev, n, mixed=False):
+        """BasicEncoder.forward (extractor.py:168-192) on `n` raw [0,255] images [n,3,H,W] -> NHWC features
+        (split-bf16, or fp16 rows when mixed)."""
         _, _, H, W = img.shape
         inst = net == "fnet"
-        key = (net, n, H, W)
+        key = (net, n, H, W, mixed)
         B = lambda nm, s, **kw: self._buf(key, nm, s, dev, **kw)  # noqa: E731
+        A, o16, rows = self._act_fmt(B, mixed)
         RELU = lib.ACT_RELU
         H2, W2 = H // 2, W // 2
-        col = B("col", (n, H2, W2, 192))
+        col = A("col", (n, H2, W2, 192))
         # 2*(x/255)-1 applied to in-bounds taps (raft.py:90-91); zero padding stays zero
         lib.im2col_nchw(img, None, col, k=7, stride=2, pad=3, replicate=False, OH=H2, OW=W2, scale=2.0 / 255.0,
                         shift=-1.0, tag=net + ".conv1")
         stats = B("stats", (n * 128 * 2,), split=False, dtype=torch.float64)
         raw = B("raw", (n * H2 * W2 * 64,), split=False)  # largest pre-norm conv output, reused
 
+        def raw_out(numel, shape):
+            # mixed: left unrounded (autocast rounds it to fp16 before the norm); rounding it through an fp16 side
+            # output costs the half-resolution convs the batched GEMM epilogue (DESIGN.md section 2)
+            return dict(out_f32=raw[:numel].view(*shape))
+
         def conv_norm_act(xs, name, geo_n, hh, ww, c_out, stride, out_split, out_f32=None, res=None, relu=True, k=3):
             """conv (+folded BN) + norm + relu [+ residual relu]; returns nothing, writes outputs."""
             oh, ow = (hh + 2 * (k // 2) - k) // stride + 1, (ww + 2 * (k // 2) - k) // stride + 1
             if inst:
-                r = raw[: geo_n * oh * ow * c_out].view(geo_n, oh, ow, c_out)
-                ops.conv(xs, P[name], kx=k, ky=k, stride=stride, pad_x=k // 2, pad_y=k // 2, act=lib.ACT_NONE, out_f32=r)
+                ro = raw_out(geo_n * oh * ow * c_out, (geo_n, oh, ow, c_out))
+                r = ro["out_f32"]
+                ops.conv(xs, P[name], kx=k, ky=k, stride=stride, pad_x=k // 2, pad_y=k // 2, act=lib.ACT_NONE, **ro)
                 lib.chan_stats(r, geo_n, oh * ow, c_out, stats)
                 lib.instnorm_act(r, stats, geo_n, oh * ow, c_out, relu=relu, res=res, out=out_f32, out_split=out_split)
             else:
                 if res is not None:
                     ops.conv(xs, P[name], kx=k, ky=k, stride=stride, pad_x=k // 2, pad_y=k // 2, act=RELU, aux=res,
-                             aux_mode=lib.AUX_ADD_RELU, out_split=out_split, out_f32=out_f32)
+                             aux_mode=lib.AUX_ADD_RELU, out_f32=out_f32, **{o16: out_split})
                 else:
                     ops.conv(xs, P[name], kx=k, ky=k, stride=stride, pad_x=k // 2, pad_y=k // 2,
-                             act=RELU if relu else lib.ACT_NONE, out_split=out_split, out_f32=out_f32)
+                             act=RELU if relu else lib.ACT_NONE, out_f32=out_f32, **{o16: out_split})
 
-        x = B("x0", (n, H2, W2, 64))
+        x = A("x0", (n, H2, W2, 64))
         xf = B("x0f", (n, H2, W2, 64), split=False)
         if inst:
-            r = raw[: n * H2 * W2 * 64].view(n, H2, W2, 64)
-            ops.linear([(col.view(2, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, out_f32=r)
+            ro = raw_out(n * H2 * W2 * 64, (n, H2, W2, 64))
+            r = ro["out_f32"]
+            ops.linear([(rows(col, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, **ro)
             lib.chan_stats(r, n, H2 * W2, 64, stats)
             lib.instnorm_act(r, stats, n, H2 * W2, 64, relu=True, out=xf, out_split=x)
         else:
-            ops.linear([(col.view(2, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, act=RELU, out_f32=xf,
-                       out_split=x)
+            ops.linear([(rows(col, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, act=RELU, out_f32=xf,
+                       **{o16: x})
         hh, ww, cin = H2, W2, 64
         for li, (dim, stride) in enumerate(((64, 1), (96, 2), (128, 2)), start=1):
             for bi in (0, 1):
                 st = stride if bi == 0 else 1
                 k = f"{net}.layer{li}.{bi}"
                 oh, ow = hh // st, ww // st
-                y1 = B(f"{k}.y1", (n, oh, ow, dim))
+                y1 = A(f"{k}.y1", (n, oh, ow, dim))
                 conv_norm_act([(x, cin)], k + ".conv1", n, hh, ww, dim, st, y1)
                 if st != 1:  # x = norm3(conv1x1_s2(x)), no ReLU (extractor.py:52-53)
                     ds = B(f"{k}.ds", (n, oh, ow, dim), split=False)
-                    conv_norm_act([(x, cin)], k + ".down", n, hh, ww, dim, st, None, out_f32=ds, relu=False, k=1)
+                    ds16 = A(f"{k}.ds16", (n, oh, ow, dim)) if mixed else None  # makes `ds` fp16-valued; never read
+                    conv_norm_act([(x, cin)], k + ".down", n, hh, ww, dim, st, ds16, out_f32=ds, relu=False, k=1)
                     res = ds
                 else:
                     res = xf
-                xo = B(f"{k}.out", (n, oh, ow, dim))
+                xo = A(f"{k}.out", (n, oh, ow, dim))
                 xof = B(f"{k}.outf", (n, oh, ow, dim), split=False)
                 conv_norm_act([(y1, dim)], k + ".conv2", n, oh, ow, dim, 1, xo, out_f32=xof, res=res)
                 x, xf, hh, ww, cin = xo, xof, oh, ow, dim
-        return x, hh, ww  # NHWC split [2, n, H/8, W/8, 128]
+        return x, hh, ww  # NHWC split [2, n, H/8, W/8, 128] (fp16 [n, H/8, W/8, 128] when mixed)
+
+    @staticmethod
+    def _act_fmt(B, mixed):
+        """Activation format of a path: (allocator, GEMM output keyword, [rows, C] view). fp32 path: split-bf16
+        [2, ...] buffers written through out_split; mixed: single-plane fp16 buffers written through out_f16."""
+        if mixed:
+            return ((lambda nm, s, **kw: B(nm, s, split=False, dtype=torch.float16, **kw)), "out_f16",
+                    (lambda t, r, c: t.view(r, c)))
+        return B, "out_split", (lambda t, r, c: t.view(2, r, c))
 
     # ------------------------------------------------------------------ forward
-    def _forward_batch(self, im1, im2, iters, flow_init, test_mode, P, dev):
+    def _forward_batch(self, im1, im2, iters, flow_init, test_mode, P, dev, mixed=False):
         """RAFT.forward (raft.py:86-148) on n image pairs at once: every kernel of the update loop covers
         the n*h*w positions of all pairs, which is what fills the 132 SMs (one 1/8-resolution pair is 51 tiles)."""
         n, _, H, W = im1.shape
@@ -249,13 +287,22 @@ class RAFT(nn.Module):
         h, w = H // 8, W // 8
         npx = h * w
         tot = n * npx
-        key = ("iter", n, H, W)
+        key = ("iter", n, H, W, mixed)
         B = lambda nm, s, **kw: self._buf(key, nm, s, dev, **kw)  # noqa: E731
+        A, o16, rows = self._act_fmt(B, mixed)
+        sh = (lambda t, *s: t.view(*s)) if mixed else (lambda t, *s: t.view(2, *s))  # noqa: E731
         RELU, SIG, TANH, NONE = lib.ACT_RELU, lib.ACT_SIGMOID, lib.ACT_TANH, lib.ACT_NONE
         # ---- feature net on all 2n images, 1x1 output conv -> fmaps [2, 2n*npx, 256] (split)
-        f128, _, _ = self._encoder(torch.cat([im1, im2], 0), "fnet", P, dev, 2 * n)
+        f128, _, _ = self._encoder(torch.cat([im1, im2], 0), "fnet", P, dev, 2 * n, mixed)
         fmap = B("fmap", (2 * tot, 256))
-        ops.linear([(f128.view(2, 2 * tot, 128), 128)], P["fnet.conv2"], 2 * tot, out_split=fmap)
+        if mixed:
+            # fp16 output (autocast), then exactly to split-bf16: the 3-term correlation below is the reference's fp32
+            # correlation of fmap.float() (raft.py:103-104)
+            fmap16 = A("fmap16", (2 * tot, 256))
+            ops.linear([(rows(f128, 2 * tot, 128), 128)], P["fnet.conv2"], 2 * tot, out_f16=fmap16)
+            lib.f16_to_split(fmap16, fmap)
+        else:
+            ops.linear([(f128.view(2, 2 * tot, 128), 128)], P["fnet.conv2"], 2 * tot, out_split=fmap)
         # ---- all-pairs correlation (corr.py:52-60): corr[i,j] = <f1_i, f2_j> / 16 per pair, then the pyramid
         pyr = [B("corr0", (tot, h, w), split=False)]
         for i in range(n):
@@ -270,16 +317,12 @@ class RAFT(nn.Module):
             pyr.append(nxt)
             hh, ww = hh // 2, ww // 2
         # ---- context net: net = tanh(c[:128]), inp = relu(c[128:]) (raft.py:112-115)
-        c128, _, _ = self._encoder(im1, "cnet", P, dev, n)
-        hsp = B("h", (tot, 128))
+        c128, _, _ = self._encoder(im1, "cnet", P, dev, n, mixed)
+        hsp = A("h", (tot, 128))
         hf = B("hf", (tot, 128), split=False)
-        xbuf = B("x", (tot, 256))  # GRU input x = [inp(128) | motion features(126) | flow(2)]
-        cw = P["cnet.conv2"]
-        if "cnet.net" not in P:
-            P["cnet.net"] = dict(cw, w=cw["w"][:, :128].contiguous(), b=cw["b"][:128].contiguous(), N=128, name="cnet.net")
-            P["cnet.inp"] = dict(cw, w=cw["w"][:, 128:].contiguous(), b=cw["b"][128:].contiguous(), N=128, name="cnet.inp")
-        ops.linear([(c128.view(2, tot, 128), 128)], P["cnet.net"], tot, act=TANH, out_split=hsp, out_f32=hf)
-        ops.linear([(c128.view(2, tot, 128), 128)], P["cnet.inp"], tot, act=RELU, out_split=xbuf, os_x=256)
+        xbuf = A("x", (tot, 256))  # GRU input x = [inp(128) | motion features(126) | flow(2)]
+        ops.linear([(rows(c128, tot, 128), 128)], P["cnet.net"], tot, act=TANH, out_f32=hf, **{o16: hsp})
+        ops.linear([(rows(c128, tot, 128), 128)], P["cnet.inp"], tot, act=RELU, os_x=256, **{o16: xbuf})
         # ---- iterations
         coords = B("coords", (tot, 2), split=False)
         ys, xs = torch.meshgrid(torch.arange(h, device=dev), torch.arange(w, device=dev), indexing="ij")
@@ -288,78 +331,79 @@ class RAFT(nn.Module):
             coords.add_(flow_init.permute(0, 2, 3, 1).reshape(tot, 2).float())
         flow_nchw = B("flow", (n, 2, h, w), split=False)
         lib.raft_flow_update(coords, None, h, w, flow_nchw, xbuf, 254, n=n)
-        look = B("look", (tot, 384), zero=True)
-        cor1 = B("cor1", (n, h, w, 256))
-        corflo = B("corflo", (n, h, w, 256))  # [cor(192) | flo(64)]
-        fcol = B("fcol", (n, h, w, 128))
-        flo1 = B("flo1", (n, h, w, 128))
+        look = A("look", (tot, 384), zero=True)
+        cor1 = A("cor1", (n, h, w, 256))
+        corflo = A("corflo", (n, h, w, 256))  # [cor(192) | flo(64)]
+        fcol = A("fcol", (n, h, w, 128))
+        flo1 = A("flo1", (n, h, w, 128))
         z = B("z", (tot, 128), split=False)
-        rh = B("rh", (n, h, w, 128))
-        fh = B("fh", (n, h, w, 256))
+        rh = A("rh", (n, h, w, 128))
+        fh = A("fh", (n, h, w, 256))
         delta = B("delta", (tot, 2), split=False)
         fh2y = B("fh2y", (32, tot), split=False)  # column-planar partial products of the flow head
-        m0 = B("m0", (n, h, w, 256))
+        m0 = A("m0", (n, h, w, 256))
         mask = B("mask", (tot, 576), split=False)
-        h4 = hsp.view(2, n, h, w, 128)
-        x4 = xbuf.view(2, n, h, w, 256)
+        h4 = sh(hsp, n, h, w, 128)
+        x4 = sh(xbuf, n, h, w, 256)
         ups = []
         for it in range(iters):
             lib.corr_lookup(pyr, coords, tot, 4, look)
             # motion encoder (update.py:89-97)
-            ops.linear([(look, 384)], P["convc1"], tot, act=RELU, out_split=cor1.view(2, tot, 256))
-            ops.conv([(cor1, 256)], P["convc2"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=corflo,
-                     out_c_total=256, out_c_offset=0)
+            ops.linear([(look, 384)], P["convc1"], tot, act=RELU, **{o16: rows(cor1, tot, 256)})
+            ops.conv([(cor1, 256)], P["convc2"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_c_total=256,
+                     out_c_offset=0, **{o16: corflo})
             lib.im2col_nchw(flow_nchw, None, fcol, k=7, stride=1, pad=3, replicate=False, OH=h, OW=w)
-            ops.linear([(fcol.view(2, tot, 128), 128)], P["convf1"], tot, act=RELU, out_split=flo1.view(2, tot, 128))
-            ops.conv([(flo1, 128)], P["convf2"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=corflo,
-                     out_c_total=256, out_c_offset=192)
-            ops.conv([(corflo, 256)], P["mconv"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=x4,
-                     out_c_total=256, out_c_offset=128)
+            ops.linear([(rows(fcol, tot, 128), 128)], P["convf1"], tot, act=RELU, **{o16: rows(flo1, tot, 128)})
+            ops.conv([(flo1, 128)], P["convf2"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_c_total=256,
+                     out_c_offset=192, **{o16: corflo})
+            ops.conv([(corflo, 256)], P["mconv"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_c_total=256,
+                     out_c_offset=128, **{o16: x4})
             # SepConvGRU (update.py:45-60): horizontal (1x5) then vertical (5x1)
             for s, (kx, ky) in (("1", (5, 1)), ("2", (1, 5))):
                 kw = dict(kx=kx, ky=ky, pad_x=kx // 2, pad_y=ky // 2, seg_counts=[128, 256])
                 # z = sigmoid(convz(hx)) and r*h = sigmoid(convr(hx)) * h as ONE N=256 GEMM over the shared input
                 ops.conv([(h4, 128), (x4, 256)], P[f"gru.zr{s}"], act=SIG, aux=hf, aux_mode=lib.AUX_GRU_ZR,
-                         out_f32=z.view(n, h, w, 128), out_split=rh, out_c_total=128, **kw)
+                         out_f32=z.view(n, h, w, 128), out_c_total=128, **{o16: rh}, **kw)
                 ops.conv([(rh, 128), (x4, 256)], P[f"gru.q{s}"], act=TANH, aux=hf, aux2=z, aux_mode=lib.AUX_GRU,
-                         out_f32=hf.view(n, h, w, 128), out_split=h4, **kw)
+                         out_f32=hf.view(n, h, w, 128), **{o16: h4}, **kw)
             # flow head (update.py:13-14)
-            ops.conv([(h4, 128)], P["fh1"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=fh)
+            ops.conv([(h4, 128)], P["fh1"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, **{o16: fh})
             # 256->2 conv as "taps as N" (1x1 GEMM with N = 18 -> 32, then shift-and-add): A is read once, not 9x
-            ops.linear([(fh.view(2, tot, 256), 256)], P["fh2t"], tot, out_f32=fh2y, os_x=1, os_c=tot)
+            ops.linear([(rows(fh, tot, 256), 256)], P["fh2t"], tot, out_f32=fh2y, os_x=1, os_c=tot)
             lib.tapsum(fh2y, n, h, w, 2, 3, P["fh2"]["b"], NONE, delta, nchw=False, tag="fh2")
-            lib.raft_flow_update(coords, delta, h, w, flow_nchw, xbuf, 254, n=n)
+            lib.raft_flow_update(coords, delta, h, w, flow_nchw, xbuf, 254, n=n, delta_f16=mixed)
             if not test_mode or it == iters - 1:
                 # mask head scaled by 0.25 (update.py:122-125,135) + convex upsampling (raft.py:73-84)
-                ops.conv([(h4, 128)], P["mask0"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=m0)
-                ops.linear([(m0.view(2, tot, 256), 256)], P["mask2"], tot, alpha=0.25, out_f32=mask)
+                ops.conv([(h4, 128)], P["mask0"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, **{o16: m0})
+                ops.linear([(rows(m0, tot, 256), 256)], P["mask2"], tot, alpha=0.25, out_f32=mask)
                 up = torch.empty(n, 2, 8 * h, 8 * w, device=dev)
                 lib.convex_upsample(mask, flow_nchw, h, w, up, n=n)
                 ups.append(up)
         return flow_nchw.clone(), ups
 
     def enable_cuda_graph(self, on=True):
-        """Replay whole forwards as CUDA graphs, one per (geometry, iters, test_mode) (fgt_b200/graphs.py)."""
+        """Replay whole forwards as CUDA graphs, one per (geometry, iters, test_mode, precision) (fgt_b200/graphs.py)."""
         self._graphs = {} if on else None
 
     def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False):
         if not image1.is_cuda:
             raise RuntimeError("fgt_b200 RAFT runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+        mixed = self._mixed()  # read on every call, as the reference reads self.args.mixed_precision
         if getattr(self, "_graphs", None) is not None and flow_init is None:
             from .graphs import GraphedCall
-            key = (iters, bool(test_mode))
+            key = (iters, bool(test_mode), mixed)
             if key not in self._graphs:
                 self._graphs[key] = GraphedCall(
-                    lambda a, b, _it=iters, _tm=test_mode: self._forward_impl(a, b, _it, None, _tm))
+                    lambda a, b, _it=iters, _tm=test_mode, _mx=mixed: self._forward_impl(a, b, _it, None, _tm, _mx))
             out = self._graphs[key](image1.float().contiguous(), image2.float().contiguous())
             return list(out) if not test_mode else out
-        return self._forward_impl(image1, image2, iters, flow_init, test_mode)
+        return self._forward_impl(image1, image2, iters, flow_init, test_mode, mixed)
 
-    def _forward_impl(self, image1, image2, iters, flow_init, test_mode):
+    def _forward_impl(self, image1, image2, iters, flow_init, test_mode, mixed=False):
         dev = image1.device
-        P = self._packed if self._packed is not None else self._pack(dev)
+        P = self._packed[mixed] if mixed in self._packed else self._pack(dev, mixed)
         image1, image2 = image1.float().contiguous(), image2.float().contiguous()
-        lo, ups = self._forward_batch(image1, image2, iters, flow_init, test_mode, P, dev)
+        lo, ups = self._forward_batch(image1, image2, iters, flow_init, test_mode, P, dev, mixed)
         if test_mode:
             return lo, ups[-1]
         return ups

@@ -48,7 +48,9 @@ enum { FGT_ACT_NONE = 0, FGT_ACT_LEAKY02 = 1, FGT_ACT_RELU = 2, FGT_ACT_SIGMOID 
  *      (1 - aux2) * aux + aux2 * act(v)   (the ConvGRU state update, RAFT/update.py:52,58) |
  *      GRU_ZR: the z and r gate convolutions of a ConvGRU as ONE GEMM with N = 2*C (update.py:48-49,54-55):
  *      columns [0,C) -> out_f32 = act(v) (z), columns [C,2C) -> out_hi = act(v) * aux (r*h); both outputs
- *      and aux have C channels per position (output strides describe a C-channel buffer). */
+ *      and aux have C channels per position (output strides describe a C-channel buffer).
+ *      With out_half (mixed-precision RAFT, autocast semantics) both GRU modes round act(v) to fp16 first; GRU_ZR
+ *      stores r*h as fp16, and GRU rounds each of (1 - z), (1 - z) * h, z * q and their sum to fp16. */
 enum { FGT_AUX_NONE = 0, FGT_AUX_ADD = 1, FGT_AUX_MUL = 2, FGT_AUX_ADD_PRE = 3, FGT_AUX_ADD_RELU = 4,
        FGT_AUX_GRU = 5, FGT_AUX_GRU_ZR = 6 };
 
@@ -111,7 +113,9 @@ typedef struct {
   int terms;                 /* 0 / 3: split-bf16 product hi*hi + hi*lo + lo*hi (fp32-grade, 3 MMAs per K step);
                                 1: the A segments and W are single-plane fp16 tensors (`hi` points at fp16 data, the
                                 plane offsets are ignored), one MMA per K step — for layers whose error budget allows */
-  int out_half;              /* 1: out_hi receives ONE plane of fp16 (the input format of a terms == 1 layer) */
+  int out_half;              /* 1: out_hi receives ONE plane of fp16 (the input format of a terms == 1 layer). With
+                                out_f32 as well (mixed-precision RAFT, autocast semantics), the value is rounded to
+                                fp16 before the activation and again after it, and out_f32 receives that fp16 value */
 } FgtGemmDesc;
 
 int fgt_gemm_tc(const FgtGemmDesc* desc, fgt_stream_t stream);
@@ -453,7 +457,9 @@ int fgt_upsample2x(const void* in_hi, long long in_plane, int n, int H, int W, i
 int fgt_chan_stats(const float* x, int n, int HW, int C, double* stats, fgt_stream_t stream);
 
 /* y = (x - mean) * rsqrt(var + eps) [ReLU] ; if res: y = relu(y + res). ResidualBlock.forward,
- * RAFT/extractor.py:47-56 and BasicEncoder.forward :176-178 for the instance-norm feature net. */
+ * RAFT/extractor.py:47-56 and BasicEncoder.forward :176-178 for the instance-norm feature net.
+ * out_hi receives split-bf16, or single-plane fp16 when out_plane == 0 (mixed precision; `out` then receives the same
+ * fp16-rounded values). */
 int fgt_instnorm_act(const float* x, const double* stats, int n, int HW, int C, float eps, int relu,
                      const float* res, float* out, void* out_hi, long long out_plane, fgt_stream_t stream);
 
@@ -464,16 +470,24 @@ int fgt_avgpool2(const float* in, long long rows, int h, int w, float* out, fgt_
  * n_pix source pixels and each pyramid level l (volume level_ptrs[l] = [n_pix, h_l, w_l] fp32), the
  * (2r+1)^2 zero-padded bilinear samples around coords/2^l. Output split-bf16 [n_pix, out_pitch],
  * channel = l*(2r+1)^2 + a*(2r+1) + b with a offsetting x and b offsetting y (reference order).
- * level_ptrs_host / level_h_host / level_w_host are HOST arrays of `levels` entries. */
+ * level_ptrs_host / level_h_host / level_w_host are HOST arrays of `levels` entries.
+ * out_plane == 0: the output is single-plane fp16 [n_pix, out_pitch] (mixed precision). */
 int fgt_corr_lookup(const float* const* level_ptrs_host, const int* level_h_host, const int* level_w_host,
                     int levels, int radius, const float* coords, int n_pix, int out_pitch, void* out_hi,
                     long long out_plane, fgt_stream_t stream);
 
 /* coords += delta (delta may be NULL) for n image pairs, coords/delta [n*h*w, 2]; writes
  * flow = coords - pixel grid as NCHW fp32 [n,2,h,w] and, if x_hi != NULL, as channels
- * [x_chan, x_chan+1] of the split GRU-input buffer (RAFT/raft.py:127-132). */
-int fgt_raft_flow_update(float* coords, const float* delta, int n, int h, int w, float* flow_nchw, void* x_hi,
-                         long long x_plane, int x_pitch, int x_chan, fgt_stream_t stream);
+ * [x_chan, x_chan+1] of the split GRU-input buffer (RAFT/raft.py:127-132); x_plane == 0: x is single-plane fp16.
+ * delta_f16 = 1 rounds delta to fp16 before the add (mixed precision: the flow head's output is an fp16 tensor under
+ * autocast); 0 adds it as given. */
+int fgt_raft_flow_update(float* coords, const float* delta, int delta_f16, int n, int h, int w, float* flow_nchw,
+                         void* x_hi, long long x_plane, int x_pitch, int x_chan, fgt_stream_t stream);
+
+/* fp16 [n] -> split-bf16 [2][n] (hi plane at out_hi, lo plane out_plane elements later), exact for every fp16 value.
+ * Mixed-precision RAFT: the feature net's fp16 output feeds the 3-term correlation GEMM. n and out_plane multiples of
+ * 8, both buffers 16-byte aligned. */
+int fgt_f16_to_split(const void* src, long long n, void* out_hi, long long out_plane, fgt_stream_t stream);
 
 /* RAFT.upsample_flow (RAFT/raft.py:73-84): mask [n*h*w, 576] fp32, flow [n,2,h,w] -> up-sampled flow
  * [n, 2, 8h, 8w]. */
