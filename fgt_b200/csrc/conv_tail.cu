@@ -13,6 +13,7 @@
 //   warps 0..3 : one warpgroup: wgmma (3-term split-bf16, M=64 x N=32, three M blocks per chunk, fp32 accumulators in
 //                registers) -> Y rows in smem (pitch 33 floats: conflict-free both ways) -> 9-tap sums -> bias,
 //                activation, coalesced stores
+// kF16 (mixed precision): activation and weights are single-plane fp16, one fp16 wgmma per K step.
 #include "common.h"
 #include "ptx.cuh"
 
@@ -45,7 +46,9 @@ struct TailParams {
   long long os_n, os_c, os_y, os_x;
 };
 
+template <bool kF16>
 __global__ void __launch_bounds__(kTailThreads, 1) conv_tail_kernel(const __grid_constant__ TailParams p) {
+  constexpr int kPlanes = kF16 ? 1 : 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sgen = smem_raw + (sbase - smem_u32(smem_raw));
@@ -75,9 +78,9 @@ __global__ void __launch_bounds__(kTailThreads, 1) conv_tail_kernel(const __grid
     // ------------------------------------------------------------ TMA producer
     if (elect_one()) {
       // weights: every (chunk, plane) block once per CTA
-      mbar_expect_tx(w_bar, static_cast<uint32_t>(p.chunks) * 2u * kTailBBlk);
+      mbar_expect_tx(w_bar, static_cast<uint32_t>(p.chunks) * kPlanes * kTailBBlk);
       for (int c = 0; c < p.chunks; ++c)
-        for (int pl = 0; pl < 2; ++pl)
+        for (int pl = 0; pl < kPlanes; ++pl)
           tma_load_3d(sbase + kTailSmemB + (c * 2 + pl) * kTailBBlk, &p.b_map, w_bar, c * 64, 0, pl);
       int stage = 0;
       uint32_t phase = 0;
@@ -88,9 +91,9 @@ __global__ void __launch_bounds__(kTailThreads, 1) conv_tail_kernel(const __grid
         for (int c = 0; c < p.chunks; ++c) {
           mbar_wait_quiet(empty_bar(stage), phase ^ 1u);
           const uint32_t sa = sbase + kTailSmemA + stage * kTailAStage;
-          mbar_expect_tx(full_bar(stage), 2u * kTailRows * 128u);
+          mbar_expect_tx(full_bar(stage), kPlanes * kTailRows * 128u);
           tma_load_5d(sa, &p.a_map, full_bar(stage), c * 64, tx * kTailTW - 1, ty * kTailTH - 1, z, 0);
-          tma_load_5d(sa + kTailAPlane, &p.a_map, full_bar(stage), c * 64, tx * kTailTW - 1, ty * kTailTH - 1, z, 1);
+          if (!kF16) tma_load_5d(sa + kTailAPlane, &p.a_map, full_bar(stage), c * 64, tx * kTailTW - 1, ty * kTailTH - 1, z, 1);
           if (++stage == kTailStages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -131,6 +134,10 @@ __global__ void __launch_bounds__(kTailThreads, 1) conv_tail_kernel(const __grid
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const uint64_t ko = static_cast<uint64_t>(k * 2);
+          if (kF16) {
+            wgmma_ss<32, true>(acc[mb], a_hi + ko, b_hi + ko, (c | k) != 0);
+            continue;
+          }
           wgmma_ss<32, false>(acc[mb], a_lo + ko, b_hi + ko, (c | k) != 0);
           wgmma_ss<32, false>(acc[mb], a_hi + ko, b_lo + ko, 1u);
           wgmma_ss<32, false>(acc[mb], a_hi + ko, b_hi + ko, 1u);
@@ -198,21 +205,28 @@ extern "C" int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, 
   FGT_REQUIRE(cout >= 1 && cout <= 3, FGT_ERR_ARG, "conv_tail: cout=%d (1..3: nine taps times cout must fit 32 columns)", cout);
   FGT_REQUIRE(k_pad == cin, FGT_ERR_ARG, "conv_tail: weights must be packed [32, cin] (k_pad=%d, cin=%d)", k_pad, cin);
   FGT_REQUIRE(n >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "conv_tail: empty problem");
-  FGT_REQUIRE(x_plane % 8 == 0 && w_plane % 8 == 0, FGT_ERR_ARG, "conv_tail: plane offsets");
+  FGT_REQUIRE(x_plane % 8 == 0 && w_plane % 8 == 0 && x_plane >= 0 && w_plane >= 0, FGT_ERR_ARG, "conv_tail: plane offsets");
+  FGT_REQUIRE((x_plane == 0) == (w_plane == 0), FGT_ERR_ARG,
+              "conv_tail: activation and weights are both split-bf16 (plane > 0) or both single-plane fp16 (plane 0), "
+              "got x_plane=%lld w_plane=%lld", x_plane, w_plane);
+  const bool f16 = x_plane == 0;
+  const uint64_t planes = f16 ? 1 : 2;
   TailParams p;
   memset(&p, 0, sizeof(p));
   {
     uint64_t dims[5] = {static_cast<uint64_t>(cin), static_cast<uint64_t>(W), static_cast<uint64_t>(H),
-                        static_cast<uint64_t>(n), 2};
+                        static_cast<uint64_t>(n), planes};
     uint64_t str[4] = {static_cast<uint64_t>(cin) * 2, static_cast<uint64_t>(W) * cin * 2,
                        static_cast<uint64_t>(H) * W * cin * 2, static_cast<uint64_t>(x_plane) * 2};
+    if (f16) str[3] = str[2] * dims[3];  // single plane: the plane dimension has extent 1
     uint32_t box[5] = {64, kTailHW, kTailHH, 1, 1};
     int rc = encode_map_bf16(&p.a_map, x_hi, 5, dims, str, box);
     if (rc) return rc;
   }
   {
-    uint64_t dims[3] = {static_cast<uint64_t>(k_pad), 32, 2};
+    uint64_t dims[3] = {static_cast<uint64_t>(k_pad), 32, planes};
     uint64_t str[2] = {static_cast<uint64_t>(k_pad) * 2, static_cast<uint64_t>(w_plane) * 2};
+    if (f16) str[1] = str[0] * dims[1];
     uint32_t box[3] = {64, 32, 1};
     int rc = encode_map_bf16(&p.b_map, w_hi, 3, dims, str, box);
     if (rc) return rc;
@@ -223,14 +237,15 @@ extern "C" int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, 
   p.total_tiles = p.tiles_x * p.tiles_y * n;
   p.H = H; p.W = W; p.cout = cout; p.act = act; p.bias = bias; p.out = out;
   p.os_n = os_n; p.os_c = os_c; p.os_y = os_y; p.os_x = os_x;
-  static bool attr_set = false;
-  if (!attr_set) {
-    FGT_CUDA(cudaFuncSetAttribute(conv_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTailSmem));
-    attr_set = true;
+  static bool attr_set[2] = {false, false};
+  auto kern = f16 ? conv_tail_kernel<true> : conv_tail_kernel<false>;
+  if (!attr_set[f16]) {
+    FGT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kTailSmem));
+    attr_set[f16] = true;
   }
   int grid = num_sms();
   if (grid > p.total_tiles) grid = p.total_tiles;
-  launch_k(conv_tail_kernel, dim3(grid), dim3(kTailThreads), kTailSmem, reinterpret_cast<cudaStream_t>(stream), p);
+  launch_k(kern, dim3(grid), dim3(kTailThreads), kTailSmem, reinterpret_cast<cudaStream_t>(stream), p);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }

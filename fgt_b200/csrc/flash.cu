@@ -11,6 +11,9 @@
 // The two warpgroups run independently, so one's softmax overlaps the other's MMAs. O is rescaled only when the
 // running max outgrows the reference max by more than 2^8 (lazy rescaling; softmax is shift-invariant, so exact).
 //
+// kF16 (mixed precision): Q, K, V and the output are single-plane fp16; QK^T and P V take one fp16 wgmma per K step
+// (P rounded to fp16 as the A operand). The scores, the online softmax and O stay fp32.
+//
 // mode DENSE    (TMHSA, attention_base.py:93-99): every key tile of the (batch=zone) sequence.
 // mode WINDOWED (SWMHSA, attention_flow.py:130-164): a 128-row query tile is two 64-token windows;
 //   its key list is [global tiles..., own window tile 2i, own window tile 2i+1] with a block-diagonal
@@ -59,7 +62,9 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+template <bool kF16>
 __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_constant__ FlashParams p) {
+  constexpr int kPlanes = kF16 ? 1 : 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5;
@@ -104,14 +109,14 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
       for (int j = 0; j < n_tiles; ++j) {
         const int r0 = key_row0(j);
         mbar_wait_quiet(k_empty(s), ph ^ 1u);
-        mbar_expect_tx(k_full(s), kKStage);
-        for (int pl = 0; pl < 2; ++pl)
+        mbar_expect_tx(k_full(s), kPlanes * 2 * kKBlk);
+        for (int pl = 0; pl < kPlanes; ++pl)
           for (int kc = 0; kc < 2; ++kc)
             tma_load_4d(sbase + kSmemK + s * kKStage + (pl * 2 + kc) * kKBlk, &p.k_map, k_full(s),
                         head * 128 + kc * 64, r0, batch, pl);
         mbar_wait_quiet(v_empty(s), ph ^ 1u);
-        mbar_expect_tx(v_full(s), kVStage);
-        for (int pl = 0; pl < 2; ++pl)
+        mbar_expect_tx(v_full(s), kPlanes * kVBlk);
+        for (int pl = 0; pl < kPlanes; ++pl)
           for (int hf = 0; hf < 2; ++hf)
             tma_load_4d(sbase + kSmemV + s * kVStage + pl * kVBlk + hf * kVHalf, &p.v_map, v_full(s),
                         head * 128 + hf * 64, r0, batch, pl);
@@ -128,7 +133,7 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
     // Q tile -> shared memory as the K-major A operand: block (plane, 64-dim chunk) of 128 rows x 128 B, 16-byte chunk c
     // of row r at c ^ (r & 7) (the 128B swizzle). 256 threads x 16 chunks.
     uint8_t* sq = smem_raw + (sbase - smem_u32(smem_raw)) + kSmemQ;
-    for (int i = threadIdx.x; i < 2 * 128 * 16; i += 256) {
+    for (int i = threadIdx.x; i < kPlanes * 128 * 16; i += 256) {
       const int pl = i >> 11, r = (i >> 4) & 127, c = i & 15;
       const int qrow = qt * 128 + r;
       uint4 v = make_uint4(0u, 0u, 0u, 0u);
@@ -174,6 +179,10 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const uint64_t ko = static_cast<uint64_t>(k * 2);
+          if (kF16) {
+            wgmma_ss<64, true>(sv, a_hi + ko, b_hi + ko, (kc | k) != 0);
+            continue;
+          }
           wgmma_ss<64, false>(sv, a_lo + ko, b_hi + ko, (kc | k) != 0);  // Q_lo * K_hi
           wgmma_ss<64, false>(sv, a_hi + ko, b_lo + ko, 1u);             // Q_hi * K_lo
           wgmma_ss<64, false>(sv, a_hi + ko, b_hi + ko, 1u);             // Q_hi * K_hi
@@ -223,7 +232,10 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
       }
       // P as the A operand: k16 chunk kk = sv[8 kk .. 8 kk + 7] -> {(g, 2qc), (g + 8, 2qc), (g, 2qc + 8), (g + 8, 2qc + 8)}
 #pragma unroll
-      for (int i = 0; i < 16; ++i) split_bf16x2(sv[2 * i], sv[2 * i + 1], pa_hi[i], pa_lo[i]);
+      for (int i = 0; i < 16; ++i) {
+        if (kF16) pa_hi[i] = pack_f16x2(sv[2 * i], sv[2 * i + 1]);
+        else split_bf16x2(sv[2 * i], sv[2 * i + 1], pa_hi[i], pa_lo[i]);
+      }
     }
 
     mbar_wait_quiet(v_full(s), ph);
@@ -237,6 +249,10 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
       for (int k = 0; k < 4; ++k) {
         const uint64_t ko = static_cast<uint64_t>(k * 128);  // 16 keys = two 8-row swizzle atoms = 2048 B >> 4
         const uint32_t ah[4] = {pa_hi[4 * k], pa_hi[4 * k + 1], pa_hi[4 * k + 2], pa_hi[4 * k + 3]};
+        if (kF16) {
+          wgmma_rs_f16_mnb128(o, ah, b_hi + ko, 1u);
+          continue;
+        }
         const uint32_t al[4] = {pa_lo[4 * k], pa_lo[4 * k + 1], pa_lo[4 * k + 2], pa_lo[4 * k + 3]};
         wgmma_rs_bf16_mnb128(o, al, b_hi + ko, 1u);  // P_lo * V_hi
         wgmma_rs_bf16_mnb128(o, ah, b_lo + ko, 1u);  // P_hi * V_lo
@@ -268,6 +284,10 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
     __nv_bfloat16* oh = p.out_hi + orow + head * 128 + 2 * qc;
 #pragma unroll
     for (int jj = 0; jj < 16; ++jj) {
+      if (kF16) {
+        *reinterpret_cast<uint32_t*>(oh + 8 * jj) = pack_f16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+        continue;
+      }
       uint32_t hw, lw;
       split_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, hw, lw);
       *reinterpret_cast<uint32_t*>(oh + 8 * jj) = hw;
@@ -285,9 +305,15 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
                   d.out_batch_stride % 8 == 0 && d.out_plane % 8 == 0,
               FGT_ERR_ARG, "attention: batch strides must be multiples of 8 elements");
   FGT_REQUIRE(d.mode == 0 || d.mode == 1, FGT_ERR_ARG, "attention: mode=%d", d.mode);
+  FGT_REQUIRE(d.f16 == 0 || d.f16 == 1, FGT_ERR_ARG, "attention: f16=%d (0 split-bf16, 1 single-plane fp16)", d.f16);
+  const bool f16 = d.f16 != 0;
+  FGT_REQUIRE(!f16 || (d.q_plane == 0 && d.k_plane == 0 && d.v_plane == 0 && d.out_plane == 0), FGT_ERR_ARG,
+              "attention: f16 operands are single-plane (plane offsets must be 0)");
+  FGT_REQUIRE(d.q_hi && d.k_hi && d.v_hi && d.out_hi, FGT_ERR_ARG, "attention: null operand");
   FlashParams p;
   memset(&p, 0, sizeof(p));
   const uint64_t hd = static_cast<uint64_t>(d.heads) * 128;
+  const uint64_t planes = f16 ? 1 : 2;
   FGT_REQUIRE((reinterpret_cast<uintptr_t>(d.q_hi) & 15) == 0 && d.q_plane % 8 == 0, FGT_ERR_ARG,
               "attention: Q misaligned");
   p.q_hi = reinterpret_cast<const __nv_bfloat16*>(d.q_hi);
@@ -295,19 +321,21 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   p.q_batch_stride = d.q_batch_stride;
   p.q_ld = d.q_ld;
   {
-    uint64_t dims[4] = {hd, static_cast<uint64_t>(d.Lk_rows), static_cast<uint64_t>(d.batches), 2};
+    uint64_t dims[4] = {hd, static_cast<uint64_t>(d.Lk_rows), static_cast<uint64_t>(d.batches), planes};
     uint64_t str[3] = {static_cast<uint64_t>(d.k_ld) * 2, static_cast<uint64_t>(d.k_batch_stride) * 2,
                        static_cast<uint64_t>(d.k_plane) * 2};
     if (d.batches == 1) str[1] = str[0] * dims[1];
+    if (f16) str[2] = str[1] * dims[2];  // single plane: the plane dimension has extent 1
     uint32_t box[4] = {64, 64, 1, 1};
     int rc = encode_map_bf16(&p.k_map, d.k_hi, 4, dims, str, box);
     if (rc) return rc;
   }
   {
-    uint64_t dims[4] = {hd, static_cast<uint64_t>(d.Lk_rows), static_cast<uint64_t>(d.batches), 2};
+    uint64_t dims[4] = {hd, static_cast<uint64_t>(d.Lk_rows), static_cast<uint64_t>(d.batches), planes};
     uint64_t str[3] = {static_cast<uint64_t>(d.v_ld) * 2, static_cast<uint64_t>(d.v_batch_stride) * 2,
                        static_cast<uint64_t>(d.v_plane) * 2};
     if (d.batches == 1) str[1] = str[0] * dims[1];
+    if (f16) str[2] = str[1] * dims[2];
     uint32_t box[4] = {64, 64, 1, 1};
     int rc = encode_map_bf16(&p.v_map, d.v_hi, 4, dims, str, box);
     if (rc) return rc;
@@ -331,13 +359,14 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   p.out_rowmap = d.out_rowmap;
   FGT_REQUIRE((reinterpret_cast<uintptr_t>(d.out_hi) & 15) == 0, FGT_ERR_ARG, "attention: output misaligned");
 
-  static bool attr_set = false;
-  if (!attr_set) {
-    FGT_CUDA(cudaFuncSetAttribute(flash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFlashSmem));
-    attr_set = true;
+  static bool attr_set[2] = {false, false};
+  auto kern = f16 ? flash_kernel<true> : flash_kernel<false>;
+  if (!attr_set[f16]) {
+    FGT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kFlashSmem));
+    attr_set[f16] = true;
   }
   dim3 grid((d.Lq + 127) / 128, d.heads, d.batches);
-  launch_k(flash_kernel, dim3(grid), dim3(kFlashThreads), kFlashSmem, stream, p);
+  launch_k(kern, dim3(grid), dim3(kFlashThreads), kFlashSmem, stream, p);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }

@@ -23,6 +23,13 @@ __device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* l
   *reinterpret_cast<uint2*>(lo) = make_uint2(pack_bf16x2(l0, l1), pack_bf16x2(l2, l3));
 }
 
+// Four consecutive 16-bit outputs: split-bf16 with the lo plane `plane` elements after hi, or single-plane fp16 rows
+// (the A operand of a 1-term layer, mixed precision) when plane == 0.
+__device__ __forceinline__ void store16x4(__nv_bfloat16* hi, long long plane, float a, float b, float c, float d) {
+  if (plane == 0) *reinterpret_cast<uint2*>(hi) = make_uint2(pack_f16x2(a, b), pack_f16x2(c, d));
+  else store_split4(hi, hi + plane, a, b, c, d);
+}
+
 // ------------------------------------------------------------------------------------------
 // pack: NCHW fp32 (two sources concatenated on C) -> NHWC split-bf16 with channel padding and
 // optional replication padding (ReplicationPad2d of the flow encoder, model.py:207).
@@ -165,7 +172,7 @@ __global__ void __launch_bounds__(256, 4) rownorm_kernel(const float* __restrict
       for (int q = 0; q < dst.n; ++q) {
         for (int v = lane; v < nvec; v += 32) {
           *reinterpret_cast<uint2*>(dst.hi[q] + ooff + v * 4) = make_uint2(0u, 0u);
-          *reinterpret_cast<uint2*>(dst.hi[q] + ooff + plane + v * 4) = make_uint2(0u, 0u);
+          if (plane) *reinterpret_cast<uint2*>(dst.hi[q] + ooff + plane + v * 4) = make_uint2(0u, 0u);
         }
       }
       continue;
@@ -202,6 +209,11 @@ __global__ void __launch_bounds__(256, 4) rownorm_kernel(const float* __restrict
           const float4 gm = __ldg(reinterpret_cast<const float4*>(gamma + v * 4));
           const float4 bt = __ldg(reinterpret_cast<const float4*>(beta + v * 4));
           o.x = o.x * gm.x + bt.x; o.y = o.y * gm.y + bt.y; o.z = o.z * gm.z + bt.z; o.w = o.w * gm.w + bt.w;
+        }
+        if (plane == 0) {  // single-plane fp16 rows (mixed precision)
+          const uint2 hv = make_uint2(pack_f16x2(o.x, o.y), pack_f16x2(o.z, o.w));
+          for (int q = 0; q < dst.n; ++q) *reinterpret_cast<uint2*>(dst.hi[q] + ooff + v * 4) = hv;
+          continue;
         }
         uint32_t h0, l0, h1, l1;
         split_bf16x2(o.x, o.y, h0, l0);
@@ -297,7 +309,7 @@ __global__ void dwconv3_res_kernel(const float* __restrict__ x, int bt, int h, i
     const float4 v = make_float4(acc.x + centre.x, acc.y + centre.y, acc.z + centre.z, acc.w + centre.w);
     const long long o = t * C + c;
     *reinterpret_cast<float4*>(out + o) = v;
-    if (hi) store_split4(hi + o, hi + plane + o, v.x, v.y, v.z, v.w);
+    if (hi) store16x4(hi + o, plane, v.x, v.y, v.z, v.w);
    }
   }
 }
@@ -388,7 +400,7 @@ __global__ void fold_kernel(const float* __restrict__ hid, int bt, int th, int t
       acc.x += a4.x; acc.y += a4.y; acc.z += a4.z; acc.w += a4.w;
     }
     if (out) *reinterpret_cast<float4*>(out + o) = acc;
-    if (hi) store_split4(hi + o, hi + plane + o, acc.x, acc.y, acc.z, acc.w);
+    if (hi) store16x4(hi + o, plane, acc.x, acc.y, acc.z, acc.w);
   }
 }
 
@@ -473,9 +485,14 @@ __global__ void fold_unfold_kernel(const float* __restrict__ hid, int bt, int th
         acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f);
       }
     }
-    uint32_t h0, l0, h1, l1;
-    split_bf16x2(acc.x, acc.y, h0, l0);
-    split_bf16x2(acc.z, acc.w, h1, l1);
+    uint32_t h0, l0 = 0u, h1, l1 = 0u;
+    if (plane == 0) {  // single-plane fp16 patches (mixed precision)
+      h0 = pack_f16x2(acc.x, acc.y);
+      h1 = pack_f16x2(acc.z, acc.w);
+    } else {
+      split_bf16x2(acc.x, acc.y, h0, l0);
+      split_bf16x2(acc.z, acc.w, h1, l1);
+    }
     for (int ty = ty_hi; ty >= 0; --ty) {
       const int ky = y + pd - st * ty;
       if (ky >= kh) break;
@@ -486,7 +503,7 @@ __global__ void fold_unfold_kernel(const float* __restrict__ hid, int bt, int th
         if (kx < 0) continue;
         const long long o = ((static_cast<long long>(b) * th + ty) * tw + tx) * hidden + (ky * kw + kx) * C + c;
         *reinterpret_cast<uint2*>(hi + o) = make_uint2(h0, h1);
-        *reinterpret_cast<uint2*>(hi + plane + o) = make_uint2(l0, l1);
+        if (plane) *reinterpret_cast<uint2*>(hi + plane + o) = make_uint2(l0, l1);
       }
     }
   }
@@ -513,6 +530,12 @@ __global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ in, long lon
         in + pl * in_plane + ((static_cast<long long>(b) * H + (y >> 1)) * W + (x >> 1)) * C + c));
     *reinterpret_cast<uint4*>(out + pl * out_plane + ((static_cast<long long>(b) * 2 * H + y) * 2 * W + x) * C + c) = v;
   }
+}
+
+// 16-bit output of the CUDA-core producers: split-bf16 (lo plane `plane` elements after hi, plane > 0) or single-plane
+// fp16 (plane == 0); both are stored 4 elements (8 bytes) at a time.
+static bool out16_ok(const void* hi, long long plane) {
+  return hi == nullptr || (plane >= 0 && plane % 4 == 0 && (reinterpret_cast<uintptr_t>(hi) & 7) == 0);
 }
 
 static int grid_for(long long work_items, int block) {
@@ -629,7 +652,13 @@ extern "C" int fgt_rownorm_bcast(const float* a, int ca, int lda, const float* b
   for (int q = 0; q < kNormMaxDst; ++q)
     dst.hi[q] = q < n_out ? reinterpret_cast<__nv_bfloat16*>(out_his_host[q]) : nullptr;
   dst.n = n_out;
-  for (int q = 0; q < n_out; ++q) FGT_REQUIRE(dst.hi[q], FGT_ERR_ARG, "rownorm: destination %d is NULL", q);
+  for (int q = 0; q < n_out; ++q) {
+    FGT_REQUIRE(dst.hi[q], FGT_ERR_ARG, "rownorm: destination %d is NULL", q);
+    FGT_REQUIRE(out16_ok(dst.hi[q], out_plane), FGT_ERR_ARG,
+                "rownorm: destination %d misaligned or plane offset %lld not a non-negative multiple of 4", q, out_plane);
+  }
+  FGT_REQUIRE(out_plane != 0 || n_out == 1, FGT_ERR_ARG,
+              "rownorm: single-plane fp16 output (out_plane = 0) takes one destination, got %d", n_out);
   FGT_REQUIRE(a && ca % 4 == 0 && cb % 4 == 0 && C <= 128 * kNormMaxVec && lda % 4 == 0 && (cb == 0 || (b && ldb % 4 == 0)),
               FGT_ERR_ARG, "rownorm: ca=%d cb=%d lda=%d ldb=%d", ca, cb, lda, ldb);
   FGT_REQUIRE(rows_per_batch >= 1 && total_rows >= 1, FGT_ERR_ARG, "rownorm: rows");
@@ -656,6 +685,8 @@ extern "C" int fgt_dwconv3x3_res(const float* x, int bt, int h, int w, int C, co
                                  float* out, void* out_hi, long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(x && weight && bias && out, FGT_ERR_ARG, "dwconv3x3_res: null argument");
   FGT_REQUIRE(C % 4 == 0, FGT_ERR_ARG, "dwconv3x3_res: C=%d must be a multiple of 4", C);
+  FGT_REQUIRE(out16_ok(out_hi, out_plane), FGT_ERR_ARG,
+              "dwconv3x3_res: 16-bit output misaligned or plane offset %lld not a non-negative multiple of 4", out_plane);
   const int tx = (C / 4) < 128 ? (C / 4 + 31) / 32 * 32 : 128;   // threads along channels (x), tokens of the row along y
   launch_k(dwconv3_res_kernel, dim3(bt * h, w >= 16 ? 4 : 1), dim3(tx, 256 / tx > 0 ? 256 / tx : 1), 0, reinterpret_cast<cudaStream_t>(stream), 
       x, bt, h, w, C, weight, bias, out, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
@@ -668,6 +699,8 @@ extern "C" int fgt_fold(const float* hid, int bt, int th, int tw, int C, int kh,
                         fgt_stream_t stream) {
   FGT_REQUIRE(hid && C % 4 == 0 && (out || out_hi), FGT_ERR_ARG, "fold: C=%d", C);
   FGT_REQUIRE(C / 4 <= 64, FGT_ERR_ARG, "fold: C=%d > 256", C);
+  FGT_REQUIRE(out16_ok(out_hi, out_plane), FGT_ERR_ARG,
+              "fold: 16-bit output misaligned or plane offset %lld not a non-negative multiple of 4", out_plane);
   const int gx = (C / 4 + 1) / 2 * 2;  // channel groups per row of the thread block
   const dim3 blk(gx, 256 / gx);
   launch_k(fold_kernel, dim3(bt * OH), dim3(blk), 0, reinterpret_cast<cudaStream_t>(stream), 
@@ -693,6 +726,8 @@ extern "C" int fgt_fold_unfold(const float* hid, int bt, int th, int tw, int C, 
                                int OH, int OW, int relu, void* out_hi, long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(hid && out_hi && C % 4 == 0 && C / 4 <= 64, FGT_ERR_ARG, "fold_unfold: C=%d", C);
   FGT_REQUIRE(kh >= stride && kw >= stride, FGT_ERR_ARG, "fold_unfold: kernel %dx%d must cover the stride %d", kh, kw, stride);
+  FGT_REQUIRE(out16_ok(out_hi, out_plane), FGT_ERR_ARG,
+              "fold_unfold: output misaligned or plane offset %lld not a non-negative multiple of 4", out_plane);
   // every pixel of the map must lie under at least one patch (last patch ends at (th-1)*stride + kh - 1 - pad)
   FGT_REQUIRE((th - 1) * stride + kh - pad >= OH && (tw - 1) * stride + kw - pad >= OW && pad < kh && pad < kw, FGT_ERR_ARG,
               "fold_unfold: patches do not cover the %dx%d map", OH, OW);

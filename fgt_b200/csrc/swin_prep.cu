@@ -47,7 +47,11 @@ __device__ __forceinline__ void swin_norm_store(const float4 (&val)[kMaxVec], in
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int v = lane + 32 * i;
-    if (v < nvec) {
+    if (v < nvec && plane == 0) {  // single-plane fp16 rows (mixed precision)
+      *reinterpret_cast<uint2*>(hi + v * 4) =
+          make_uint2(pack_f16x2((val[i].x - mean) * rstd, (val[i].y - mean) * rstd),
+                     pack_f16x2((val[i].z - mean) * rstd, (val[i].w - mean) * rstd));
+    } else if (v < nvec) {
       uint32_t h0, l0, h1, l1;
       split_bf16x2((val[i].x - mean) * rstd, (val[i].y - mean) * rstd, h0, l0);
       split_bf16x2((val[i].z - mean) * rstd, (val[i].w - mean) * rstd, h1, l1);
@@ -60,7 +64,7 @@ __device__ __forceinline__ void swin_norm_store(const float4 (&val)[kMaxVec], in
 __device__ __forceinline__ void swin_zero_row(__nv_bfloat16* __restrict__ hi, long long plane, int nvec, int lane) {
   for (int v = lane; v < nvec; v += 32) {
     *reinterpret_cast<uint2*>(hi + v * 4) = make_uint2(0u, 0u);
-    *reinterpret_cast<uint2*>(hi + plane + v * 4) = make_uint2(0u, 0u);
+    if (plane) *reinterpret_cast<uint2*>(hi + plane + v * 4) = make_uint2(0u, 0u);
   }
 }
 
@@ -209,6 +213,11 @@ extern "C" int fgt_swin_prep(const float* x, const float* fp, int d, int df, int
   FGT_REQUIRE(bt >= 1 && h >= 1 && w >= 1 && nl >= 1 && gd >= 1 && gh >= 1 && gw >= 1 && R >= nl + gh * gw, FGT_ERR_ARG,
               "swin_prep: geometry bt=%d h=%d w=%d nl=%d R=%d gd=%d gh=%d gw=%d", bt, h, w, nl, R, gd, gh, gw);
   FGT_REQUIRE(qkn_plane % 4 == 0 && vn_plane % 4 == 0, FGT_ERR_ARG, "swin_prep: plane offsets");
+  FGT_REQUIRE(qkn_plane >= 0 && vn_plane >= 0 && (qkn_plane == 0) == (vn_plane == 0), FGT_ERR_ARG,
+              "swin_prep: qkn and vn are both split-bf16 (plane > 0) or both single-plane fp16 (plane 0), got %lld / %lld",
+              qkn_plane, vn_plane);
+  FGT_REQUIRE(((reinterpret_cast<uintptr_t>(qkn_hi) | reinterpret_cast<uintptr_t>(vn_hi)) & 7) == 0, FGT_ERR_ARG,
+              "swin_prep: outputs must be 8-byte aligned");
   fgt::SwinPrepArgs a;
   a.x = x; a.fp = fp; a.d = d; a.df = df; a.bt = bt; a.h = h; a.w = w; a.win_map = win_map; a.nl = nl; a.R = R;
   a.gd = gd; a.gh = gh; a.gw = gw; a.gk_w = gk_w; a.gk_b = gk_b; a.gv_w = gv_w; a.gv_b = gv_b;

@@ -135,6 +135,11 @@ class _Decoder(nn.Module):
 # layer class needs the 3-term split product: each costs 2e-4..7e-4 end to end on its own even in fp16.
 _FLOW_TERMS = int(os.environ.get("FGT_FLOW_TERMS", "1"))
 
+def _terms(wp):
+    """MMA terms of a packed layer: 1 for fp16 weights (single-plane fp16 operands), 3 for split-bf16 ones."""
+    return 1 if wp["w"].dtype == torch.float16 else 3
+
+
 def _pick_bn(n_per_group, groups):
     if n_per_group % 128 == 0:
         return 128
@@ -201,8 +206,9 @@ class FGT(nn.Module):
         self.decoder = _Decoder(cnum * 2, 3)
         if init_weights:
             self.init_weights()
-        self._packed = None
+        self._packed = {}   # precision (half: bool) -> packed weights
         self._geo = {}
+        self._mixed = False
         self.capture = None  # set to a dict to record intermediate activations (tests)
 
     def _cap(self, name, t):
@@ -221,17 +227,17 @@ class FGT(nn.Module):
     def _drop_graphs(self):
         """Captured CUDA graphs bake in the addresses of the packed weights and workspaces: whenever those are
         re-created (new weights, .to(), .float() ...) the captures must go too, or a replay reads freed memory."""
-        if getattr(self, "_graphed", None) is not None:
-            self._graphed.entries.clear()
+        for gc in (getattr(self, "_graphed", None) or {}).values():
+            gc.entries.clear()
 
     def _apply(self, fn, *a, **k):
-        self._packed = None
+        self._packed = {}
         self._geo = {}
         self._drop_graphs()
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, *a, **k):
-        self._packed = None
+        self._packed = {}
         self._drop_graphs()
         return super().load_state_dict(*a, **k)
 
@@ -241,12 +247,18 @@ class FGT(nn.Module):
         idx = torch.arange(P * c).reshape(c, P).t().reshape(-1)  # new[p*c + ci] = old[ci*P + p]
         return idx
 
-    def _pack(self, dev):
+    def _pack(self, dev, half=False):
+        """half: the mixed-precision set. Every layer of the generator is a 1-term fp16 layer: weights and biases are
+        rounded to fp16 once (the casts autocast applies to a Linear's / conv's parameters), LayerNorm affines folded
+        into a Linear are folded in fp64 first. LayerNorm affines applied by the norm kernel stay fp32 (autocast runs
+        layer_norm in fp32)."""
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
         P = {}
+        rnd = (lambda t: t.half().float()) if half else (lambda t: t)  # noqa: E731
 
         def put(name, w, b, segs=None):
-            P[name] = dict(w=pack_weight(w, segs).to(dev), b=b.float().contiguous().to(dev), N=w.shape[0], name=name)
+            P[name] = dict(w=pack_weight(rnd(w), segs, half=half).to(dev), b=rnd(b.float()).contiguous().to(dev),
+                           N=w.shape[0], name=name)
 
         def conv(name, key, segs=None):
             put(name, sd[key + ".weight"], sd[key + ".bias"], segs)
@@ -255,10 +267,10 @@ class FGT(nn.Module):
         for i in (2, 4, 6, 8):
             conv(f"enc{i}", enc + str(i))
         # tiny-channel first layers consume im2col rows (fgt_im2col_nchw): one K=64 GEMM each
-        fh = _FLOW_TERMS == 1
-        for name, key, half in (("enc0", enc + "0", False), ("fenc1", "flow_encoder.1.featureConv", fh)):
-            P[name] = dict(w=pack_weight_im2col(sd[key + ".weight"], half=half).to(dev),
-                           b=sd[key + ".bias"].contiguous().to(dev), N=sd[key + ".weight"].shape[0], name=name)
+        fh = _FLOW_TERMS == 1 or half
+        for name, key, h16 in (("enc0", enc + "0", half), ("fenc1", "flow_encoder.1.featureConv", fh)):
+            P[name] = dict(w=pack_weight_im2col(sd[key + ".weight"], half=h16).to(dev),
+                           b=rnd(sd[key + ".bias"]).contiguous().to(dev), N=sd[key + ".weight"].shape[0], name=name)
         conv("enc10", enc + "10", [128, 192])
         conv("enc12", enc + "12", [64, 128])
         # enc14 (8 groups of 32+48 -> 32 channels) as 2 super-groups of 4 with block-diagonal weights: the engine then
@@ -275,15 +287,15 @@ class FGT(nn.Module):
         conv("enc16", enc + "16", [256, 256])
         for name, key in (("fenc2", "flow_encoder.2.featureConv"), ("fenc3", "flow_encoder.3.featureConv"),
                           ("fenc4", "flow_encoder.4.featureConv"), ("f_patch2vec", "f_patch2vec")):
-            P[name] = dict(w=pack_weight(sd[key + ".weight"], half=fh).to(dev), b=sd[key + ".bias"].contiguous().to(dev),
-                           N=sd[key + ".weight"].shape[0], name=name)
+            P[name] = dict(w=pack_weight(sd[key + ".weight"], half=fh).to(dev),
+                           b=rnd(sd[key + ".bias"]).contiguous().to(dev), N=sd[key + ".weight"].shape[0], name=name)
         conv("patch2vec", "patch2vec")
-        P["pos_w"] = sd["add_pos_emb.proj.weight"].reshape(-1).contiguous().to(dev)
-        P["pos_b"] = sd["add_pos_emb.proj.bias"].contiguous().to(dev)
+        P["pos_w"] = rnd(sd["add_pos_emb.proj.weight"]).reshape(-1).contiguous().to(dev)
+        P["pos_b"] = rnd(sd["add_pos_emb.proj.bias"]).contiguous().to(dev)
         perm_ffn = self._perm_hidden(self.mlp_c).to(sd["patch2vec.weight"].device)
 
         def ffn(pre, name, gamma, beta):
-            w1, b1 = fold_layernorm(sd[pre + "ffn.conv1.weight"], sd[pre + "ffn.conv1.bias"], gamma, beta)
+            w1, b1 = fold_layernorm(sd[pre + "ffn.conv1.weight"], sd[pre + "ffn.conv1.bias"], gamma, beta, half=half)
             put(name + ".ffn1", w1[perm_ffn], b1[perm_ffn])
             put(name + ".ffn2", sd[pre + "ffn.conv2.2.weight"][:, perm_ffn], sd[pre + "ffn.conv2.2.bias"])
 
@@ -302,19 +314,19 @@ class FGT(nn.Module):
             a = pre + "attention."
             put(name + ".gate", sd[a + "reweightFlow.0.weight"], sd[a + "reweightFlow.0.bias"], [self.d, self.df])
             wq, bq = fold_layernorm(sd[a + "query_embedding.weight"], sd[a + "query_embedding.bias"],
-                                    sd[a + "q_norm.weight"], sd[a + "q_norm.bias"])
+                                    sd[a + "q_norm.weight"], sd[a + "q_norm.bias"], half=half)
             wk, bk = fold_layernorm(sd[a + "key_embedding.weight"], sd[a + "key_embedding.bias"],
-                                    sd[a + "k_norm.weight"], sd[a + "k_norm.bias"])
+                                    sd[a + "k_norm.weight"], sd[a + "k_norm.bias"], half=half)
             wv, bv = fold_layernorm(sd[a + "value_embedding.weight"], sd[a + "value_embedding.bias"],
-                                    sd[a + "v_norm.weight"], sd[a + "v_norm.bias"])
+                                    sd[a + "v_norm.weight"], sd[a + "v_norm.bias"], half=half)
             put(name + ".qk", torch.cat([wq, wk], 0), torch.cat([bq, bk], 0))
             put(name + ".v", wv, bv)
             put(name + ".o", sd[a + "output_linear.weight"], sd[a + "output_linear.bias"])
             # depthwise pooling weights tap-major [gd*gd, C] (fgt_swin_prep reads one coalesced row per tap)
-            P[name + ".gk_w"] = sd[a + "global_extract_k.weight"].reshape(self.d + self.df, -1).t().contiguous().to(dev)
-            P[name + ".gk_b"] = sd[a + "global_extract_k.bias"].contiguous().to(dev)
-            P[name + ".gv_w"] = sd[a + "global_extract_v.weight"].reshape(self.d, -1).t().contiguous().to(dev)
-            P[name + ".gv_b"] = sd[a + "global_extract_v.bias"].contiguous().to(dev)
+            P[name + ".gk_w"] = rnd(sd[a + "global_extract_k.weight"]).reshape(self.d + self.df, -1).t().contiguous().to(dev)
+            P[name + ".gk_b"] = rnd(sd[a + "global_extract_k.bias"]).contiguous().to(dev)
+            P[name + ".gv_w"] = rnd(sd[a + "global_extract_v.weight"]).reshape(self.d, -1).t().contiguous().to(dev)
+            P[name + ".gv_b"] = rnd(sd[a + "global_extract_v.bias"]).contiguous().to(dev)
             ffn(pre, name, sd[pre + "norm.weight"], sd[pre + "norm.bias"])
 
         tblock("first_t_transformer.", "t0")
@@ -328,7 +340,7 @@ class FGT(nn.Module):
         # only sees 2x2 low-res inputs, so each deconv becomes four 2x2 "phase" convs on the low-res map with
         # pre-summed taps (2.25x fewer MACs, no upsampled intermediate): rows {i-1,i} for py=0, {i,i+1} for py=1.
         def deconv(name, key):
-            w, b = sd[key + ".weight"], sd[key + ".bias"]
+            w, b = rnd(sd[key + ".weight"]), sd[key + ".bias"]  # mixed: the fp16 taps are summed, then rounded once
             rows = {0: ([0], [1, 2]), 1: ([0, 1], [2])}  # phase -> 3x3 tap indices merged into each of the 2 taps
             for py in (0, 1):
                 for px in (0, 1):
@@ -343,17 +355,18 @@ class FGT(nn.Module):
         # final 64->3 conv as "taps as N": a 1x1 GEMM with N = 9*3 (padded to 32) + fgt_tapsum (shift, add, bias, tanh)
         w4 = sd["decoder.final.featureConv.weight"]
         put("dec4t", lib.pack_taps_as_n(w4), torch.zeros(32))
-        self._packed = P
+        self._packed[half] = P
         return P
 
     # ------------------------------------------------------------------ geometry / workspaces
-    def _geometry(self, b, t, H, W, dev):
-        key = (b, t, H, W, str(dev))
+    def _geometry(self, b, t, H, W, dev, mixed=False):
+        key = (b, t, H, W, str(dev), mixed)
         if key in self._geo:
             return self._geo[key]
         if H % 4 or W % 4:
             raise ValueError(f"FGT input {H}x{W} must be divisible by 4 (model.py:55-63 views features as H//4 x W//4)")
         g = type("Geo", (), {})()
+        g.mixed = mixed  # workspaces of the mixed-precision path: single-plane fp16 where the fp32 path is split-bf16
         bt = b * t
         g.b, g.t, g.bt, g.H, g.W = b, t, bt, H, W
         g.OH, g.OW = H // 4, W // 4
@@ -400,7 +413,9 @@ class FGT(nn.Module):
     @staticmethod
     def _buf(g, name, shape, dev, dtype=torch.float32, split=False, zero=False):
         if name not in g.bufs:
-            if split:
+            if split and g.mixed:
+                dtype = torch.float16
+            elif split:
                 shape = (2,) + tuple(shape)
                 dtype = torch.bfloat16
             g.bufs[name] = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=dev)
@@ -409,8 +424,10 @@ class FGT(nn.Module):
     # ------------------------------------------------------------------ op helpers
     @staticmethod
     def _conv(x, cin, n, h, w, wp, k, *, stride=1, pad=None, act=lib.ACT_LEAKY02, out_split=None, out_f32=None,
-              extra_seg=None, groups=1, seg_counts=None, nchw_out=False, terms=3, out_f16=None, alg_k=None):
-        """NHWC split x [2,n,h,w,cin] (+ optional second segment) -> conv -> NHWC outputs."""
+              extra_seg=None, groups=1, seg_counts=None, nchw_out=False, terms=None, out_f16=None, alg_k=None):
+        """NHWC split x [2,n,h,w,cin] (+ optional second segment) -> conv -> NHWC outputs. terms: 1 for fp16 weights
+        (single-plane fp16 operands), 3 otherwise."""
+        terms = _terms(wp) if terms is None else terms
         pad = k // 2 if pad is None else pad
         oh = (h + 2 * pad - k) // stride + 1
         ow = (w + 2 * pad - k) // stride + 1
@@ -443,12 +460,13 @@ class FGT(nn.Module):
                 wp = P[f"{name}.p{py}{px}"]
                 N = wp["N"]
                 lib.gemm_tc([lib.ASeg(x, cin, w, h, n)], wp["w"], N, kx=2, ky=2, pad_x=1 - px, pad_y=1 - py, out_w=w,
-                            out_h=h, out_z=n, box_w=bw, box_h=bh, bn=_pick_bn(N, 1), bias=wp["b"],
+                            out_h=h, out_z=n, box_w=bw, box_h=bh, bn=_pick_bn(N, 1), bias=wp["b"], terms=_terms(wp),
                             act=lib.ACT_LEAKY02, out_split=out_split, out_elem_offset=(py * 2 * w + px) * N,
                             os_z=4 * h * w * N, os_y=4 * w * N, os_x=2 * N, os_c=1, tag=wp["name"])
 
     @staticmethod
     def _linear(segs, wp, rows, bn=None, **kw):
+        kw.setdefault("terms", _terms(wp))
         lib.gemm_tc(segs, wp["w"], wp["N"], out_w=rows,
                     bn=bn or _fill_sms(_pick_bn(wp["N"], 1), wp["N"], rows), bias=wp["b"], tag=wp["name"], **kw)
 
@@ -486,6 +504,8 @@ class FGT(nn.Module):
         if total_frames is None:
             self._fshard = None
             return
+        if self._mixed:
+            raise ValueError("frame sharding runs the fp32 path only: call enable_mixed_precision(False) first")
         import torch.distributed as dist
         from . import parallel
         if exchange not in ("p2p", "nccl"):
@@ -646,9 +666,23 @@ class FGT(nn.Module):
 
     # ------------------------------------------------------------------ forward
     def enable_cuda_graph(self, on=True):
-        """Replay the whole forward as one CUDA graph per input geometry (fgt_b200/graphs.py)."""
+        """Replay the whole forward as one CUDA graph per input geometry and precision (fgt_b200/graphs.py)."""
         from .graphs import GraphedCall
-        self._graphed = GraphedCall(self._forward_impl) if on else None
+        self._graphed = {m: GraphedCall(lambda *a, _m=m: self._forward_impl(*a, mixed=_m)) for m in (False, True)} \
+            if on else None
+
+    def enable_mixed_precision(self, on=True):
+        """Mixed precision, opt-in: the generator runs as the reference does under
+        torch.autocast("cuda", dtype=torch.float16). Every Linear / conv is a 1-term fp16 tensor-core GEMM (fp16
+        weights and activation rows, fp32 accumulation), the attention takes fp16 Q, K, V with its scores and softmax
+        in fp32, LayerNorm statistics stay fp32. The fp16 weights, workspaces and CUDA graphs are kept apart from the
+        fp32 path's, so the flag may change between calls; off (the default) gives the fp32 path's outputs bit for
+        bit. Not available with frame sharding. DESIGN.md section 2 lists where the rounding points differ from
+        autocast."""
+        if on and getattr(self, "_fshard", None) is not None:
+            raise ValueError("mixed precision is not available with frame sharding: call enable_frame_sharding(None) "
+                             "first")
+        self._mixed = bool(on)
 
     def forward(self, masked_frames, flows, masks):
         if not masked_frames.is_cuda:
@@ -656,11 +690,11 @@ class FGT(nn.Module):
         fs = getattr(self, "_fshard", None)
         graph_ok = fs is None or fs["exchange"] == "p2p"  # NCCL calls are not captured; the P2P exchange is kernels only
         if getattr(self, "_graphed", None) is not None and self.capture is None and graph_ok:
-            return self._graphed(masked_frames.float().contiguous(), flows.float().contiguous(),
-                                 masks.float().contiguous())
-        return self._forward_impl(masked_frames, flows, masks)
+            return self._graphed[self._mixed](masked_frames.float().contiguous(), flows.float().contiguous(),
+                                              masks.float().contiguous())
+        return self._forward_impl(masked_frames, flows, masks, mixed=self._mixed)
 
-    def _forward_impl(self, masked_frames, flows, masks):
+    def _forward_impl(self, masked_frames, flows, masks, mixed=False):
         dev = masked_frames.device
         b, t, c, H, W = masked_frames.shape
         bt = b * t
@@ -671,8 +705,8 @@ class FGT(nn.Module):
         if fs is not None and fs["exchange"] == "p2p":
             fs["layer"] = 0
             fs["peer"].barrier()  # every peer has finished reading the exchange buffers of the previous forward
-        P = self._packed if self._packed is not None else self._pack(dev)
-        g = self._geometry(b, t, H, W, dev)
+        P = self._packed[mixed] if mixed in self._packed else self._pack(dev, mixed)
+        g = self._geometry(b, t, H, W, dev, mixed)
         B = lambda name, shape, **kw: self._buf(g, name, shape, dev, **kw)  # noqa: E731
         frames = masked_frames.reshape(bt, c, H, W).float().contiguous()
         mk = masks.reshape(bt, 1, H, W).float().contiguous()
@@ -709,19 +743,20 @@ class FGT(nn.Module):
         # ---- flow encoder (model.py:206-212)
         lib._scope[-1] = "flow_encoder"
         # 1-term mode: the branch's activations are single-plane fp16 tensors; 3-term mode: split-bf16 like the rest
-        fkw = dict(dtype=torch.float16) if _FLOW_TERMS == 1 else dict(split=True)
-        okey = "out_f16" if _FLOW_TERMS == 1 else "out_split"
+        flow16 = _FLOW_TERMS == 1 or mixed
+        fkw = dict(dtype=torch.float16) if flow16 else dict(split=True)
+        okey = "out_f16" if flow16 else "out_split"
         fcol = B("f_col", (bt, H, W, 64), **fkw)
         lib.im2col_nchw(fl, None, fcol, k=5, stride=1, pad=2, replicate=True, OH=H, OW=W, tag="fenc1")
         f1 = B("f1", (bt, H, W, 64), **fkw)
         f2 = B("f2", (bt, H2, W2, 128), **fkw)
         f3 = B("f3", (bt, H2, W2, 128), **fkw)
         f4 = B("f4", (bt, OH, OW, 128), **fkw)
-        self._linear([lib.ASeg(fcol, 64, bt * H * W)], P["fenc1"], bt * H * W, act=lib.ACT_LEAKY02, terms=_FLOW_TERMS,
+        self._linear([lib.ASeg(fcol, 64, bt * H * W)], P["fenc1"], bt * H * W, act=lib.ACT_LEAKY02,
                      **{okey: f1})
-        self._conv(f1, 64, bt, H, W, P["fenc2"], 3, stride=2, terms=_FLOW_TERMS, **{okey: f2})
-        self._conv(f2, 128, bt, H2, W2, P["fenc3"], 3, terms=_FLOW_TERMS, **{okey: f3})
-        self._conv(f3, 128, bt, H2, W2, P["fenc4"], 3, stride=2, terms=_FLOW_TERMS, **{okey: f4})
+        self._conv(f1, 64, bt, H, W, P["fenc2"], 3, stride=2, **{okey: f2})
+        self._conv(f2, 128, bt, H2, W2, P["fenc3"], 3, **{okey: f3})
+        self._conv(f3, 128, bt, H2, W2, P["fenc4"], 3, stride=2, **{okey: f4})
         # ---- patch embedding (model.py:261-262,270-271): conv output NHWC == token-major
         lib._scope[-1] = "patch_embed"
         rows = bt * g.n
@@ -733,7 +768,7 @@ class FGT(nn.Module):
         k, s, p = self.ksz[0], self.stride[0], self.padding[0]
         self._conv(enc, 128, bt, OH, OW, P["patch2vec"], k, stride=s, pad=p, act=lib.ACT_NONE, out_f32=xa)
         self._conv(f4, 128, bt, OH, OW, P["f_patch2vec"], k, stride=s, pad=p, act=lib.ACT_NONE, out_f32=f,
-                   out_split=fs, terms=_FLOW_TERMS)
+                   out_split=fs)
         self._cap("enc", enc_f)
         self._cap("tok0", xa)
         self._cap("ftok", f)

@@ -50,7 +50,8 @@ class FgtAttnDesc(ctypes.Structure):
                 ("batches", ctypes.c_int), ("heads", ctypes.c_int), ("head_dim", ctypes.c_int),
                 ("Lq", ctypes.c_int), ("Lk", ctypes.c_int), ("Lk_rows", ctypes.c_int),
                 ("scale", ctypes.c_float), ("mode", ctypes.c_int),
-                ("glob_start", ctypes.c_int), ("glob_count", ctypes.c_int), ("out_rowmap", _c_p)]
+                ("glob_start", ctypes.c_int), ("glob_count", ctypes.c_int), ("out_rowmap", _c_p),
+                ("f16", ctypes.c_int)]
 
 
 _lib = None
@@ -302,8 +303,11 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
             os_z=0, os_y=0, os_x=None, os_c=1, rowmap=None, lin_batch=0, aux2=None, terms=3, out_f16=None, alg_k=None,
             tag=""):
     """Generic launcher for fgt_gemm_tc. Output strides are in elements; see include/fgt_b200.h.
-    terms=1: the A segments' tensors and w_split are plain fp16 tensors (one plane); out_f16: plain fp16 output."""
+    terms=1: the A segments' tensors and w_split are plain fp16 tensors (one plane); out_f16: plain fp16 output
+    (an fp16 tensor passed as out_split is taken as out_f16)."""
     lib = load()
+    if out_split is not None and out_split.dtype == torch.float16:
+        out_split, out_f16 = None, out_split
     d = FgtGemmDesc()
     d.num_segs = len(segs)
     k_real = 0
@@ -359,14 +363,16 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
 def attention(q, k, v, out, *, batches, heads, Lq, Lk, Lk_rows=None, q_ld, k_ld, v_ld, out_ld,
               q_batch_stride, k_batch_stride, v_batch_stride, out_batch_stride, scale, mode=0,
               glob_start=0, glob_count=0, q_off=0, k_off=0, v_off=0, out_rowmap=None, tag=""):
-    """fgt_attention launcher. q/k/v/out are split-bf16 row-major tensors; strides in elements; q_off/k_off/v_off
-    are element offsets into the plane (e.g. when Q, K and V share one [rows, 3*C] projection buffer)."""
+    """fgt_attention launcher. q/k/v/out are split-bf16 row-major tensors, or all four plain fp16 tensors (the
+    single-plane fp16 mode); strides in elements; q_off/k_off/v_off are element offsets into the plane (e.g. when Q,
+    K and V share one [rows, 3*C] projection buffer)."""
     lib = load()
     d = FgtAttnDesc()
-    d.q_hi, d.q_plane, d.q_batch_stride, d.q_ld = q.data_ptr() + 2 * q_off, plane_elems(q), q_batch_stride, q_ld
-    d.k_hi, d.k_plane, d.k_batch_stride, d.k_ld = k.data_ptr() + 2 * k_off, plane_elems(k), k_batch_stride, k_ld
-    d.v_hi, d.v_plane, d.v_batch_stride, d.v_ld = v.data_ptr() + 2 * v_off, plane_elems(v), v_batch_stride, v_ld
-    d.out_hi, d.out_plane, d.out_batch_stride, d.out_ld = out.data_ptr(), plane_elems(out), out_batch_stride, out_ld
+    d.f16 = 1 if q.dtype == torch.float16 else 0
+    d.q_hi, d.q_plane, d.q_batch_stride, d.q_ld = q.data_ptr() + 2 * q_off, _plane16(q), q_batch_stride, q_ld
+    d.k_hi, d.k_plane, d.k_batch_stride, d.k_ld = k.data_ptr() + 2 * k_off, _plane16(k), k_batch_stride, k_ld
+    d.v_hi, d.v_plane, d.v_batch_stride, d.v_ld = v.data_ptr() + 2 * v_off, _plane16(v), v_batch_stride, v_ld
+    d.out_hi, d.out_plane, d.out_batch_stride, d.out_ld = out.data_ptr(), _plane16(out), out_batch_stride, out_ld
     d.batches, d.heads, d.head_dim = batches, heads, 128
     d.Lq, d.Lk = Lq, Lk
     d.Lk_rows = Lk if Lk_rows is None else Lk_rows
@@ -409,12 +415,13 @@ def im2col_nchw(src0, src1, out_split, *, k, stride, pad, replicate, OH, OW, sca
 
 def rownorm(a, b, out_split, *, gather=None, rows_per_batch, total_rows, dst_batch_rows, dst_row0=0, eps=1e-5,
             gamma=None, beta=None, tag=""):
+    """out_split: split-bf16 [2, ...] or a plain fp16 tensor (single-plane rows of a 1-term layer)."""
     ca, lda = a.shape[-1], a.shape[-1]
     cb, ldb = (b.shape[-1], b.shape[-1]) if b is not None else (0, 0)
     with _Prof("rownorm", tag, 0, 8.0 * total_rows * (ca + cb)):
         check(load().fgt_rownorm(_dp(a), ca, lda, _dp(b), cb, ldb, _dp(gather), rows_per_batch, total_rows,
                                  dst_batch_rows, dst_row0, _dp(gamma), _dp(beta), _dp(out_split),
-                                 plane_elems(out_split), eps, stream_ptr()), "fgt_rownorm")
+                                 _plane16(out_split), eps, stream_ptr()), "fgt_rownorm")
 
 
 def rownorm_bcast(a, dst_ptrs, plane, *, gather=None, rows_per_batch, total_rows, dst_batch_rows, dst_row0=0, eps=1e-5,
@@ -459,39 +466,41 @@ def dwpool(a, b, bt, h, w, k, gh, gw, weight, bias, out, tag=""):
 
 def conv_tail(x_split, n, H, W, cin, w_split, cout, bias, act, out, *, nchw, tag=""):
     """3x3 conv (pad 1) with cout <= 3 + bias + activation: x_split [2,n,H,W,cin] -> out [n,cout,H,W] (nchw) or
-    [n,H,W,cout] fp32, one kernel (taps-as-N GEMM + in-SM tap sum). w_split = pack_weight(pack_taps_as_n(w))."""
+    [n,H,W,cout] fp32, one kernel (taps-as-N GEMM + in-SM tap sum). w_split = pack_weight(pack_taps_as_n(w)).
+    x_split and w_split may instead both be plain fp16 tensors (1-term fp16 MMAs)."""
     st = (cout * H * W, H * W, W, 1) if nchw else (H * W * cout, 1, W * cout, cout)
     # 2*9*cout*cin FLOP per 4*(cin+cout) bytes = ~13 FLOP/B at 64 -> 3: HBM-bound, reported against the copy roofline
     nbytes = 4.0 * n * H * W * (cin + cout)
     with _Prof("conv_tail", tag, 0.0, nbytes):
-        check(load().fgt_conv_tail(_dp(x_split), plane_elems(x_split), n, H, W, cin, _dp(w_split), plane_elems(w_split),
+        check(load().fgt_conv_tail(_dp(x_split), _plane16(x_split), n, H, W, cin, _dp(w_split), _plane16(w_split),
                                    w_split.shape[-1], cout, _dp(bias), act, _dp(out), *st, stream_ptr()), "fgt_conv_tail")
 
 
 def swin_prep(x, fp, bt, h, w, win_map, nl, R, gd, gh, gw, gk_w, gk_b, gv_w, gv_b, qkn, vn, eps=1e-5, tag=""):
     """SWMHSA operand preparation in one launch: LayerNorm'd window rows and pooled global rows of [x ; f'] -> qkn
-    and of x -> vn (split-bf16 [bt*R, .]); see include/fgt_b200.h."""
+    and of x -> vn (split-bf16 [bt*R, .], or both plain fp16); see include/fgt_b200.h."""
     d, df = x.shape[-1], fp.shape[-1]
     G = gh * gw
     nbytes = 4.0 * bt * ((nl + 2 * h * w) * (d + df) + (nl + G) * (2 * d + df))  # reads (rows + pooling) + split writes
     with _Prof("swin_prep", tag, 0, nbytes):
         check(load().fgt_swin_prep(_dp(x), _dp(fp), d, df, bt, h, w, _dp(win_map), nl, R, gd, gh, gw, _dp(gk_w),
-                                   _dp(gk_b), _dp(gv_w), _dp(gv_b), _dp(qkn), plane_elems(qkn), _dp(vn),
-                                   plane_elems(vn), eps, stream_ptr()), "fgt_swin_prep")
+                                   _dp(gk_b), _dp(gv_w), _dp(gv_b), _dp(qkn), _plane16(qkn), _dp(vn),
+                                   _plane16(vn), eps, stream_ptr()), "fgt_swin_prep")
 
 
 def dwconv3x3_res(x, bt, h, w, C, weight, bias, out, out_split=None, tag=""):
+    """out_split (optional 16-bit copy): split-bf16 or plain fp16."""
     with _Prof("dwconv3x3_res", tag, 0, 12.0 * bt * h * w * C):
         check(load().fgt_dwconv3x3_res(_dp(x), bt, h, w, C, _dp(weight), _dp(bias), _dp(out), _dp(out_split),
-                                       plane_elems(out_split) if out_split is not None else 0, stream_ptr()),
+                                       _plane16(out_split), stream_ptr()),
               "fgt_dwconv3x3_res")
 
 
 def fold(hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, *, normalize, add=None, out=None, out_split=None, tag=""):
+    """out_split (optional 16-bit output): split-bf16 or plain fp16."""
     with _Prof("fold", tag, 0, 4.0 * bt * (th * tw * kh * kw * C + OH * OW * C * (2 if add is not None else 1))):
         check(load().fgt_fold(_dp(hid), bt, th, tw, C, kh, kw, stride, pad, OH, OW, 1 if normalize else 0, _dp(add),
-                              _dp(out), _dp(out_split), plane_elems(out_split) if out_split is not None else 0,
-                              stream_ptr()), "fgt_fold")
+                              _dp(out), _dp(out_split), _plane16(out_split), stream_ptr()), "fgt_fold")
 
 
 def unfold(img, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu=True, tag=""):
@@ -501,10 +510,11 @@ def unfold(img, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu=True
 
 
 def fold_unfold(hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu=True, tag=""):
-    """fold (normalised) + unfold (+ReLU) of the fusion FFN in one launch: hid fp32 [bt*th*tw, kh*kw*C] -> split."""
+    """fold (normalised) + unfold (+ReLU) of the fusion FFN in one launch: hid fp32 [bt*th*tw, kh*kw*C] -> split-bf16
+    (or plain fp16)."""
     with _Prof("fold_unfold", tag, 0, 8.0 * bt * th * tw * kh * kw * C):
         check(load().fgt_fold_unfold(_dp(hid), bt, th, tw, C, kh, kw, stride, pad, OH, OW, 1 if relu else 0,
-                                     _dp(out_split), plane_elems(out_split), stream_ptr()), "fgt_fold_unfold")
+                                     _dp(out_split), _plane16(out_split), stream_ptr()), "fgt_fold_unfold")
 
 
 def upsample2x(in_split, n, H, W, C, out_split, tag=""):

@@ -43,14 +43,17 @@ def pack_weight(w, seg_counts=None, half=False):
     return packed.to(torch.float16) if half else to_split(packed)
 
 
-def fold_layernorm(weight, bias, gamma, beta):
+def fold_layernorm(weight, bias, gamma, beta, half=False):
     """Folds a LayerNorm affine (gamma, beta) that precedes Linear(weight, bias) into the Linear:
-    W (gamma * n + beta) + b == (W * gamma) n + (W beta + b)."""
+    W (gamma * n + beta) + b == (W * gamma) n + (W beta + b). Computed in fp64, rounded once to fp32 (or, half=True,
+    to fp16 values, returned as fp32 tensors)."""
     w = weight.detach().double()
     g = gamma.detach().double()
     b = beta.detach().double()
     w2 = w * g[None, :]
     b2 = w @ b + (bias.detach().double() if bias is not None else 0.0)
+    if half:
+        return w2.half().float(), b2.half().float()
     return w2.float(), b2.float()
 
 

@@ -578,10 +578,11 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
 
 
 # ------------------------------------------------------------------------------------------------ command line
-def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False):
+def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False, fgt_mixed_precision=False):
     """initialize_RAFT / initialize_LAFC / initialize_FGT (:186-230) with the drop-in modules: the same checkpoint
     layout (a `module.`-prefixed RAFT state dict; directories holding one *.tar with `model_state_dict` and one
-    *.yaml config). mixed_precision: RAFT's fp16 mode (the reference's --mixed_precision). Returns
+    *.yaml config). mixed_precision: RAFT's fp16 mode (the reference's --mixed_precision, RAFT only).
+    fgt_mixed_precision: the FGT generator's fp16 mode (FGT.enable_mixed_precision). Returns
     (GpuBackend, lafc_config)."""
     import glob
     import os
@@ -609,14 +610,13 @@ def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False
     fgt_sd, fgt_cfg = ckpt_dir(fgt_ckpts)
     fgt = FGTModel(fgt_cfg)
     fgt.load_state_dict(fgt_sd)
+    fgt.net.enable_mixed_precision(bool(fgt_mixed_precision))
     # inference only: no BatchNorm / dropout in LAFC or FGT (the driver never calls .eval() on them), but be explicit
     return GpuBackend(raft, lafc.to(device).eval(), fgt.to(device).eval(), device=device), lafc_cfg
 
 
-def main(argv=None):
-    """`python -m fgt_b200.pipeline --path frames/ --path_mask masks/ --outroot out/ [--mode ...] ...` — the driver's
-    command line (:764-855; the visualisation switches are not offered)."""
-    from . import io as IO
+def arg_parser():
+    """The command line of main()."""
     ap = argparse.ArgumentParser(description=main.__doc__)
     ap.add_argument("--path", required=True, help="directory of *.png / *.jpg frames")
     ap.add_argument("--path_mask", default=None, help="directory of masks (non-zero = remove); not needed for video_extrapolation")
@@ -631,16 +631,28 @@ def main(argv=None):
     ap.add_argument("--mixed_precision", action="store_true",
                     help="run RAFT with fp16 tensor-core operands, as the reference's autocast mode (faster, not "
                          "fp32-accurate)")
+    ap.add_argument("--fgt_mixed_precision", action="store_true",
+                    help="run the FGT generator with fp16 tensor-core operands, as the reference under CUDA autocast "
+                         "(faster, not fp32-accurate; independent of --mixed_precision)")
     for k, v in DEFAULTS.items():
         if k == "mode":
             ap.add_argument("--mode", default=v, choices=list(MODES))
         elif k not in ("Nonlocal", "raft_iters"):
             ap.add_argument("--" + k, type=type(v), default=v)
+    return ap
+
+
+def main(argv=None):
+    """`python -m fgt_b200.pipeline --path frames/ --path_mask masks/ --outroot out/ [--mode ...] ...` — the driver's
+    command line (:764-855; the visualisation switches are not offered)."""
+    from . import io as IO
+    ap = arg_parser()
     ns = ap.parse_args(argv)
     if ns.native and ns.mode == "video_extrapolation":
         ap.error("--native: video_extrapolation has no original frame to paste the result into")
     dev = torch.device("cuda", ns.gpu)
-    backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev, ns.mixed_precision)
+    fgt_kw = dict(fgt_mixed_precision=True) if ns.fgt_mixed_precision else {}
+    backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev, ns.mixed_precision, **fgt_kw)
     args = make_args(**{k: getattr(ns, k) for k in DEFAULTS if hasattr(ns, k)})
     frames = IO.read_frames(ns.path)
     masks = IO.read_masks(ns.path_mask, rgb=ns.mode == "watermark_removal") if ns.mode != "video_extrapolation" else [None] * len(frames)

@@ -144,6 +144,8 @@ typedef struct {
   int glob_start, glob_count;   /* windowed mode */
   const int* out_rowmap;        /* optional [batches * Lq]: query row -> row of a [rows, out_ld] output buffer (< 0 = drop);
                                    out_batch_stride is ignored then. Undoes the zone / window regrouping in the store. */
+  int f16;                      /* 1: Q, K, V and the output are single-plane fp16 (every plane offset 0; one fp16 wgmma
+                                   per K step for Q K^T and P V, scores and softmax in fp32); 0: split-bf16 */
 } FgtAttnDesc;
 
 int fgt_attention(const FgtAttnDesc* desc, fgt_stream_t stream);
@@ -173,6 +175,9 @@ int fgt_im2col_nchw(const float* src0, int c0, const float* src1, int c1, int n,
  * gather[d] (or d when gather == NULL); gather[d] < 0 writes a zero row (the reference's F.pad).
  * Replaces nn.LayerNorm at model.py:126,128,147 and attention_flow.py:142-143,154 together with the
  * window / zone partition copies at attention_flow.py:132-133,150-153, attention_base.py:93-98. */
+/* Mixed precision: fgt_rownorm, fgt_swin_prep, fgt_fold, fgt_fold_unfold and fgt_dwconv3x3_res write their 16-bit
+ * output as single-plane fp16 rows when its plane offset is 0 (split-bf16 otherwise); fgt_conv_tail reads fp16
+ * activations and weights when both plane offsets are 0. */
 int fgt_rownorm(const float* a, int ca, int lda, const float* b, int cb, int ldb, const int* gather,
                 int rows_per_batch, long long total_rows, int dst_batch_rows, int dst_row0, const float* gamma,
                 const float* beta, void* out_hi, long long out_plane, float eps, fgt_stream_t stream);
