@@ -9,15 +9,15 @@ The nn.Modules below only HOLD parameters under the reference's names; forward()
 them. All arithmetic runs in libfgt_sm90a.so (wgmma implicit-GEMM engine, fused flash
 attention, HBM-bound helpers) through fgt_b200.lib. There is no CPU / PyTorch fallback.
 """
+import functools
 import math
-import os
 
 import torch
 import torch.nn as nn
 
-from . import lib
-from .ops import pick_box
-from .packing import fold_layernorm, pack_weight, pack_weight_im2col
+from . import lib, ops
+from .graphs import NativeNet, workspace
+from .packing import fold_layernorm
 
 LN_EPS = 1e-5
 
@@ -128,19 +128,7 @@ class _Decoder(nn.Module):
         self.final = _ConvHolder(c // 2, cout, 3)
 
 
-# MMA terms of the flow branch (flow encoder + f_patch2vec). 1 = single-plane fp16 operands and activations (one MMA per
-# K step instead of three, half the activation bytes): the flow features only steer the spatial attention's gate and
-# Q/K, the flow tokens themselves stay within 1e-3 of the fp32 reference (fp16 has three more mantissa bits than bf16)
-# and the end-to-end error of the whole branch in fp16 is < 1e-4 (tools/precision_study.py, DESIGN.md 2). Every other
-# layer class needs the 3-term split product: each costs 2e-4..7e-4 end to end on its own even in fp16.
-_FLOW_TERMS = int(os.environ.get("FGT_FLOW_TERMS", "1"))
-
-def _terms(wp):
-    """MMA terms of a packed layer: 1 for fp16 weights (single-plane fp16 operands), 3 for split-bf16 ones."""
-    return 1 if wp["w"].dtype == torch.float16 else 3
-
-
-def _pick_bn(n_per_group, groups):
+def _pick_bn(n_per_group, groups=1):
     if n_per_group % 128 == 0:
         return 128
     if n_per_group <= 128:
@@ -163,7 +151,17 @@ def _fill_sms(bn, n_total, m_positions, groups=1, n_sms=132):
     return bn
 
 
-class FGT(nn.Module):
+def _tile(n_total, groups, m_positions):
+    """FGT's channel-tile policy (ops.conv_tile is the conv networks')."""
+    return _fill_sms(_pick_bn(n_total // groups, groups), n_total, m_positions, groups)
+
+
+# every GEMM of the generator takes its channel tile from FGT's policy
+conv = functools.partial(ops.conv, tile=_tile)
+linear = functools.partial(ops.linear, tile=_tile)
+
+
+class FGT(NativeNet):
     """Parameter layout of FGT (model.py:196-246) + the sm_90a forward schedule (model.py:249-283)."""
 
     def __init__(self, t_groupSize, s_windowSize, g_downSize, input_resolution, in_channels, cnum, flow_inChannel,
@@ -206,8 +204,6 @@ class FGT(nn.Module):
         self.decoder = _Decoder(cnum * 2, 3)
         if init_weights:
             self.init_weights()
-        self._packed = {}   # precision (half: bool) -> packed weights
-        self._geo = {}
         self._mixed = False
         self.capture = None  # set to a dict to record intermediate activations (tests)
 
@@ -224,23 +220,6 @@ class FGT(nn.Module):
                     nn.init.constant_(m.bias.data, 0.0)
 
     # ------------------------------------------------------------------ weight packing (one-time)
-    def _drop_graphs(self):
-        """Captured CUDA graphs bake in the addresses of the packed weights and workspaces: whenever those are
-        re-created (new weights, .to(), .float() ...) the captures must go too, or a replay reads freed memory."""
-        for gc in (getattr(self, "_graphed", None) or {}).values():
-            gc.entries.clear()
-
-    def _apply(self, fn, *a, **k):
-        self._packed = {}
-        self._geo = {}
-        self._drop_graphs()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._packed = {}
-        self._drop_graphs()
-        return super().load_state_dict(*a, **k)
-
     def _perm_hidden(self, c):
         """hidden index c*P + p (torch fold layout) -> p*c_count + c (position-major)."""
         P = self.ksz[0] * self.ksz[1]
@@ -257,22 +236,25 @@ class FGT(nn.Module):
         rnd = (lambda t: t.half().float()) if half else (lambda t: t)  # noqa: E731
 
         def put(name, w, b, segs=None):
-            P[name] = dict(w=pack_weight(rnd(w), segs, half=half).to(dev), b=rnd(b.float()).contiguous().to(dev),
-                           N=w.shape[0], name=name)
+            P[name] = ops.packed(name, rnd(w), rnd(b), dev, segs, half=half)
 
-        def conv(name, key, segs=None):
+        def layer(name, key, segs=None):
             put(name, sd[key + ".weight"], sd[key + ".bias"], segs)
 
         enc = "frame_endoder.layers."
         for i in (2, 4, 6, 8):
-            conv(f"enc{i}", enc + str(i))
-        # tiny-channel first layers consume im2col rows (fgt_im2col_nchw): one K=64 GEMM each
-        fh = _FLOW_TERMS == 1 or half
-        for name, key, h16 in (("enc0", enc + "0", half), ("fenc1", "flow_encoder.1.featureConv", fh)):
-            P[name] = dict(w=pack_weight_im2col(sd[key + ".weight"], half=h16).to(dev),
-                           b=rnd(sd[key + ".bias"]).contiguous().to(dev), N=sd[key + ".weight"].shape[0], name=name)
-        conv("enc10", enc + "10", [128, 192])
-        conv("enc12", enc + "12", [64, 128])
+            layer(f"enc{i}", enc + str(i))
+        # The flow branch (flow encoder + f_patch2vec) has fp16 weights in both sets: single-plane fp16 operands and
+        # activations, one MMA per K step instead of three and half the activation bytes. The flow features only steer
+        # the spatial attention's gate and Q/K; the flow tokens stay within 1e-3 of the fp32 reference (fp16 has three
+        # more mantissa bits than bf16) and the end-to-end error of the whole branch in fp16 is < 1e-4
+        # (tools/precision_study.py, DESIGN.md 2). Every other layer class of the fp32 set needs the 3-term split
+        # product: each costs 2e-4..7e-4 end to end on its own even in fp16.
+        # Tiny-channel first layers consume im2col rows (fgt_im2col_nchw): one K=64 GEMM each.
+        for name, key, h16 in (("enc0", enc + "0", half), ("fenc1", "flow_encoder.1.featureConv", True)):
+            P[name] = ops.packed(name, sd[key + ".weight"], rnd(sd[key + ".bias"]), dev, im2col_pad=64, half=h16)
+        layer("enc10", enc + "10", [128, 192])
+        layer("enc12", enc + "12", [64, 128])
         # enc14 (8 groups of 32+48 -> 32 channels) as 2 super-groups of 4 with block-diagonal weights: the engine then
         # works on 128-wide tiles and full 64-channel chunks (5 per tap for 4 groups instead of 2 half-empty ones per
         # group), which cuts its operand traffic by 3/8 at the price of multiplying exact zeros
@@ -284,12 +266,11 @@ class FGT(nn.Module):
             wbd[rows_o, j * c0_g:(j + 1) * c0_g] = w14[rows_o, :c0_g]
             wbd[rows_o, G14 * c0_g + j * c1_g:G14 * c0_g + (j + 1) * c1_g] = w14[rows_o, c0_g:]
         put("enc14", wbd, sd[enc + "14.bias"], [G14 * c0_g, G14 * c1_g])
-        conv("enc16", enc + "16", [256, 256])
+        layer("enc16", enc + "16", [256, 256])
         for name, key in (("fenc2", "flow_encoder.2.featureConv"), ("fenc3", "flow_encoder.3.featureConv"),
                           ("fenc4", "flow_encoder.4.featureConv"), ("f_patch2vec", "f_patch2vec")):
-            P[name] = dict(w=pack_weight(sd[key + ".weight"], half=fh).to(dev),
-                           b=rnd(sd[key + ".bias"]).contiguous().to(dev), N=sd[key + ".weight"].shape[0], name=name)
-        conv("patch2vec", "patch2vec")
+            P[name] = ops.packed(name, sd[key + ".weight"], rnd(sd[key + ".bias"]), dev, half=True)
+        layer("patch2vec", "patch2vec")
         P["pos_w"] = rnd(sd["add_pos_emb.proj.weight"]).reshape(-1).contiguous().to(dev)
         P["pos_b"] = rnd(sd["add_pos_emb.proj.bias"]).contiguous().to(dev)
         perm_ffn = self._perm_hidden(self.mlp_c).to(sd["patch2vec.weight"].device)
@@ -349,9 +330,9 @@ class FGT(nn.Module):
                     put(f"{name}.p{py}{px}", w2, b)
 
         deconv("dec1", "decoder.layer1.conv.featureConv")
-        conv("dec2", "decoder.layer2.featureConv")
+        layer("dec2", "decoder.layer2.featureConv")
         deconv("dec3", "decoder.layer3.conv.featureConv")
-        conv("dec4", "decoder.final.featureConv")
+        layer("dec4", "decoder.final.featureConv")
         # final 64->3 conv as "taps as N": a 1x1 GEMM with N = 9*3 (padded to 32) + fgt_tapsum (shift, add, bias, tanh)
         w4 = sd["decoder.final.featureConv.weight"]
         put("dec4t", lib.pack_taps_as_n(w4), torch.zeros(32))
@@ -366,7 +347,7 @@ class FGT(nn.Module):
         if H % 4 or W % 4:
             raise ValueError(f"FGT input {H}x{W} must be divisible by 4 (model.py:55-63 views features as H//4 x W//4)")
         g = type("Geo", (), {})()
-        g.mixed = mixed  # workspaces of the mixed-precision path: single-plane fp16 where the fp32 path is split-bf16
+        g.a16 = torch.float16 if mixed else torch.bfloat16  # 16-bit activations: fp16 (mixed) or split-bf16
         bt = b * t
         g.b, g.t, g.bt, g.H, g.W = b, t, bt, H, W
         g.OH, g.OW = H // 4, W // 4
@@ -411,64 +392,18 @@ class FGT(nn.Module):
         return g
 
     @staticmethod
-    def _buf(g, name, shape, dev, dtype=torch.float32, split=False, zero=False):
-        if name not in g.bufs:
-            if split and g.mixed:
-                dtype = torch.float16
-            elif split:
-                shape = (2,) + tuple(shape)
-                dtype = torch.bfloat16
-            g.bufs[name] = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=dev)
-        return g.bufs[name]
+    def _buf(g, name, shape, dev, dtype=torch.float32, zero=False):
+        return workspace(g.bufs, name, shape, dev, dtype, zero)
 
     # ------------------------------------------------------------------ op helpers
     @staticmethod
-    def _conv(x, cin, n, h, w, wp, k, *, stride=1, pad=None, act=lib.ACT_LEAKY02, out_split=None, out_f32=None,
-              extra_seg=None, groups=1, seg_counts=None, nchw_out=False, terms=None, out_f16=None, alg_k=None):
-        """NHWC split x [2,n,h,w,cin] (+ optional second segment) -> conv -> NHWC outputs. terms: 1 for fp16 weights
-        (single-plane fp16 operands), 3 otherwise."""
-        terms = _terms(wp) if terms is None else terms
-        pad = k // 2 if pad is None else pad
-        oh = (h + 2 * pad - k) // stride + 1
-        ow = (w + 2 * pad - k) // stride + 1
-        N = wp["N"]
-        if seg_counts is None:
-            segs = [lib.ASeg(x, cin, w, h, n)]
-        else:
-            x2, cin2 = extra_seg
-            cpg = [c if groups > 1 else 0 for c in seg_counts]
-            segs = [lib.ASeg(x, cin, w, h, n, c_per_group=cpg[0], c_count=seg_counts[0]),
-                    lib.ASeg(x2, cin2, w, h, n, c_per_group=cpg[1], c_count=seg_counts[1])]
-        bw, bh = pick_box(ow, oh)
-        if nchw_out:
-            strides = dict(os_z=N * oh * ow, os_y=ow, os_x=1, os_c=oh * ow)
-        else:
-            strides = dict(os_z=oh * ow * N, os_y=ow * N, os_x=N, os_c=1)
-        lib.gemm_tc(segs, wp["w"], N, kx=k, ky=k, stride=stride, pad_x=pad, pad_y=pad, groups=groups, out_w=ow,
-                    out_h=oh, out_z=n, box_w=bw, box_h=bh,
-                    bn=_fill_sms(_pick_bn(N // groups, groups), N, n * oh * ow, groups), bias=wp["b"], act=act,
-                    out_f32=out_f32, out_split=out_split, out_f16=out_f16, tag=wp["name"], terms=terms, alg_k=alg_k,
-                    **strides)
-        return oh, ow
-
-    @staticmethod
-    def _deconv(x, cin, n, h, w, P, name, out_split):
+    def _deconv(x, cin, P, name, out_split):
         """nearest-x2 + 3x3 conv + LeakyReLU as four 2x2 phase convs writing the interleaved [n,2h,2w,N] output."""
-        bw, bh = pick_box(w, h)
         for py in (0, 1):
             for px in (0, 1):
                 wp = P[f"{name}.p{py}{px}"]
-                N = wp["N"]
-                lib.gemm_tc([lib.ASeg(x, cin, w, h, n)], wp["w"], N, kx=2, ky=2, pad_x=1 - px, pad_y=1 - py, out_w=w,
-                            out_h=h, out_z=n, box_w=bw, box_h=bh, bn=_pick_bn(N, 1), bias=wp["b"], terms=_terms(wp),
-                            act=lib.ACT_LEAKY02, out_split=out_split, out_elem_offset=(py * 2 * w + px) * N,
-                            os_z=4 * h * w * N, os_y=4 * w * N, os_x=2 * N, os_c=1, tag=wp["name"])
-
-    @staticmethod
-    def _linear(segs, wp, rows, bn=None, **kw):
-        kw.setdefault("terms", _terms(wp))
-        lib.gemm_tc(segs, wp["w"], wp["N"], out_w=rows,
-                    bn=bn or _fill_sms(_pick_bn(wp["N"], 1), wp["N"], rows), bias=wp["b"], tag=wp["name"], **kw)
+                ops.conv([(x, cin)], wp, kx=2, ky=2, pad_x=1 - px, pad_y=1 - py, out_phase=(py, px),
+                         bn=_pick_bn(wp["N"]), out_split=out_split)
 
     def _ffn(self, g, P, name, x, xs, dev, need_split=True):
         """x += FusionFeedForward(LN(x)) (ffn_base.py:53-77, model.py:128-129 / 147-148). need_split: whether the next
@@ -481,15 +416,14 @@ class FGT(nn.Module):
         rows, d = g.bt * g.n, self.d
         k, s, p = self.ksz[0], self.stride[0], self.padding[0]
         hidden = k * k * self.mlp_c
-        y = self._buf(g, "ffn_y", (rows, d), dev, split=True)
+        y = self._buf(g, "ffn_y", (rows, d), dev, g.a16)
         hid = self._buf(g, "ffn_hid", (rows, hidden), dev)
-        hid2 = self._buf(g, "ffn_hid2", (rows, hidden), dev, split=True)
+        hid2 = self._buf(g, "ffn_hid2", (rows, hidden), dev, g.a16)
         lib.rownorm(x, None, y, rows_per_batch=rows, total_rows=rows, dst_batch_rows=rows, eps=LN_EPS)
-        self._linear([lib.ASeg(y, d, rows)], P[name + ".ffn1"], rows, out_f32=hid)
+        linear([(y, d)], P[name + ".ffn1"], rows, out_f32=hid)
         # fold / coverage division / unfold / ReLU (ffn_base.py:57-75) in one launch, no image round trip
         lib.fold_unfold(hid, g.bt, g.h, g.w, self.mlp_c, k, k, s, p, g.OH, g.OW, hid2, relu=True)
-        self._linear([lib.ASeg(hid2, hidden, rows)], P[name + ".ffn2"], rows, aux=x, aux_mode=lib.AUX_ADD, out_f32=x,
-                     out_split=xs)
+        linear([(hid2, hidden)], P[name + ".ffn2"], rows, aux=x, aux_mode=lib.AUX_ADD, out_f32=x, out_split=xs)
 
     def enable_frame_sharding(self, total_frames, group=None, rank=None, world=None, exchange="p2p"):
         """Frame-sharded execution of ONE clip window over the ranks of `group` (SURVEY §8e): this rank's
@@ -539,9 +473,9 @@ class FGT(nn.Module):
         ptrs, s_all = fs["work"][key][fs["layer"] % 2]
         fs["layer"] += 1
         self._split_qkv(P, name)
-        q = self._buf(g, f"tp_q{T}", (g.zones * Lzl, d), dev, split=True)
-        kv = self._buf(g, f"tp_kv{T}", (g.zones * Lz, 2 * d), dev, split=True)
-        att = self._buf(g, "att_tok", (g.bt * g.n, d), dev, split=True)   # attention output in token order
+        q = self._buf(g, f"tp_q{T}", (g.zones * Lzl, d), dev, g.a16)
+        kv = self._buf(g, f"tp_kv{T}", (g.zones * Lz, 2 * d), dev, g.a16)
+        att = self._buf(g, "att_tok", (g.bt * g.n, d), dev, g.a16)   # attention output in token order
         lib.rownorm_bcast(x, ptrs, plane, gather=g.zone_map, rows_per_batch=Lzl, total_rows=g.zones * Lzl,
                           dst_batch_rows=Lz, dst_row0=off * zl, eps=LN_EPS, gamma=P[name + ".ln_g"],
                           beta=P[name + ".ln_b"])
@@ -549,12 +483,12 @@ class FGT(nn.Module):
         # rows were written by this rank's own LayerNorm launch (stream order), so the Q projection runs BEFORE the
         # barrier and hides the time the peers' rows need to arrive over NVLink.
         wq = P[name + ".q"]
-        bw, bh = pick_box(Lzl, g.zones)
+        bw, bh = ops.pick_box(Lzl, g.zones)
         lib.gemm_tc([lib.ASeg(s_all, d, Lzl, g.zones, 1, sx=d, sy=Lz * d, elem_offset=off * zl * d)], wq["w"], d,
-                    out_w=Lzl, out_h=g.zones, box_w=bw, box_h=bh, bn=_pick_bn(d, 1), bias=wq["b"],
+                    out_w=Lzl, out_h=g.zones, box_w=bw, box_h=bh, bn=_pick_bn(d), bias=wq["b"],
                     out_split=q, os_x=d, os_y=Lzl * d, tag=wq["name"])
         pg.barrier()  # every peer's rows of this layer are in s_all
-        self._linear([lib.ASeg(s_all, d, g.zones * Lz)], P[name + ".kv"], g.zones * Lz, out_split=kv)
+        linear([(s_all, d)], P[name + ".kv"], g.zones * Lz, out_split=kv)
         lib.attention(q, kv, kv, att, batches=g.zones, heads=self.heads, Lq=Lzl, Lk=Lz, q_ld=d, k_ld=2 * d, v_ld=2 * d,
                       out_ld=d, q_batch_stride=Lzl * d, k_batch_stride=Lz * 2 * d, v_batch_stride=Lz * 2 * d,
                       out_batch_stride=Lzl * d, scale=1.0 / math.sqrt(d // self.heads), v_off=d, out_rowmap=g.zone_map,
@@ -566,7 +500,7 @@ class FGT(nn.Module):
         attention kernel has already undone the zone / window regrouping in its store (out_rowmap), so this is a plain
         row-major GEMM over the real tokens with the residual in its epilogue."""
         rows = g.bt * g.n
-        self._linear([lib.ASeg(att, self.d, rows)], P[name + ".o"], rows, aux=x, aux_mode=lib.AUX_ADD, out_f32=x)
+        linear([(att, self.d)], P[name + ".o"], rows, aux=x, aux_mode=lib.AUX_ADD, out_f32=x)
 
     def _split_qkv(self, P, name):
         """Q-only and K|V-only slices of the fused temporal projection (frame-sharded TMHSA: Q for the local
@@ -589,16 +523,16 @@ class FGT(nn.Module):
         T, tmax = sum(counts), max(counts)
         Lzl, Lz, Lqp = g.Lz, T * zl, tmax * zl
         self._split_qkv(P, name)
-        s_loc = self._buf(g, f"ts_s{T}", (g.zones * Lqp, d), dev, split=True, zero=True)
-        q = self._buf(g, f"ts_q{T}", (g.zones * Lqp, d), dev, split=True)
-        kv = self._buf(g, f"ts_kv{T}", (g.zones * Lz, 2 * d), dev, split=True)
-        att = self._buf(g, "att_tok", (g.bt * g.n, d), dev, split=True)   # attention output in token order
+        s_loc = self._buf(g, f"ts_s{T}", (g.zones * Lqp, d), dev, g.a16, zero=True)
+        q = self._buf(g, f"ts_q{T}", (g.zones * Lqp, d), dev, g.a16)
+        kv = self._buf(g, f"ts_kv{T}", (g.zones * Lz, 2 * d), dev, g.a16)
+        att = self._buf(g, "att_tok", (g.bt * g.n, d), dev, g.a16)   # attention output in token order
         lib.rownorm(x, None, s_loc, gather=g.zone_map, rows_per_batch=Lzl, total_rows=g.zones * Lzl,
                     dst_batch_rows=Lqp, eps=LN_EPS, gamma=P[name + ".ln_g"], beta=P[name + ".ln_b"])
         s_all = parallel.allgather_zone_rows(s_loc.view(2, g.zones, Lqp, d), counts, zl, fs["group"], fs["work"])
         s_all = s_all.view(2, g.zones * Lz, d)
-        self._linear([lib.ASeg(s_loc, d, g.zones * Lqp)], P[name + ".q"], g.zones * Lqp, out_split=q)
-        self._linear([lib.ASeg(s_all, d, g.zones * Lz)], P[name + ".kv"], g.zones * Lz, out_split=kv)
+        linear([(s_loc, d)], P[name + ".q"], g.zones * Lqp, out_split=q)
+        linear([(s_all, d)], P[name + ".kv"], g.zones * Lz, out_split=kv)
         lib.attention(q, kv, kv, att, batches=g.zones, heads=self.heads, Lq=Lzl, Lk=Lz, q_ld=d, k_ld=2 * d, v_ld=2 * d,
                       out_ld=d, q_batch_stride=Lqp * d, k_batch_stride=Lz * 2 * d, v_batch_stride=Lz * 2 * d,
                       out_batch_stride=Lzl * d, scale=1.0 / math.sqrt(d // self.heads), v_off=d, out_rowmap=g.zone_map,
@@ -617,13 +551,12 @@ class FGT(nn.Module):
     def _tmhsa(self, g, P, name, x, dev):
         """x += TMHSA(LN(x)): LayerNorm + zone gather, fused QKV GEMM, dense flash attention, out-projection."""
         d, rows_z = self.d, g.zones * g.Lz
-        s_zm = self._buf(g, "t_s", (rows_z, d), dev, split=True)
-        qkv = self._buf(g, "t_qkv", (rows_z, 3 * d), dev, split=True)
-        att = self._buf(g, "att_tok", (g.bt * g.n, d), dev, split=True)   # attention output in token order
+        s_zm = self._buf(g, "t_s", (rows_z, d), dev, g.a16)
+        qkv = self._buf(g, "t_qkv", (rows_z, 3 * d), dev, g.a16)
+        att = self._buf(g, "att_tok", (g.bt * g.n, d), dev, g.a16)   # attention output in token order
         lib.rownorm(x, None, s_zm, gather=g.zone_map, rows_per_batch=rows_z, total_rows=rows_z,
                     dst_batch_rows=rows_z, eps=LN_EPS, gamma=P[name + ".ln_g"], beta=P[name + ".ln_b"])
-        a = [lib.ASeg(s_zm, d, rows_z)]
-        self._linear(a, P[name + ".qkv"], rows_z, out_split=qkv)  # one N=1536 GEMM: Q | K | V, all row-major
+        linear([(s_zm, d)], P[name + ".qkv"], rows_z, out_split=qkv)  # one N=1536 GEMM: Q | K | V, all row-major
         lib.attention(qkv, qkv, qkv, att, batches=g.zones, heads=self.heads, Lq=g.Lz, Lk=g.Lz, q_ld=3 * d, k_ld=3 * d,
                       v_ld=3 * d, out_ld=d, q_batch_stride=g.Lz * 3 * d, k_batch_stride=g.Lz * 3 * d,
                       v_batch_stride=g.Lz * 3 * d, out_batch_stride=g.Lz * d, scale=1.0 / math.sqrt(d // self.heads),
@@ -642,22 +575,21 @@ class FGT(nn.Module):
         d, df, bt = self.d, self.df, g.bt
         rows = bt * g.n
         fp = self._buf(g, "s_fp", (rows, df), dev)
-        qkn = self._buf(g, "s_qkn", (bt * g.R, d + df), dev, split=True, zero=True)
-        vn = self._buf(g, "s_vn", (bt * g.R, d), dev, split=True, zero=True)
-        qkv = self._buf(g, "s_qkv", (bt * g.R, 3 * d), dev, split=True)
-        att = self._buf(g, "att_tok", (rows, d), dev, split=True)         # attention output in token order
+        qkn = self._buf(g, "s_qkn", (bt * g.R, d + df), dev, g.a16, zero=True)
+        vn = self._buf(g, "s_vn", (bt * g.R, d), dev, g.a16, zero=True)
+        qkv = self._buf(g, "s_qkv", (bt * g.R, 3 * d), dev, g.a16)
+        att = self._buf(g, "att_tok", (rows, d), dev, g.a16)         # attention output in token order
         # flow re-weighting gate: f' = f * sigmoid(W_r [x; f] + b_r)   (attention_flow.py:126-128)
-        self._linear([lib.ASeg(xs, d, rows), lib.ASeg(fs, df, rows)], P[name + ".gate"], rows, act=lib.ACT_SIGMOID,
-                     aux=f, aux_mode=lib.AUX_MUL, out_f32=fp, bn=64 if rows <= 128 * 66 else None)  # <= half a wave of 128-wide tiles -> 64 wide
+        linear([(xs, d), (fs, df)], P[name + ".gate"], rows, act=lib.ACT_SIGMOID, aux=f, aux_mode=lib.AUX_MUL,
+               out_f32=fp, bn=64 if rows <= 128 * 66 else None)  # <= half a wave of 128-wide tiles -> 64 wide
         # pooled global tokens (attention_flow.py:135,145) and the LayerNorm statistics of window rows and pooled
         # rows (attention_flow.py:142-143,154): one launch
         nl = g.nwp * 64
         lib.swin_prep(x, fp, bt, g.h, g.w, g.win_map, nl, g.R, self.gd, g.gh, g.gw, P[name + ".gk_w"],
                       P[name + ".gk_b"], P[name + ".gv_w"], P[name + ".gv_b"], qkn, vn, eps=LN_EPS, tag=name)
         # Q | K from the 768-wide normalised rows, V from the 512-wide ones: two GEMMs into one [rows, 3d] buffer
-        self._linear([lib.ASeg(qkn, d + df, bt * g.R)], P[name + ".qk"], bt * g.R, out_split=qkv, os_x=3 * d)
-        self._linear([lib.ASeg(vn, d, bt * g.R)], P[name + ".v"], bt * g.R, out_split=qkv, os_x=3 * d,
-                     out_elem_offset=2 * d)
+        linear([(qkn, d + df)], P[name + ".qk"], bt * g.R, out_split=qkv, os_x=3 * d)
+        linear([(vn, d)], P[name + ".v"], bt * g.R, out_split=qkv, os_x=3 * d, out_elem_offset=2 * d)
         lib.attention(qkv, qkv, qkv, att, batches=bt, heads=self.heads, Lq=nl, Lk=g.R, Lk_rows=g.R, q_ld=3 * d,
                       k_ld=3 * d, v_ld=3 * d, out_ld=d, q_batch_stride=g.R * 3 * d, k_batch_stride=g.R * 3 * d,
                       v_batch_stride=g.R * 3 * d, out_batch_stride=nl * d, scale=1.0 / math.sqrt(d // self.heads),
@@ -665,12 +597,6 @@ class FGT(nn.Module):
         self._out_proj(g, P, name, att, x)
 
     # ------------------------------------------------------------------ forward
-    def enable_cuda_graph(self, on=True):
-        """Replay the whole forward as one CUDA graph per input geometry and precision (fgt_b200/graphs.py)."""
-        from .graphs import GraphedCall
-        self._graphed = {m: GraphedCall(lambda *a, _m=m: self._forward_impl(*a, mixed=_m)) for m in (False, True)} \
-            if on else None
-
     def enable_mixed_precision(self, on=True):
         """Mixed precision, opt-in: the generator runs as the reference does under
         torch.autocast("cuda", dtype=torch.float16). Every Linear / conv is a 1-term fp16 tensor-core GEMM (fp16
@@ -689,10 +615,11 @@ class FGT(nn.Module):
             raise RuntimeError("fgt_b200.FGT runs on a CUDA (sm_90a) device only; there is no CPU fallback")
         fs = getattr(self, "_fshard", None)
         graph_ok = fs is None or fs["exchange"] == "p2p"  # NCCL calls are not captured; the P2P exchange is kernels only
-        if getattr(self, "_graphed", None) is not None and self.capture is None and graph_ok:
-            return self._graphed[self._mixed](masked_frames.float().contiguous(), flows.float().contiguous(),
-                                              masks.float().contiguous())
-        return self._forward_impl(masked_frames, flows, masks, mixed=self._mixed)
+        mixed = self._mixed
+        if self._graphs is not None and self.capture is None and graph_ok:
+            return self._graphed((mixed,), lambda *a: self._forward_impl(*a, mixed=mixed),
+                                 masked_frames.float().contiguous(), flows.float().contiguous(), masks.float().contiguous())
+        return self._forward_impl(masked_frames, flows, masks, mixed=mixed)
 
     def _forward_impl(self, masked_frames, flows, masks, mixed=False):
         dev = masked_frames.device
@@ -705,9 +632,10 @@ class FGT(nn.Module):
         if fs is not None and fs["exchange"] == "p2p":
             fs["layer"] = 0
             fs["peer"].barrier()  # every peer has finished reading the exchange buffers of the previous forward
-        P = self._packed[mixed] if mixed in self._packed else self._pack(dev, mixed)
+        P = self._packed.get(mixed) or self._pack(dev, mixed)
         g = self._geometry(b, t, H, W, dev, mixed)
-        B = lambda name, shape, **kw: self._buf(g, name, shape, dev, **kw)  # noqa: E731
+        B = lambda name, shape, dtype=torch.float32: self._buf(g, name, shape, dev, dtype)  # noqa: E731
+        A = lambda name, shape: self._buf(g, name, shape, dev, g.a16)  # noqa: E731
         frames = masked_frames.reshape(bt, c, H, W).float().contiguous()
         mk = masks.reshape(bt, 1, H, W).float().contiguous()
         fl = flows.reshape(bt, flows.shape[2], H, W).float().contiguous()
@@ -715,60 +643,53 @@ class FGT(nn.Module):
 
         # ---- frame encoder (model.py:53-66)
         lib._scope[1:] = ["encoder"]  # module labels for the per-launch profiler (bench.py "modules")
-        incol = B("in_col", (bt, H2, W2, 64), split=True)
+        incol = A("in_col", (bt, H2, W2, 64))
         lib.im2col_nchw(frames, mk, incol, k=3, stride=2, pad=1, replicate=False, OH=H2, OW=W2, tag="enc0")
-        e0 = B("e0", (bt, H2, W2, 64), split=True)
-        e2 = B("e2", (bt, H2, W2, 64), split=True)
-        e4 = B("e4", (bt, OH, OW, 128), split=True)
-        x0 = B("e6", (bt, OH, OW, 256), split=True)
-        e8 = B("e8", (bt, OH, OW, 384), split=True)
-        e10 = B("e10", (bt, OH, OW, 512), split=True)
-        e12 = B("e12", (bt, OH, OW, 384), split=True)
-        e14 = B("e14", (bt, OH, OW, 256), split=True)
-        enc = B("enc", (bt, OH, OW, 128), split=True)
+        e0 = A("e0", (bt, H2, W2, 64))
+        e2 = A("e2", (bt, H2, W2, 64))
+        e4 = A("e4", (bt, OH, OW, 128))
+        x0 = A("e6", (bt, OH, OW, 256))
+        e8 = A("e8", (bt, OH, OW, 384))
+        e10 = A("e10", (bt, OH, OW, 512))
+        e12 = A("e12", (bt, OH, OW, 384))
+        e14 = A("e14", (bt, OH, OW, 256))
+        enc = A("enc", (bt, OH, OW, 128))
         enc_f = B("enc_f", (bt, OH, OW, 128))
-        self._linear([lib.ASeg(incol, 64, bt * H2 * W2)], P["enc0"], bt * H2 * W2, act=lib.ACT_LEAKY02, out_split=e0)
-        self._conv(e0, 64, bt, H2, W2, P["enc2"], 3, out_split=e2)
-        self._conv(e2, 64, bt, H2, W2, P["enc4"], 3, stride=2, out_split=e4)
-        self._conv(e4, 128, bt, OH, OW, P["enc6"], 3, out_split=x0)
-        self._conv(x0, 256, bt, OH, OW, P["enc8"], 3, out_split=e8)
-        self._conv(x0, 256, bt, OH, OW, P["enc10"], 3, out_split=e10, extra_seg=(e8, 384), groups=2,
-                   seg_counts=[128, 192])
-        self._conv(x0, 256, bt, OH, OW, P["enc12"], 3, out_split=e12, extra_seg=(e10, 512), groups=4,
-                   seg_counts=[64, 128])
-        self._conv(x0, 256, bt, OH, OW, P["enc14"], 3, out_split=e14, extra_seg=(e12, 384), groups=2,
-                   seg_counts=[128, 192], alg_k=9 * (32 + 48))  # roofline accounting: the reference's 8-group conv
-        self._conv(x0, 256, bt, OH, OW, P["enc16"], 3, out_split=enc, out_f32=enc_f, extra_seg=(e14, 256), groups=1,
-                   seg_counts=[256, 256])
-        # ---- flow encoder (model.py:206-212)
+        k3 = dict(kx=3, ky=3, pad_x=1, pad_y=1)
+        linear([(incol, 64)], P["enc0"], bt * H2 * W2, act=lib.ACT_LEAKY02, out_split=e0)
+        conv([(e0, 64)], P["enc2"], out_split=e2, **k3)
+        conv([(e2, 64)], P["enc4"], stride=2, out_split=e4, **k3)
+        conv([(e4, 128)], P["enc6"], out_split=x0, **k3)
+        conv([(x0, 256)], P["enc8"], out_split=e8, **k3)
+        conv([(x0, 256), (e8, 384)], P["enc10"], out_split=e10, groups=2, seg_counts=[128, 192], **k3)
+        conv([(x0, 256), (e10, 512)], P["enc12"], out_split=e12, groups=4, seg_counts=[64, 128], **k3)
+        conv([(x0, 256), (e12, 384)], P["enc14"], out_split=e14, groups=2, seg_counts=[128, 192],
+             alg_k=9 * (32 + 48), **k3)  # roofline accounting: the reference's 8-group conv
+        conv([(x0, 256), (e14, 256)], P["enc16"], out_split=enc, out_f32=enc_f, seg_counts=[256, 256], **k3)
+        # ---- flow encoder (model.py:206-212): fp16 weights and activations in both precisions (see _pack)
         lib._scope[-1] = "flow_encoder"
-        # 1-term mode: the branch's activations are single-plane fp16 tensors; 3-term mode: split-bf16 like the rest
-        flow16 = _FLOW_TERMS == 1 or mixed
-        fkw = dict(dtype=torch.float16) if flow16 else dict(split=True)
-        okey = "out_f16" if flow16 else "out_split"
-        fcol = B("f_col", (bt, H, W, 64), **fkw)
+        fcol = B("f_col", (bt, H, W, 64), torch.float16)
         lib.im2col_nchw(fl, None, fcol, k=5, stride=1, pad=2, replicate=True, OH=H, OW=W, tag="fenc1")
-        f1 = B("f1", (bt, H, W, 64), **fkw)
-        f2 = B("f2", (bt, H2, W2, 128), **fkw)
-        f3 = B("f3", (bt, H2, W2, 128), **fkw)
-        f4 = B("f4", (bt, OH, OW, 128), **fkw)
-        self._linear([lib.ASeg(fcol, 64, bt * H * W)], P["fenc1"], bt * H * W, act=lib.ACT_LEAKY02,
-                     **{okey: f1})
-        self._conv(f1, 64, bt, H, W, P["fenc2"], 3, stride=2, **{okey: f2})
-        self._conv(f2, 128, bt, H2, W2, P["fenc3"], 3, **{okey: f3})
-        self._conv(f3, 128, bt, H2, W2, P["fenc4"], 3, stride=2, **{okey: f4})
+        f1 = B("f1", (bt, H, W, 64), torch.float16)
+        f2 = B("f2", (bt, H2, W2, 128), torch.float16)
+        f3 = B("f3", (bt, H2, W2, 128), torch.float16)
+        f4 = B("f4", (bt, OH, OW, 128), torch.float16)
+        linear([(fcol, 64)], P["fenc1"], bt * H * W, act=lib.ACT_LEAKY02, out_split=f1)
+        conv([(f1, 64)], P["fenc2"], stride=2, out_split=f2, **k3)
+        conv([(f2, 128)], P["fenc3"], out_split=f3, **k3)
+        conv([(f3, 128)], P["fenc4"], stride=2, out_split=f4, **k3)
         # ---- patch embedding (model.py:261-262,270-271): conv output NHWC == token-major
         lib._scope[-1] = "patch_embed"
         rows = bt * g.n
         xa = B("x_a", (rows, self.d))
         xb = B("x_b", (rows, self.d))
-        xs = B("x_s", (rows, self.d), split=True)
+        xs = A("x_s", (rows, self.d))
         f = B("f", (rows, self.df))
-        fs = B("f_s", (rows, self.df), split=True)
+        fs = A("f_s", (rows, self.df))
         k, s, p = self.ksz[0], self.stride[0], self.padding[0]
-        self._conv(enc, 128, bt, OH, OW, P["patch2vec"], k, stride=s, pad=p, act=lib.ACT_NONE, out_f32=xa)
-        self._conv(f4, 128, bt, OH, OW, P["f_patch2vec"], k, stride=s, pad=p, act=lib.ACT_NONE, out_f32=f,
-                   out_split=fs)
+        kp = dict(kx=k, ky=k, stride=s, pad_x=p, pad_y=p, act=lib.ACT_NONE)
+        conv([(enc, 128)], P["patch2vec"], out_f32=xa, **kp)
+        conv([(f4, 128)], P["f_patch2vec"], out_f32=f, out_split=fs, **kp)
         self._cap("enc", enc_f)
         self._cap("tok0", xa)
         self._cap("ftok", f)
@@ -788,19 +709,19 @@ class FGT(nn.Module):
         # ---- vec2patch + skip (model.py:278-279)
         lib._scope[-1] = "vec2patch"
         v2p = B("v2p", (rows, k * k * self.cnum * 2))
-        feat = B("feat", (bt, OH, OW, self.cnum * 2), split=True)
-        self._linear([lib.ASeg(xs, self.d, rows)], P["vec2patch"], rows, out_f32=v2p)
+        feat = A("feat", (bt, OH, OW, self.cnum * 2))
+        linear([(xs, self.d)], P["vec2patch"], rows, out_f32=v2p)
         lib.fold(v2p, bt, g.h, g.w, self.cnum * 2, k, k, s, p, OH, OW, normalize=False, add=enc_f, out_split=feat)
         # ---- decoder (model.py:188-193,281-282)
         lib._scope[-1] = "decoder"
         c2 = self.cnum * 2
-        d1 = B("d1", (bt, H2, W2, c2), split=True)
-        d2 = B("d2", (bt, H2, W2, c2 // 2), split=True)
-        d3 = B("d3", (bt, H, W, c2 // 2), split=True)
+        d1 = A("d1", (bt, H2, W2, c2))
+        d2 = A("d2", (bt, H2, W2, c2 // 2))
+        d3 = A("d3", (bt, H, W, c2 // 2))
         out = torch.empty(bt, 3, H, W, device=dev, dtype=torch.float32)
-        self._deconv(feat, c2, bt, OH, OW, P, "dec1", d1)
-        self._conv(d1, c2, bt, H2, W2, P["dec2"], 3, out_split=d2)
-        self._deconv(d2, c2 // 2, bt, H2, W2, P, "dec3", d3)
+        self._deconv(feat, c2, P, "dec1", d1)
+        conv([(d1, c2)], P["dec2"], out_split=d2, **k3)
+        self._deconv(d2, c2 // 2, P, "dec3", d3)
         # final 64 -> 3 conv + tanh: taps-as-N tensor-core GEMM and the 9-tap sum in one kernel (no HBM intermediate)
         lib.conv_tail(d3, bt, H, W, c2 // 2, P["dec4t"]["w"], 3, P["dec4"]["b"], lib.ACT_TANH, out, nchw=True, tag="dec4")
         lib._scope[1:] = []

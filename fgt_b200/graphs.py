@@ -1,4 +1,5 @@
-"""CUDA-graph replay of a whole model forward (opt-in).
+"""Host caches of the network modules (NativeNet: packed weights, workspaces, CUDA graphs) and CUDA-graph replay of
+a whole model forward (opt-in).
 
 Every forward here is a fixed sequence of kernel launches over cached workspaces, so after one eager
 call per input geometry the sequence is captured into a CUDA graph and replayed: one graph launch
@@ -7,6 +8,7 @@ gains little). TMA descriptors are encoded on the host at capture time and baked
 is valid because all buffers are static. Inputs are copied into static tensors, outputs are cloned.
 """
 import torch
+import torch.nn as nn
 
 from . import lib
 
@@ -39,3 +41,55 @@ class GraphedCall:
         if isinstance(out, torch.Tensor):
             return out.clone()
         return type(out)(o.clone() if isinstance(o, torch.Tensor) else o for o in out)
+
+
+def workspace(bufs, name, shape, dev, dtype=torch.float32, zero=False):
+    """Buffer `name` of the workspace dict `bufs`, allocated on first use. A bfloat16 buffer is split-bf16, [2, *shape]
+    (hi and lo planes); fp16 and fp32 buffers are [*shape]."""
+    t = bufs.get(name)
+    if t is None:
+        if dtype == torch.bfloat16:
+            shape = (2,) + tuple(shape)
+        t = bufs[name] = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=dev)
+    return t
+
+
+def _drop_weights(net, incompatible_keys):
+    net._packed = {}
+    net._drop_graphs()
+
+
+class NativeNet(nn.Module):
+    """Host caches of a network whose forward runs on the native kernels: packed weights per precision (`_packed`),
+    workspaces per input geometry (`_geo`) and, while enabled, CUDA graphs per call (`_graphs`, keyed by the call's
+    non-tensor arguments). Packed weights are copies of the parameters and graphs hold the addresses of packed weights
+    and workspaces, so `.to()` / `.half()` / ... drop all three, and a state-dict load drops the packed weights and the
+    graphs, also when the load is called on a wrapper module or on nn.DataParallel."""
+
+    def __init__(self):
+        super().__init__()
+        self._packed = {}
+        self._geo = {}
+        self._graphs = None
+        self.register_load_state_dict_post_hook(_drop_weights)
+
+    def _drop_graphs(self):
+        if self._graphs:
+            self._graphs.clear()
+
+    def _apply(self, fn, *a, **k):
+        self._packed = {}
+        self._geo = {}
+        self._drop_graphs()
+        return super()._apply(fn, *a, **k)
+
+    def enable_cuda_graph(self, on=True):
+        """Replay whole forwards as CUDA graphs, one per input geometry and call key."""
+        self._graphs = {} if on else None
+
+    def _graphed(self, key, fn, *tensors):
+        """fn(*tensors) through the GraphedCall of `key` (the call's non-tensor arguments)."""
+        gc = self._graphs.get(key)
+        if gc is None:
+            gc = self._graphs[key] = GraphedCall(fn)
+        return gc(*tensors)

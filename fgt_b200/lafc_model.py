@@ -11,6 +11,7 @@ import torch
 import torch.nn as nn
 
 from . import lib, ops
+from .graphs import NativeNet, workspace
 
 
 class _C3(nn.Module):
@@ -47,7 +48,7 @@ class _Edge(nn.Module):
         self.out_layer = _C2(mid, 1, 1)
 
 
-class P3DNet(nn.Module):
+class P3DNet(NativeNet):
     def __init__(self, num_flows, num_feats, in_channels, passmask, use_residual, res_blocks, use_bias, conv_type,
                  init_weights):
         super().__init__()
@@ -73,24 +74,6 @@ class P3DNet(nn.Module):
                 if isinstance(m, (nn.Conv2d, nn.Conv3d)):
                     nn.init.kaiming_normal_(m.weight.data, a=0, mode='fan_in')
                     nn.init.constant_(m.bias.data, 0.0)
-        self._packed = None
-        self._bufs = {}
-
-    def _drop_graphs(self):
-        """Captured CUDA graphs hold the addresses of the packed weights / workspaces they were recorded with."""
-        if getattr(self, "_graphed", None) is not None:
-            self._graphed.entries.clear()
-
-    def _apply(self, fn, *a, **k):
-        self._packed = None
-        self._bufs = {}
-        self._drop_graphs()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._packed = None
-        self._drop_graphs()
-        return super().load_state_dict(*a, **k)
 
     def _pack(self, dev):
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
@@ -127,25 +110,16 @@ class P3DNet(nn.Module):
         put("edge_1", "edgeDetector.mid_layer_1")
         put("edge_2", "edgeDetector.mid_layer_2")
         put("edge_o", "edgeDetector.out_layer")
-        self._packed = P
+        self._packed[False] = P
         return P
-
-    def _buf(self, key, name, shape, dev, split=True):
-        d = self._bufs.setdefault(key, {})
-        if name not in d:
-            if split:
-                d[name] = torch.empty((2,) + tuple(shape), dtype=torch.bfloat16, device=dev)
-            else:
-                d[name] = torch.empty(shape, dtype=torch.float32, device=dev)
-        return d[name]
 
     def _forward_one(self, x, P, dev):
         """x: [T, 3, H, W] fp32 (flows + mask per candidate frame) -> (flow [2,H,W], edge [1,H,W])."""
         T, _, H, W = x.shape
         c = self.c
         H2, W2, H4, W4 = H // 2, W // 2, H // 4, W // 4
-        key = (T, H, W)
-        B = lambda n, s, split=True: self._buf(key, n, s, dev, split)  # noqa: E731
+        bufs = self._geo.setdefault((T, H, W), {})
+        B = lambda n, s, split=True: workspace(bufs, n, s, dev, torch.bfloat16 if split else torch.float32)  # noqa: E731
         L = lib.ACT_LEAKY02
         # encoder2 (lafc.py:23-30): ReplicationPad + (1,5,5) conv via im2col, then the (3,1,1) conv
         col = B("col", (T, H, W, 128))
@@ -227,18 +201,13 @@ class P3DNet(nn.Module):
         ops.conv([(e2_, 16)], P["edge_o"], act=lib.ACT_SIGMOID, out_f32=edge, nchw_out=True)
         return flow, edge
 
-    def enable_cuda_graph(self, on=True):
-        """Replay the whole forward as one CUDA graph per input geometry (fgt_b200/graphs.py)."""
-        from .graphs import GraphedCall
-        self._graphed = GraphedCall(self._forward_impl) if on else None
-
     def forward(self, flows, masks, edges=None):
         if edges is not None:
             raise ValueError("fgt_b200 LAFC: the `edges` input is unused by the shipped driver (always None)")
         if not flows.is_cuda:
             raise RuntimeError("fgt_b200 LAFC runs on a CUDA (sm_90a) device only; there is no CPU fallback")
-        if getattr(self, "_graphed", None) is not None:
-            return self._graphed(flows.float().contiguous(), masks.float().contiguous())
+        if self._graphs is not None:
+            return self._graphed((), self._forward_impl, flows.float().contiguous(), masks.float().contiguous())
         return self._forward_impl(flows, masks)
 
     def _forward_impl(self, flows, masks):
@@ -246,7 +215,7 @@ class P3DNet(nn.Module):
         if T != self.T or H % 4 or W % 4:
             raise ValueError(f"LAFC input [T={T},{H}x{W}]: T must be {self.T} and H, W divisible by 4")
         dev = flows.device
-        P = self._packed if self._packed is not None else self._pack(dev)
+        P = self._packed.get(False) or self._pack(dev)
         x = torch.cat([flows.float(), masks.float()], 1).permute(0, 2, 1, 3, 4).contiguous()  # [b,T,3,H,W]
         outs = [self._forward_one(x[i], P, dev) for i in range(b)]
         return torch.cat([o[0] for o in outs], 0), torch.cat([o[1] for o in outs], 0)

@@ -277,6 +277,11 @@ def empty_split(shape, device):
     return torch.empty((2,) + tuple(shape), dtype=torch.bfloat16, device=device)
 
 
+def view16(t, *shape):
+    """A 16-bit activation tensor viewed as `shape`: [2, *shape] when split-bf16, [*shape] when fp16."""
+    return t.view(*shape) if t.dtype == torch.float16 else t.view(2, *shape)
+
+
 def plane_elems(s):
     """Element offset from the hi plane to the lo plane (works for row-sliced views too)."""
     return s.stride(0)
@@ -300,21 +305,26 @@ class ASeg:
 def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad_y=0, pad_z=0, groups=1,
             out_w, out_h=1, out_z=1, box_w=128, box_h=1, bn=128, bias=None, alpha=1.0, act=ACT_NONE,
             aux=None, aux_mode=AUX_NONE, out_f32=None, out_split=None, out_elem_offset=0,
-            os_z=0, os_y=0, os_x=None, os_c=1, rowmap=None, lin_batch=0, aux2=None, terms=3, out_f16=None, alg_k=None,
-            tag=""):
+            os_z=0, os_y=0, os_x=None, os_c=1, rowmap=None, lin_batch=0, aux2=None, terms=None, out_f16=None,
+            alg_k=None, tag=""):
     """Generic launcher for fgt_gemm_tc. Output strides are in elements; see include/fgt_b200.h.
-    terms=1: the A segments' tensors and w_split are plain fp16 tensors (one plane); out_f16: plain fp16 output
-    (an fp16 tensor passed as out_split is taken as out_f16)."""
+    The weight's dtype selects the MMA form: a split-bf16 weight takes split-bf16 A segments (3 terms), an fp16 weight
+    plain fp16 ones (1 term). out_split, the optional 16-bit output, is split-bf16 or plain fp16. Optional checks of
+    the caller's expectation: terms, the MMA form; out_f16, a 16-bit output that must be fp16."""
     lib = load()
-    if out_split is not None and out_split.dtype == torch.float16:
-        out_split, out_f16 = None, out_split
+    f16 = w_split.dtype == torch.float16
+    assert terms is None or terms == (1 if f16 else 3), "terms=1 takes fp16 weights, terms=3 split-bf16 ones"
+    if out_f16 is not None:
+        assert out_split is None and out_f16.dtype == torch.float16
+        out_split = out_f16
     d = FgtGemmDesc()
     d.num_segs = len(segs)
     k_real = 0
     for i, s in enumerate(segs):
+        assert (s.split.dtype == torch.float16) == f16, "A segments and weight: both split-bf16 or both fp16"
         a = d.seg[i]
         a.hi = s.split.data_ptr() + 2 * s.elem_offset
-        a.plane = plane_elems(s.split) if terms != 1 else 0
+        a.plane = 0 if f16 else plane_elems(s.split)
         a.C, a.DX, a.DY, a.DZ = s.C, s.DX, s.DY, s.DZ
         a.sx, a.sy, a.sz = s.sx, s.sy, s.sz
         a.c_base, a.c_per_group, a.c_count = s.c_base, s.c_per_group, s.c_count
@@ -322,8 +332,7 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
     d.kx, d.ky, d.kz, d.stride, d.dil = kx, ky, kz, stride, dil
     d.pad_x, d.pad_y, d.pad_z = pad_x, pad_y, pad_z
     d.w_hi = w_split.data_ptr()
-    d.w_plane = plane_elems(w_split) if terms != 1 else 0
-    assert (w_split.dtype == torch.float16) == (terms == 1), "terms=1 takes fp16 weights, terms=3 split-bf16 ones"
+    d.w_plane = 0 if f16 else plane_elems(w_split)
     d.N = N
     d.k_pad = w_split.shape[-1]
     d.groups = groups
@@ -338,17 +347,13 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
     d.out_f32 = (out_f32.data_ptr() + 4 * out_elem_offset) if out_f32 is not None else None
     if out_split is not None:
         d.out_hi = out_split.data_ptr() + 2 * out_elem_offset
-        d.out_plane = plane_elems(out_split)
-    if out_f16 is not None:
-        assert out_split is None and out_f16.dtype == torch.float16
-        d.out_hi = out_f16.data_ptr() + 2 * out_elem_offset
-        d.out_plane = 0
-        d.out_half = 1
+        d.out_plane = _plane16(out_split)
+        d.out_half = 1 if out_split.dtype == torch.float16 else 0
     d.os_z, d.os_y, d.os_c = os_z, os_y, os_c
     d.os_x = N if os_x is None else os_x
     d.rowmap = rowmap.data_ptr() if rowmap is not None else None
     d.lin_batch = lin_batch
-    d.terms = terms
+    d.terms = 1 if f16 else 3
     # algorithmic work: every valid output position x N x (taps * real input channels), padding excluded
     # (alg_k: the layer's true reduction length per output when the packed weight carries structural zeros, e.g. a
     #  grouped convolution run as block-diagonal super-groups — zeros are not algorithmic work)

@@ -24,6 +24,7 @@ import torch
 import torch.nn as nn
 
 from . import lib, ops
+from .graphs import NativeNet, workspace
 
 
 class _ResBlock(nn.Module):
@@ -86,7 +87,7 @@ class _UpdateBlock(nn.Module):
         self.mask = nn.Sequential(nn.Conv2d(128, 256, 3, padding=1), nn.ReLU(), nn.Conv2d(256, 576, 1))
 
 
-class RAFT(nn.Module):
+class RAFT(NativeNet):
     def __init__(self, args):
         super().__init__()
         self.args = args
@@ -103,27 +104,9 @@ class RAFT(nn.Module):
             for m in net.modules():
                 if isinstance(m, nn.Conv2d):
                     nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
-        self._packed = {}
-        self._bufs = {}
 
     def _mixed(self):
         return bool(getattr(self.args, "mixed_precision", False))
-
-    def _drop_graphs(self):
-        """Captured CUDA graphs hold the addresses of the packed weights / workspaces they were recorded with."""
-        if getattr(self, "_graphs", None) is not None:
-            self._graphs.clear()
-
-    def _apply(self, fn, *a, **k):
-        self._packed = {}
-        self._bufs = {}
-        self._drop_graphs()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._packed = {}
-        self._drop_graphs()
-        return super().load_state_dict(*a, **k)
 
     # ------------------------------------------------------------------ weight packing
     def _pack(self, dev, half=False):
@@ -185,15 +168,13 @@ class RAFT(nn.Module):
         self._packed[half] = P
         return P
 
-    def _buf(self, key, name, shape, dev, split=True, zero=False, dtype=None):
-        d = self._bufs.setdefault(key, {})
-        if name not in d:
-            if split:
-                shape, dtype = (2,) + tuple(shape), torch.bfloat16
-            elif dtype is None:
-                dtype = torch.float32
-            d[name] = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=dev)
-        return d[name]
+    def _allocators(self, key, dev, mixed):
+        """(B, A) workspace allocators of geometry `key`: B(name, shape, dtype=fp32) and A(name, shape) for the 16-bit
+        activations of the path, split-bf16 (fp32 path) or fp16 (mixed)."""
+        bufs = self._geo.setdefault(key, {})
+        a16 = torch.float16 if mixed else torch.bfloat16
+        return ((lambda nm, s, dtype=torch.float32: workspace(bufs, nm, s, dev, dtype)),
+                (lambda nm, s, zero=False: workspace(bufs, nm, s, dev, a16, zero)))
 
     # ------------------------------------------------------------------ encoders
     def _encoder(self, img, net, P, dev, n, mixed=False):
@@ -201,17 +182,15 @@ class RAFT(nn.Module):
         (split-bf16, or fp16 rows when mixed)."""
         _, _, H, W = img.shape
         inst = net == "fnet"
-        key = (net, n, H, W, mixed)
-        B = lambda nm, s, **kw: self._buf(key, nm, s, dev, **kw)  # noqa: E731
-        A, o16, rows = self._act_fmt(B, mixed)
+        B, A = self._allocators((net, n, H, W, mixed), dev, mixed)
         RELU = lib.ACT_RELU
         H2, W2 = H // 2, W // 2
         col = A("col", (n, H2, W2, 192))
         # 2*(x/255)-1 applied to in-bounds taps (raft.py:90-91); zero padding stays zero
         lib.im2col_nchw(img, None, col, k=7, stride=2, pad=3, replicate=False, OH=H2, OW=W2, scale=2.0 / 255.0,
                         shift=-1.0, tag=net + ".conv1")
-        stats = B("stats", (n * 128 * 2,), split=False, dtype=torch.float64)
-        raw = B("raw", (n * H2 * W2 * 64,), split=False)  # largest pre-norm conv output, reused
+        stats = B("stats", (n * 128 * 2,), dtype=torch.float64)
+        raw = B("raw", (n * H2 * W2 * 64,))  # largest pre-norm conv output, reused
 
         def raw_out(numel, shape):
             # mixed: left unrounded (autocast rounds it to fp16 before the norm); rounding it through an fp16 side
@@ -230,22 +209,22 @@ class RAFT(nn.Module):
             else:
                 if res is not None:
                     ops.conv(xs, P[name], kx=k, ky=k, stride=stride, pad_x=k // 2, pad_y=k // 2, act=RELU, aux=res,
-                             aux_mode=lib.AUX_ADD_RELU, out_f32=out_f32, **{o16: out_split})
+                             aux_mode=lib.AUX_ADD_RELU, out_f32=out_f32, out_split=out_split)
                 else:
                     ops.conv(xs, P[name], kx=k, ky=k, stride=stride, pad_x=k // 2, pad_y=k // 2,
-                             act=RELU if relu else lib.ACT_NONE, out_f32=out_f32, **{o16: out_split})
+                             act=RELU if relu else lib.ACT_NONE, out_f32=out_f32, out_split=out_split)
 
         x = A("x0", (n, H2, W2, 64))
-        xf = B("x0f", (n, H2, W2, 64), split=False)
+        xf = B("x0f", (n, H2, W2, 64))
         if inst:
             ro = raw_out(n * H2 * W2 * 64, (n, H2, W2, 64))
             r = ro["out_f32"]
-            ops.linear([(rows(col, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, **ro)
+            ops.linear([(lib.view16(col, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, **ro)
             lib.chan_stats(r, n, H2 * W2, 64, stats)
             lib.instnorm_act(r, stats, n, H2 * W2, 64, relu=True, out=xf, out_split=x)
         else:
-            ops.linear([(rows(col, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, act=RELU, out_f32=xf,
-                       **{o16: x})
+            ops.linear([(lib.view16(col, n * H2 * W2, 192), 192)], P[net + ".conv1"], n * H2 * W2, act=RELU, out_f32=xf,
+                       out_split=x)
         hh, ww, cin = H2, W2, 64
         for li, (dim, stride) in enumerate(((64, 1), (96, 2), (128, 2)), start=1):
             for bi in (0, 1):
@@ -255,26 +234,17 @@ class RAFT(nn.Module):
                 y1 = A(f"{k}.y1", (n, oh, ow, dim))
                 conv_norm_act([(x, cin)], k + ".conv1", n, hh, ww, dim, st, y1)
                 if st != 1:  # x = norm3(conv1x1_s2(x)), no ReLU (extractor.py:52-53)
-                    ds = B(f"{k}.ds", (n, oh, ow, dim), split=False)
+                    ds = B(f"{k}.ds", (n, oh, ow, dim))
                     ds16 = A(f"{k}.ds16", (n, oh, ow, dim)) if mixed else None  # makes `ds` fp16-valued; never read
                     conv_norm_act([(x, cin)], k + ".down", n, hh, ww, dim, st, ds16, out_f32=ds, relu=False, k=1)
                     res = ds
                 else:
                     res = xf
                 xo = A(f"{k}.out", (n, oh, ow, dim))
-                xof = B(f"{k}.outf", (n, oh, ow, dim), split=False)
+                xof = B(f"{k}.outf", (n, oh, ow, dim))
                 conv_norm_act([(y1, dim)], k + ".conv2", n, oh, ow, dim, 1, xo, out_f32=xof, res=res)
                 x, xf, hh, ww, cin = xo, xof, oh, ow, dim
         return x, hh, ww  # NHWC split [2, n, H/8, W/8, 128] (fp16 [n, H/8, W/8, 128] when mixed)
-
-    @staticmethod
-    def _act_fmt(B, mixed):
-        """Activation format of a path: (allocator, GEMM output keyword, [rows, C] view). fp32 path: split-bf16
-        [2, ...] buffers written through out_split; mixed: single-plane fp16 buffers written through out_f16."""
-        if mixed:
-            return ((lambda nm, s, **kw: B(nm, s, split=False, dtype=torch.float16, **kw)), "out_f16",
-                    (lambda t, r, c: t.view(r, c)))
-        return B, "out_split", (lambda t, r, c: t.view(2, r, c))
 
     # ------------------------------------------------------------------ forward
     def _forward_batch(self, im1, im2, iters, flow_init, test_mode, P, dev, mixed=False):
@@ -287,24 +257,21 @@ class RAFT(nn.Module):
         h, w = H // 8, W // 8
         npx = h * w
         tot = n * npx
-        key = ("iter", n, H, W, mixed)
-        B = lambda nm, s, **kw: self._buf(key, nm, s, dev, **kw)  # noqa: E731
-        A, o16, rows = self._act_fmt(B, mixed)
-        sh = (lambda t, *s: t.view(*s)) if mixed else (lambda t, *s: t.view(2, *s))  # noqa: E731
+        B, A = self._allocators(("iter", n, H, W, mixed), dev, mixed)
         RELU, SIG, TANH, NONE = lib.ACT_RELU, lib.ACT_SIGMOID, lib.ACT_TANH, lib.ACT_NONE
         # ---- feature net on all 2n images, 1x1 output conv -> fmaps [2, 2n*npx, 256] (split)
         f128, _, _ = self._encoder(torch.cat([im1, im2], 0), "fnet", P, dev, 2 * n, mixed)
-        fmap = B("fmap", (2 * tot, 256))
+        fmap = B("fmap", (2 * tot, 256), dtype=torch.bfloat16)
         if mixed:
             # fp16 output (autocast), then exactly to split-bf16: the 3-term correlation below is the reference's fp32
             # correlation of fmap.float() (raft.py:103-104)
             fmap16 = A("fmap16", (2 * tot, 256))
-            ops.linear([(rows(f128, 2 * tot, 128), 128)], P["fnet.conv2"], 2 * tot, out_f16=fmap16)
+            ops.linear([(lib.view16(f128, 2 * tot, 128), 128)], P["fnet.conv2"], 2 * tot, out_split=fmap16)
             lib.f16_to_split(fmap16, fmap)
         else:
             ops.linear([(f128.view(2, 2 * tot, 128), 128)], P["fnet.conv2"], 2 * tot, out_split=fmap)
         # ---- all-pairs correlation (corr.py:52-60): corr[i,j] = <f1_i, f2_j> / 16 per pair, then the pyramid
-        pyr = [B("corr0", (tot, h, w), split=False)]
+        pyr = [B("corr0", (tot, h, w))]
         for i in range(n):
             f1 = lib.ASeg(fmap[:, i * npx:(i + 1) * npx], 256, npx)
             f2 = fmap[:, (n + i) * npx:(n + i + 1) * npx]  # rows of image 2 as the "weight" operand [N=npx, K=256]
@@ -312,96 +279,89 @@ class RAFT(nn.Module):
                         tag="corr")
         hh, ww = h, w
         for i in range(1, 4):
-            nxt = B(f"corr{i}", (tot, hh // 2, ww // 2), split=False)
+            nxt = B(f"corr{i}", (tot, hh // 2, ww // 2))
             lib.avgpool2(pyr[-1], tot, hh, ww, nxt)
             pyr.append(nxt)
             hh, ww = hh // 2, ww // 2
         # ---- context net: net = tanh(c[:128]), inp = relu(c[128:]) (raft.py:112-115)
         c128, _, _ = self._encoder(im1, "cnet", P, dev, n, mixed)
         hsp = A("h", (tot, 128))
-        hf = B("hf", (tot, 128), split=False)
+        hf = B("hf", (tot, 128))
         xbuf = A("x", (tot, 256))  # GRU input x = [inp(128) | motion features(126) | flow(2)]
-        ops.linear([(rows(c128, tot, 128), 128)], P["cnet.net"], tot, act=TANH, out_f32=hf, **{o16: hsp})
-        ops.linear([(rows(c128, tot, 128), 128)], P["cnet.inp"], tot, act=RELU, os_x=256, **{o16: xbuf})
+        ops.linear([(lib.view16(c128, tot, 128), 128)], P["cnet.net"], tot, act=TANH, out_f32=hf, out_split=hsp)
+        ops.linear([(lib.view16(c128, tot, 128), 128)], P["cnet.inp"], tot, act=RELU, os_x=256, out_split=xbuf)
         # ---- iterations
-        coords = B("coords", (tot, 2), split=False)
+        coords = B("coords", (tot, 2))
         ys, xs = torch.meshgrid(torch.arange(h, device=dev), torch.arange(w, device=dev), indexing="ij")
         coords.view(n, npx, 2).copy_(torch.stack([xs, ys], -1).reshape(1, npx, 2).float().expand(n, npx, 2))
         if flow_init is not None:
             coords.add_(flow_init.permute(0, 2, 3, 1).reshape(tot, 2).float())
-        flow_nchw = B("flow", (n, 2, h, w), split=False)
+        flow_nchw = B("flow", (n, 2, h, w))
         lib.raft_flow_update(coords, None, h, w, flow_nchw, xbuf, 254, n=n)
         look = A("look", (tot, 384), zero=True)
         cor1 = A("cor1", (n, h, w, 256))
         corflo = A("corflo", (n, h, w, 256))  # [cor(192) | flo(64)]
         fcol = A("fcol", (n, h, w, 128))
         flo1 = A("flo1", (n, h, w, 128))
-        z = B("z", (tot, 128), split=False)
+        z = B("z", (tot, 128))
         rh = A("rh", (n, h, w, 128))
         fh = A("fh", (n, h, w, 256))
-        delta = B("delta", (tot, 2), split=False)
-        fh2y = B("fh2y", (32, tot), split=False)  # column-planar partial products of the flow head
+        delta = B("delta", (tot, 2))
+        fh2y = B("fh2y", (32, tot))  # column-planar partial products of the flow head
         m0 = A("m0", (n, h, w, 256))
-        mask = B("mask", (tot, 576), split=False)
-        h4 = sh(hsp, n, h, w, 128)
-        x4 = sh(xbuf, n, h, w, 256)
+        mask = B("mask", (tot, 576))
+        h4 = lib.view16(hsp, n, h, w, 128)
+        x4 = lib.view16(xbuf, n, h, w, 256)
         ups = []
         for it in range(iters):
             lib.corr_lookup(pyr, coords, tot, 4, look)
             # motion encoder (update.py:89-97)
-            ops.linear([(look, 384)], P["convc1"], tot, act=RELU, **{o16: rows(cor1, tot, 256)})
+            ops.linear([(look, 384)], P["convc1"], tot, act=RELU, out_split=lib.view16(cor1, tot, 256))
             ops.conv([(cor1, 256)], P["convc2"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_c_total=256,
-                     out_c_offset=0, **{o16: corflo})
+                     out_c_offset=0, out_split=corflo)
             lib.im2col_nchw(flow_nchw, None, fcol, k=7, stride=1, pad=3, replicate=False, OH=h, OW=w)
-            ops.linear([(rows(fcol, tot, 128), 128)], P["convf1"], tot, act=RELU, **{o16: rows(flo1, tot, 128)})
+            ops.linear([(lib.view16(fcol, tot, 128), 128)], P["convf1"], tot, act=RELU, out_split=lib.view16(flo1, tot, 128))
             ops.conv([(flo1, 128)], P["convf2"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_c_total=256,
-                     out_c_offset=192, **{o16: corflo})
+                     out_c_offset=192, out_split=corflo)
             ops.conv([(corflo, 256)], P["mconv"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_c_total=256,
-                     out_c_offset=128, **{o16: x4})
+                     out_c_offset=128, out_split=x4)
             # SepConvGRU (update.py:45-60): horizontal (1x5) then vertical (5x1)
             for s, (kx, ky) in (("1", (5, 1)), ("2", (1, 5))):
                 kw = dict(kx=kx, ky=ky, pad_x=kx // 2, pad_y=ky // 2, seg_counts=[128, 256])
                 # z = sigmoid(convz(hx)) and r*h = sigmoid(convr(hx)) * h as ONE N=256 GEMM over the shared input
                 ops.conv([(h4, 128), (x4, 256)], P[f"gru.zr{s}"], act=SIG, aux=hf, aux_mode=lib.AUX_GRU_ZR,
-                         out_f32=z.view(n, h, w, 128), out_c_total=128, **{o16: rh}, **kw)
+                         out_f32=z.view(n, h, w, 128), out_c_total=128, out_split=rh, **kw)
                 ops.conv([(rh, 128), (x4, 256)], P[f"gru.q{s}"], act=TANH, aux=hf, aux2=z, aux_mode=lib.AUX_GRU,
-                         out_f32=hf.view(n, h, w, 128), **{o16: h4}, **kw)
+                         out_f32=hf.view(n, h, w, 128), out_split=h4, **kw)
             # flow head (update.py:13-14)
-            ops.conv([(h4, 128)], P["fh1"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, **{o16: fh})
+            ops.conv([(h4, 128)], P["fh1"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=fh)
             # 256->2 conv as "taps as N" (1x1 GEMM with N = 18 -> 32, then shift-and-add): A is read once, not 9x
-            ops.linear([(rows(fh, tot, 256), 256)], P["fh2t"], tot, out_f32=fh2y, os_x=1, os_c=tot)
+            ops.linear([(lib.view16(fh, tot, 256), 256)], P["fh2t"], tot, out_f32=fh2y, os_x=1, os_c=tot)
             lib.tapsum(fh2y, n, h, w, 2, 3, P["fh2"]["b"], NONE, delta, nchw=False, tag="fh2")
             lib.raft_flow_update(coords, delta, h, w, flow_nchw, xbuf, 254, n=n, delta_f16=mixed)
             if not test_mode or it == iters - 1:
                 # mask head scaled by 0.25 (update.py:122-125,135) + convex upsampling (raft.py:73-84)
-                ops.conv([(h4, 128)], P["mask0"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, **{o16: m0})
-                ops.linear([(rows(m0, tot, 256), 256)], P["mask2"], tot, alpha=0.25, out_f32=mask)
+                ops.conv([(h4, 128)], P["mask0"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=m0)
+                ops.linear([(lib.view16(m0, tot, 256), 256)], P["mask2"], tot, alpha=0.25, out_f32=mask)
                 up = torch.empty(n, 2, 8 * h, 8 * w, device=dev)
                 lib.convex_upsample(mask, flow_nchw, h, w, up, n=n)
                 ups.append(up)
         return flow_nchw.clone(), ups
 
-    def enable_cuda_graph(self, on=True):
-        """Replay whole forwards as CUDA graphs, one per (geometry, iters, test_mode, precision) (fgt_b200/graphs.py)."""
-        self._graphs = {} if on else None
-
     def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False):
         if not image1.is_cuda:
             raise RuntimeError("fgt_b200 RAFT runs on a CUDA (sm_90a) device only; there is no CPU fallback")
         mixed = self._mixed()  # read on every call, as the reference reads self.args.mixed_precision
-        if getattr(self, "_graphs", None) is not None and flow_init is None:
-            from .graphs import GraphedCall
-            key = (iters, bool(test_mode), mixed)
-            if key not in self._graphs:
-                self._graphs[key] = GraphedCall(
-                    lambda a, b, _it=iters, _tm=test_mode, _mx=mixed: self._forward_impl(a, b, _it, None, _tm, _mx))
-            out = self._graphs[key](image1.float().contiguous(), image2.float().contiguous())
+        if self._graphs is not None and flow_init is None:
+            out = self._graphed((iters, bool(test_mode), mixed),
+                                lambda a, b: self._forward_impl(a, b, iters, None, test_mode, mixed),
+                                image1.float().contiguous(), image2.float().contiguous())
             return list(out) if not test_mode else out
         return self._forward_impl(image1, image2, iters, flow_init, test_mode, mixed)
 
     def _forward_impl(self, image1, image2, iters, flow_init, test_mode, mixed=False):
         dev = image1.device
-        P = self._packed[mixed] if mixed in self._packed else self._pack(dev, mixed)
+        P = self._packed.get(mixed) or self._pack(dev, mixed)
         image1, image2 = image1.float().contiguous(), image2.float().contiguous()
         lo, ups = self._forward_batch(image1, image2, iters, flow_init, test_mode, P, dev, mixed)
         if test_mode:
