@@ -79,24 +79,41 @@ def test_schedules_bit_identical_tiles_and_k_steps(tiles, bn, terms):
 
 
 @pytest.mark.parametrize("bn", (64, 128))
-@pytest.mark.parametrize("act", ("none", "leaky02", "relu", "sigmoid", "tanh"))
-@pytest.mark.parametrize("aux_mode", ("none", "add", "mul"))
+@pytest.mark.parametrize("act", ("none", "leaky02", "relu", "sigmoid", "tanh", "leaky001"))
+# "half" is not an aux mode: aux NONE with 1-term operands and fp16 + fp32 outputs (the out_half rounding path)
+@pytest.mark.parametrize("aux_mode", ("none", "add", "mul", "add_pre", "add_relu", "gru", "gru_zr", "half"))
 def test_schedules_bit_identical_epilogues(aux_mode, act, bn):
-    """Every kExt = 0 activation x aux mode, fp32 + split outputs, M tail (1500 rows) and an N tail (N = 712)."""
+    """Every kExt = 0 activation x aux mode, fp32 + split outputs, M tail (1500 rows) and an N tail (N = 712); and the
+    kExt = 1 instantiation: LeakyReLU(0.01), pre-activation add, add + ReLU, the GRU update (aux2 = z), the fused z | r
+    gates (N = 256, two C-channel outputs) and 1-term fp16 + fp32 outputs ("half", the mixed-precision rounding)."""
     lib, _ = _lib()
     dev = torch.device("cuda:0")
-    M, N, K = 1500, 712, 320
-    a_p, w_p, b = _operands(M, N, K, 3, seed=5)
+    M, K = 1500, 320
+    N = 256 if aux_mode == "gru_zr" else 712
+    terms = 1 if aux_mode == "half" else 3
+    a_p, w_p, b = _operands(M, N, K, terms, seed=5)
     aux = torch.randn(M, N, device=dev)
+    z = torch.rand(M, N, device=dev)
     acts = dict(none=lib.ACT_NONE, leaky02=lib.ACT_LEAKY02, relu=lib.ACT_RELU, sigmoid=lib.ACT_SIGMOID,
-                tanh=lib.ACT_TANH)
-    modes = dict(none=lib.AUX_NONE, add=lib.AUX_ADD, mul=lib.AUX_MUL)
+                tanh=lib.ACT_TANH, leaky001=lib.ACT_LEAKY001)
+    modes = dict(none=lib.AUX_NONE, add=lib.AUX_ADD, mul=lib.AUX_MUL, add_pre=lib.AUX_ADD_PRE,
+                 add_relu=lib.AUX_ADD_RELU, gru=lib.AUX_GRU, gru_zr=lib.AUX_GRU_ZR, half=lib.AUX_NONE)
 
     def run():
+        if aux_mode == "gru_zr":   # z -> fp32 [M, N/2], r*h -> split [M, N/2], h = aux [M, N/2]
+            zo = torch.full((M, N // 2), float("nan"), device=dev)
+            rh = torch.full((2, M, N // 2), float("nan"), dtype=torch.bfloat16, device=dev)
+            lib.gemm_tc([lib.ASeg(a_p, K, M)], w_p, N, out_w=M, bn=bn, bias=b, act=acts[act],
+                        aux=aux[:, :N // 2].contiguous(), aux_mode=lib.AUX_GRU_ZR, out_f32=zo, out_split=rh, os_x=N // 2)
+            return zo, rh
         o32 = torch.full((M, N), float("nan"), device=dev)
-        osp = torch.full((2, M, N), float("nan"), dtype=torch.bfloat16, device=dev)
+        if aux_mode == "half":
+            osp = torch.full((M, N), float("nan"), dtype=torch.float16, device=dev)
+        else:
+            osp = torch.full((2, M, N), float("nan"), dtype=torch.bfloat16, device=dev)
         lib.gemm_tc([lib.ASeg(a_p, K, M)], w_p, N, out_w=M, bn=bn, bias=b, act=acts[act],
-                    aux=aux if aux_mode != "none" else None, aux_mode=modes[aux_mode], out_f32=o32, out_split=osp)
+                    aux=aux if aux_mode not in ("none", "half") else None, aux_mode=modes[aux_mode],
+                    aux2=z if aux_mode == "gru" else None, out_f32=o32, out_split=osp)
         return o32, osp
 
     _assert_equal(_both(run), f"aux={aux_mode} act={act} bn={bn}")

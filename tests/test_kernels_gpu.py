@@ -160,6 +160,88 @@ def test_attention_windowed(frames, heads, nwin, nglob, qs):
     assert D.window_case(frames, heads, nwin, nglob, qscale=qs)
 
 
+def _zone_rowmap(t, h, w, gs=2):
+    """FGT's temporal-zone row map (fgt_model._geometry): zone-major rows (frame, y, x inside the zone) -> token index
+    of a [t, h, w] grid, -1 for the rows of the zone padding past the grid."""
+    zh, zw = -(-h // gs), -(-w // gs)
+    zy, zx, ti, yy, xx = torch.meshgrid(torch.arange(gs), torch.arange(gs), torch.arange(t), torch.arange(zh),
+                                        torch.arange(zw), indexing="ij")
+    Y, X = zy * zh + yy, zx * zw + xx
+    tok = torch.where((Y < h) & (X < w), (ti * h + Y) * w + X, torch.full_like(Y, -1))
+    return tok.reshape(-1).to(torch.int32), zh * zw
+
+
+@pytest.mark.parametrize("f16", (False, True))
+@pytest.mark.parametrize("T,sharded", [(3, False), (5, False), (3, True)])
+def test_attention_production_layouts(T, sharded, f16):
+    """TMHSA as the FGT forward calls it: 4 zones of Lz = 11*18*T keys (odd T, not a multiple of the 64-key tile, so the
+    last key tile of a zone runs into the next zone's rows), Q|K|V in one fused [rows, 3d] buffer read through k_off /
+    v_off, the output scattered through the zone row map (-1 rows dropped). sharded: the frame-sharded call, Q of this
+    rank's first frame only (Lq = Lz / T < Lk) from its own buffer, K|V from a [rows, 2d] buffer with v_off = d.
+    The first 64 key rows of every zone (and the rows past the last zone) are scaled so that one of them would dominate
+    the softmax of any query that wrongly saw it. Output rows no query row maps to keep their sentinel bit for bit.
+    Bars: KTOL (split-bf16) or test_fgt_mixed_gpu's 2e-3 relative (fp16) against a float64 softmax of the operands."""
+    import math
+    lib = _lib()
+    dev = torch.device("cuda:0")
+    H, d, h, w = 4, 512, 21, 36
+    g = torch.Generator().manual_seed(100 * T + sharded)
+    zl = -(-h // 2) * -(-w // 2)
+    zones, Lk = 4, T * zl
+    t = 1 if sharded else T
+    Lq = t * zl
+    rowmap, _ = _zone_rowmap(t, h, w)
+    kv_cols = 2 * d if sharded else 3 * d
+    kv = torch.randn(zones * Lk + 64, kv_cols, generator=g)
+    koff = 0 if sharded else d
+    for z in range(zones + 1):   # dominating keys at the head of every zone's rows and past the last zone
+        kv[z * Lk:z * Lk + 64, koff:koff + d] *= 6.0
+    q_src = torch.randn(zones * Lq, d, generator=g) if sharded else None
+    enc = (lambda x: x.half().contiguous()) if f16 else lib.to_split   # noqa: E731
+    kv16 = enc(kv)
+    q16 = enc(q_src) if sharded else kv16
+    val = (lambda s: s.double()) if f16 else (lambda s: s[0].double() + s[1].double())   # noqa: E731
+    kvv, qv = val(kv16), val(q16)
+    rows_out = T * h * w + 37   # every token row of the window plus rows no query maps to
+    sent = torch.full((rows_out, d), -1234.5, dtype=torch.float16) if f16 else \
+        torch.full((2, rows_out, d), -1234.5, dtype=torch.bfloat16)
+    out = sent.clone().to(dev)
+    rm = rowmap.to(dev)
+    scale = 1.0 / math.sqrt(128)
+    if sharded:
+        lib.attention(q16.to(dev), kv16.to(dev), kv16.to(dev), out, batches=zones, heads=H, Lq=Lq, Lk=Lk, q_ld=d,
+                      k_ld=2 * d, v_ld=2 * d, out_ld=d, q_batch_stride=Lq * d, k_batch_stride=Lk * 2 * d,
+                      v_batch_stride=Lk * 2 * d, out_batch_stride=Lq * d, scale=scale, v_off=d, out_rowmap=rm)
+    else:
+        x = kv16.to(dev)
+        lib.attention(x, x, x, out, batches=zones, heads=H, Lq=Lq, Lk=Lk, q_ld=3 * d, k_ld=3 * d, v_ld=3 * d, out_ld=d,
+                      q_batch_stride=Lk * 3 * d, k_batch_stride=Lk * 3 * d, v_batch_stride=Lk * 3 * d,
+                      out_batch_stride=Lq * d, scale=scale, k_off=d, v_off=2 * d, out_rowmap=rm)
+    torch.cuda.synchronize()
+    out = out.cpu()
+    want = torch.zeros(rows_out, d, dtype=torch.float64)
+    hit = torch.zeros(rows_out, dtype=torch.bool)
+    for z in range(zones):
+        qz = qv[z * Lq:(z + 1) * Lq] if sharded else qv[z * Lk:z * Lk + Lq, :d]
+        kz = kvv[z * Lk:(z + 1) * Lk, koff:koff + d]
+        vz = kvv[z * Lk:(z + 1) * Lk, koff + d:koff + 2 * d]
+        qh, kh, vh = (a.reshape(-1, H, 128).transpose(0, 1) for a in (qz, kz, vz))
+        o = (torch.softmax(qh @ kh.transpose(1, 2) * scale, -1) @ vh).transpose(0, 1).reshape(Lq, d)
+        m = rowmap[z * Lq:(z + 1) * Lq].long()
+        keep = m >= 0
+        want[m[keep]] = o[keep]
+        hit[m[keep]] = True
+    assert int(hit.sum()) == t * h * w
+    if f16:
+        assert torch.equal(out[~hit], sent[~hit]), "rows outside the row map written"
+        got = out[hit].double()
+        rel = ((got - want[hit]).norm() / want[hit].norm()).item()
+        assert torch.isfinite(got).all() and rel < 2e-3, rel
+    else:
+        assert torch.equal(out[:, ~hit], sent[:, ~hit]), "rows outside the row map written"
+        assert_close(out[0, hit].double() + out[1, hit].double(), want[hit], KTOL, "zone attention")
+
+
 def test_rownorm_gather_affine():
     lib = _lib()
     dev = torch.device("cuda:0")

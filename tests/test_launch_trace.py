@@ -82,10 +82,10 @@ class _Recorder:
 
 
 @contextlib.contextmanager
-def recording():
+def recording(rec=None):
     """Swaps the library `lib.load()` returns for a recorder (argument types declared by `lib.load()` itself) and
-    the stream handle for a constant."""
-    rec = _Recorder()
+    the stream handle for a constant. `rec`: a stand-in other than a fresh _Recorder (tests/gemm_emulator.py)."""
+    rec = _Recorder() if rec is None else rec
     saved = lib._lib, lib.LIB_PATH, lib.stream_ptr, ctypes.CDLL
     try:
         lib._lib, lib.LIB_PATH, ctypes.CDLL = None, __file__, (lambda path: rec)
