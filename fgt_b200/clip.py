@@ -42,10 +42,8 @@ def inpaint_clip_device(model, frames, masks, flows, step=10, num_ref=-1, neighb
         raise ValueError(f"clip: masks {tuple(masks.shape)} / flows {tuple(flows.shape)} do not match frames {tuple(frames.shape)}")
     frames, flows = frames.float().contiguous(), flows.float().contiguous()
     masks = (masks != 0).to(torch.uint8).contiguous()
-    L = lib.load()
-    sp = lib.stream_ptr
     fmax = torch.empty(N, 2, dtype=torch.float32, device=dev)
-    lib.check(L.fgt_plane_max(flows.data_ptr(), N * 2, H * W, fmax.data_ptr(), sp()), "fgt_plane_max")
+    lib.call("fgt_plane_max", flows, N * 2, H * W, fmax)
     comp = torch.empty(N, H, W, 3, dtype=torch.float32, device=dev)
     seen = [False] * N
     for f, neighbor_ids, ref_ids in window_schedule(N, neighbor_stride, step, num_ref):
@@ -55,24 +53,19 @@ def inpaint_clip_device(model, frames, masks, flows, step=10, num_ref=-1, neighb
         w_frames = torch.empty(1, t, 3, H, W, dtype=torch.float32, device=dev)
         w_flows = torch.empty(1, t, 2, H, W, dtype=torch.float32, device=dev)
         w_masks = torch.empty(1, t, 1, H, W, dtype=torch.float32, device=dev)
-        lib.check(L.fgt_window_gather(frames.data_ptr(), masks.data_ptr(), flows.data_ptr(), fmax.data_ptr(),
-                                      d_ids.data_ptr(), t, H, W, w_frames.data_ptr(), w_flows.data_ptr(),
-                                      w_masks.data_ptr(), sp()), "fgt_window_gather")
+        lib.call("fgt_window_gather", frames, masks, flows, fmax, d_ids, t, H, W, w_frames, w_flows, w_masks)
         with torch.no_grad():
             filled = model(w_frames, w_flows, w_masks)
         filled = filled.float().contiguous()
         if tuple(filled.shape) != (t, 3, H, W):
             raise ValueError(f"clip: model returned {tuple(filled.shape)}, expected {(t, 3, H, W)}")
         first = torch.tensor([0 if seen[i] else 1 for i in neighbor_ids], dtype=torch.uint8, device=dev)
-        lib.check(L.fgt_window_compose(filled.data_ptr(), frames.data_ptr(), masks.data_ptr(), d_ids.data_ptr(),
-                                       first.data_ptr(), k, H, W, comp.data_ptr(), sp()), "fgt_window_compose")
-        lib.COUNTERS["launches"] += 2
+        lib.call("fgt_window_compose", filled, frames, masks, d_ids, first, k, H, W, comp)
         for i in neighbor_ids:
             seen[i] = True
     assert all(seen)
     out = torch.empty(N, H, W, 3, dtype=torch.uint8, device=dev)
-    lib.check(L.fgt_comp_to_u8(comp.data_ptr(), comp.numel(), out.data_ptr(), sp()), "fgt_comp_to_u8")
-    lib.COUNTERS["launches"] += 2
+    lib.call("fgt_comp_to_u8", comp, comp.numel(), out)
     return out
 
 

@@ -19,9 +19,7 @@ def warp(feat, flow, mode):
     flow = flow.to(feat.device).float().contiguous()
     out = torch.empty_like(feat)
     wsum = torch.empty(b, h, w, dtype=torch.float32, device=feat.device)
-    lib.check(lib.load().fgt_flow_splat(feat.data_ptr(), flow.data_ptr(), b, c, h, w, int(mode == "backward"),
-                                        out.data_ptr(), wsum.data_ptr(), lib.stream_ptr()), "fgt_flow_splat")
-    lib.COUNTERS["launches"] += 2
+    lib.call("fgt_flow_splat", feat, flow, b, c, h, w, int(mode == "backward"), out, wsum, kernels=2)
     return out
 
 

@@ -52,10 +52,7 @@ def inpaint_telea(images, masks, radius=3, device=None, timing=None):
         stride = H * W
     else:
         raise ValueError(f"inpaint_telea: masks {tuple(m.shape)} must be [H,W] or [B,H,W] for images {tuple(img.shape)}")
-    L = lib.load()
-    per_mask = L.fgt_inpaint_telea_workspace(1, H, W)
-    if per_mask < 0:
-        lib.check(int(per_mask), "fgt_inpaint_telea_workspace")
+    per_mask = lib.call("fgt_inpaint_telea_workspace", 1, H, W)
     out = torch.empty_like(img)
     chunk = B if stride == 0 else max(1, min(B, WORKSPACE_BUDGET // per_mask))
     ws = torch.empty(per_mask * (1 if stride == 0 else chunk), dtype=torch.uint8, device=dev)
@@ -65,14 +62,12 @@ def inpaint_telea(images, masks, radius=3, device=None, timing=None):
         e = min(B, s + chunk)
         if ev:
             ev[0].record()
-        lib.check(L.fgt_inpaint_telea_plan(m.data_ptr() + s * stride, 1 if stride == 0 else e - s, H, W, float(radius),
-                                           ws.data_ptr(), ws.numel(), lib.stream_ptr()), "fgt_inpaint_telea_plan")
-        lib.COUNTERS["launches"] += 1                     # marches + levels
+        lib.call("fgt_inpaint_telea_plan", m.data_ptr() + s * stride, 1 if stride == 0 else e - s, H, W, float(radius),
+                 ws, ws.numel(), kernels=2)                # marches + levels
         if ev:
             ev[1].record()
-        lib.check(L.fgt_inpaint_telea_fill(img[s].data_ptr(), e - s, H, W, C, 1 if stride == 0 else 0, float(radius),
-                                           ws.data_ptr(), ws.numel(), out[s].data_ptr(), lib.stream_ptr()),
-                  "fgt_inpaint_telea_fill")
+        lib.call("fgt_inpaint_telea_fill", img[s], e - s, H, W, C, 1 if stride == 0 else 0, float(radius), ws, ws.numel(),
+                 out[s])
         if ev:
             ev[2].record()
             ev[2].synchronize()
@@ -95,8 +90,8 @@ def inpaint_telea_host(image, mask, radius=3):
         raise ValueError(f"inpaint_telea_host: image {img.shape} / mask {m.shape} must be [H,W(,C)] / [H,W]")
     out = np.empty_like(img)
     C = 1 if img.ndim == 2 else img.shape[2]
-    lib.check_rc(lib.load().fgt_inpaint_telea_host(img.ctypes.data, m.ctypes.data, img.shape[0], img.shape[1], C,
-                                                    float(radius), out.ctypes.data), "fgt_inpaint_telea_host")
+    lib.call("fgt_inpaint_telea_host", img.ctypes.data, m.ctypes.data, img.shape[0], img.shape[1], C, float(radius),
+             out.ctypes.data)
     return out
 
 
@@ -114,13 +109,11 @@ def prepare_gradients(video, mask, mask_dilated, device=None):
     v = torch.from_numpy(np.ascontiguousarray(frames)).to(dev)
     m = torch.from_numpy(hole).to(dev).to(torch.uint8)
     md = torch.from_numpy(np.ascontiguousarray(np.moveaxis(np.asarray(mask_dilated), -1, 0)).astype(np.uint8)).to(dev)
-    L = lib.load()
     u8 = torch.empty((N, H, W, 3), dtype=torch.uint8, device=dev)
-    lib.check(L.fgt_grad_prep_pre(v.data_ptr(), m.data_ptr(), N, H, W, u8.data_ptr(), lib.stream_ptr()), "fgt_grad_prep_pre")
+    lib.call("fgt_grad_prep_pre", v, m, N, H, W, u8)
     filled = inpaint_telea(u8, m, 3, device=dev)
     gx = torch.empty((N, H, W, 3), dtype=torch.float32, device=dev)
     gy = torch.empty_like(gx)
-    lib.check(L.fgt_grad_prep_post(filled.data_ptr(), md.data_ptr(), N, H, W, gx.data_ptr(), gy.data_ptr(), lib.stream_ptr()),
-              "fgt_grad_prep_post")
+    lib.call("fgt_grad_prep_post", filled, md, N, H, W, gx, gy)
     frames[hole] = 0                                                     # :592, in place
     return np.moveaxis(gx.cpu().numpy(), 0, -1), np.moveaxis(gy.cpu().numpy(), 0, -1)

@@ -33,9 +33,7 @@ def binary_dilation(masks, iterations=1, device=None):
         raise ValueError("binary_dilation: iterations must be >= 1 (scipy's 'repeat until stable' mode is not used by the driver)")
     B, H, W = m.shape
     tmp, out = torch.empty_like(m), torch.empty_like(m)
-    lib.check(lib.load().fgt_binary_dilate(m.data_ptr(), B, H, W, iterations, tmp.data_ptr(), out.data_ptr(), lib.stream_ptr()),
-              "fgt_binary_dilate")
-    lib.COUNTERS["launches"] += iterations - 1
+    lib.call("fgt_binary_dilate", m, B, H, W, iterations, tmp, out, kernels=iterations)
     return out.bool()
 
 
@@ -46,16 +44,13 @@ def binary_fill_holes(masks, device=None, passes_per_check=3):
     B, H, W = m.shape
     reach = torch.empty_like(m)
     changed = torch.zeros(1, dtype=torch.int32, device=dev)
-    L = lib.load()
-    lib.check(L.fgt_fill_holes_init(m.data_ptr(), B, H, W, reach.data_ptr(), lib.stream_ptr()), "fgt_fill_holes_init")
+    lib.call("fgt_fill_holes_init", m, B, H, W, reach, kernels=0)   # a memset
     for _ in range(H * W):                      # terminates: every pass but the last adds at least one pixel
-        lib.check(L.fgt_fill_holes_pass(m.data_ptr(), B, H, W, reach.data_ptr(), changed.data_ptr(), passes_per_check,
-                                        lib.stream_ptr()), "fgt_fill_holes_pass")
-        lib.COUNTERS["launches"] += 2 * passes_per_check - 1
+        lib.call("fgt_fill_holes_pass", m, B, H, W, reach, changed, passes_per_check, kernels=2 * passes_per_check)
         if int(changed.item()) == 0:            # one host sync per group of passes
             break
     out = torch.empty_like(m)
-    lib.check(L.fgt_fill_holes_finish(reach.data_ptr(), B, H, W, out.data_ptr(), lib.stream_ptr()), "fgt_fill_holes_finish")
+    lib.call("fgt_fill_holes_finish", reach, B, H, W, out)
     return out.bool()
 
 
@@ -68,8 +63,7 @@ def resize_nearest(masks, size, device=None):
         t = t[..., None]
     B, H, W, C = t.shape
     out = torch.empty(B, size[0], size[1], C, dtype=torch.uint8, device=dev)
-    lib.check(lib.load().fgt_resize_nearest_u8(t.data_ptr(), B, H, W, C, size[0], size[1], out.data_ptr(), lib.stream_ptr()),
-              "fgt_resize_nearest_u8")
+    lib.call("fgt_resize_nearest_u8", t, B, H, W, C, size[0], size[1], out)
     return out[..., 0] if squeeze else out
 
 
@@ -85,6 +79,5 @@ def resize_bilinear(x, size, layout="nhwc", channel_scale=None, device=None):
     B, H, W, C = (t.shape[0], t.shape[2], t.shape[3], t.shape[1]) if nchw else tuple(t.shape)
     out = torch.empty((B, C, size[0], size[1]) if nchw else (B, size[0], size[1], C), dtype=torch.float32, device=dev)
     s0, s1 = channel_scale if channel_scale is not None else (1.0, 1.0)
-    lib.check(lib.load().fgt_resize_bilinear_f32(t.data_ptr(), B, H, W, C, size[0], size[1], 1 if nchw else 0, float(s0),
-                                                 float(s1), out.data_ptr(), lib.stream_ptr()), "fgt_resize_bilinear_f32")
+    lib.call("fgt_resize_bilinear_f32", t, B, H, W, C, size[0], size[1], 1 if nchw else 0, float(s0), float(s1), out)
     return out

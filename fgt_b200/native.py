@@ -53,14 +53,10 @@ def composite_native(comp, frames, masks, frame_dilates, device=None):
     M = hole.shape[0]
     shared = int(M == 1)
     k, r = native_window(h, w, imgH, imgW, frame_dilates)
-    L = lib.load()
-    nbytes = L.fgt_native_workspace(M, h, w, k)
-    if nbytes < 0:
-        lib.check(int(nbytes), "fgt_native_workspace")
+    nbytes = lib.call("fgt_native_workspace", M, h, w, k)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     D = morph.binary_dilation(hole, r + 2 * k, device=dev)              # bool storage: one byte, 0 / 1
-    lib.check(L.fgt_native_count(D.data_ptr(), M, h, w, k, ws.data_ptr(), nbytes, lib.stream_ptr()), "fgt_native_count")
+    lib.call("fgt_native_count", D, M, h, w, k, ws, nbytes, kernels=2)
     out = torch.empty_like(fr)
-    lib.check(L.fgt_native_composite(cp.data_ptr(), N, imgH, imgW, fr.data_ptr(), h, w, C, shared, k, ws.data_ptr(), nbytes,
-                                     out.data_ptr(), lib.stream_ptr()), "fgt_native_composite")
+    lib.call("fgt_native_composite", cp, N, imgH, imgW, fr, h, w, C, shared, k, ws, nbytes, out)
     return out

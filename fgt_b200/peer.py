@@ -37,12 +37,11 @@ class PeerGroup:
     def alloc(self, nbytes):
         """Collective: every rank allocates `nbytes` (zeroed). Returns ([address on this rank of rank q's buffer
         for q in ranks], uint8 torch view of the local buffer)."""
-        L = lib.load()
         p = ctypes.c_void_p()
-        lib.check_rc(L.fgt_peer_alloc(nbytes, ctypes.byref(p)), "fgt_peer_alloc")
+        lib.call("fgt_peer_alloc", nbytes, ctypes.byref(p))
         self._local.append(p.value)
         handle = ctypes.create_string_buffer(64)
-        lib.check_rc(L.fgt_peer_export(p, handle), "fgt_peer_export")
+        lib.call("fgt_peer_export", p, handle)
         handles = [None] * self.world
         if self.world > 1:
             dist.all_gather_object(handles, handle.raw, group=self.group)
@@ -52,7 +51,7 @@ class PeerGroup:
                 ptrs.append(p.value)
                 continue
             r = ctypes.c_void_p()
-            lib.check_rc(L.fgt_peer_import(handles[q], ctypes.byref(r)), "fgt_peer_import")
+            lib.call("fgt_peer_import", handles[q], ctypes.byref(r))
             self._imported.append(r.value)
             ptrs.append(r.value)
         raw = _Raw(p.value, nbytes)
@@ -62,16 +61,24 @@ class PeerGroup:
 
     def barrier(self):
         """Enqueue the device-side barrier on the current stream (no host synchronisation)."""
-        lib.check(lib.load().fgt_peer_barrier(self._flag_arr, self.world, self.rank, ctypes.c_void_p(self.epoch_ptr),
-                                              lib.stream_ptr()), "fgt_peer_barrier")
+        lib.call("fgt_peer_barrier", self._flag_arr, self.world, self.rank, self.epoch_ptr)
 
     def close(self):
+        """Unimports the peers' buffers and frees this rank's, attempting every one; raises the first failure."""
         torch.cuda.synchronize()
-        L = lib.load()
+        failed = []
         for r in self._imported:
-            L.fgt_peer_unimport(ctypes.c_void_p(r))
+            try:
+                lib.call("fgt_peer_unimport", r)
+            except RuntimeError as e:
+                failed.append(e)
         if self.world > 1:
             dist.barrier(group=self.group)  # nobody frees memory a peer still has mapped
         for p in self._local:
-            L.fgt_peer_free(ctypes.c_void_p(p))
+            try:
+                lib.call("fgt_peer_free", p)
+            except RuntimeError as e:
+                failed.append(e)
         self._imported, self._local, self._keep = [], [], []
+        if failed:
+            raise failed[0]

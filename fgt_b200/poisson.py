@@ -33,10 +33,6 @@ def _mask(m, dev, shape, name):
     return t
 
 
-def _ptr(t):
-    return t.data_ptr() if t is not None else None
-
-
 def poisson_blend_batch(trg, gx, gy, hole, gmask=None, edge=None, device=None, return_info=False,
                         atol=1e-6, btol=1e-6, conlim=1e8, max_iters=MAX_ITERS, use_graph=True):
     """trg [F,H,W,3], gx [F,H,W-1,3], gy [F,H-1,W,3] (forward differences of the source), hole [F,H,W],
@@ -72,43 +68,33 @@ def poisson_blend_batch(trg, gx, gy, hole, gmask=None, edge=None, device=None, r
     plist = torch.zeros(F, H * W, dtype=torch.int32, device=dev)    # uint32 entries: pixel | code << 24, 0 = none
     cnt = torch.zeros(F, dtype=torch.int32, device=dev)
     kctr = torch.zeros(2, dtype=torch.int32, device=dev)             # device-side iteration index (csrc/poisson.cu)
-    L = lib.load()
-    sp = lib.stream_ptr
-    lib.check(L.fgt_poisson_setup(trg.data_ptr(), gx.data_ptr(), gy.data_ptr(), hole.data_ptr(), _ptr(gmask), _ptr(edge),
-                                  F, H, W, code.data_ptr(), u.data_ptr(), bb.data_ptr(), plist.data_ptr(), cnt.data_ptr(),
-                                  sp()), "fgt_poisson_setup")
+    lib.call("fgt_poisson_setup", trg, gx, gy, hole, gmask, edge, F, H, W, code, u, bb, plist, cnt)
     clr = torch.empty(2, F, H, W, dtype=torch.uint8, device=dev)
-    lib.check(L.fgt_poisson_unfilled(hole.data_ptr(), _ptr(gmask), F, H, W, clr.data_ptr(), sp()), "fgt_poisson_unfilled")
-    lib.COUNTERS["launches"] += 2
+    lib.call("fgt_poisson_unfilled", hole, gmask, F, H, W, clr)
     max_cnt = int(cnt.max())                           # pixels owning equations, largest frame (one host sync)
-    iter_args = (plist.data_ptr(), max_cnt, F, H, W, u.data_ptr(), v.data_ptr(), w.data_ptr(), x.data_ptr(),
-                 bb.data_ptr(), aa.data_ptr(), ww.data_ptr(), state.data_ptr(), kctr.data_ptr(), CHUNK, atol, btol,
-                 conlim, iter_lim)
+    iter_args = (plist, max_cnt, F, H, W, u, v, w, x, bb, aa, ww, state, kctr, CHUNK, atol, btol, conlim, iter_lim)
     exec_ = ctypes.c_void_p()
     if use_graph:
-        lib.check(L.fgt_poisson_graph_create(*iter_args, ctypes.byref(exec_)), "fgt_poisson_graph_create")
+        lib.call("fgt_poisson_graph_create", *iter_args, ctypes.byref(exec_))
     k = 0
     try:
         while True:
             if k > min(max_iters, iter_lim) + CHUNK:   # cannot happen with max_iters = iter_lim (istop = 7 by then)
                 raise RuntimeError(f"poisson: LSQR did not stop within {max_iters} iterations")
             if use_graph:
-                lib.check(L.fgt_poisson_graph_launch(exec_, sp()), "fgt_poisson_graph_launch")
+                lib.call("fgt_poisson_graph_launch", exec_, kernels=2 * CHUNK)
             else:
-                lib.check(L.fgt_poisson_iters(*iter_args, sp()), "fgt_poisson_iters")
-            lib.COUNTERS["launches"] += 2 * CHUNK
+                lib.call("fgt_poisson_iters", *iter_args, kernels=2 * CHUNK)
             k += CHUNK
             last = state[(k - 1) & 1]                     # written by iteration k-1
             if bool((last[:, 12] != 0).all()):             # one host sync per CHUNK iterations
                 break
     finally:
         if exec_:
-            L.fgt_poisson_graph_destroy(exec_)
+            lib.call("fgt_poisson_graph_destroy", exec_)
     out = torch.empty_like(trg)
     unf = torch.empty(F, H, W, dtype=torch.uint8, device=dev)
-    lib.check(L.fgt_poisson_finish(trg.data_ptr(), hole.data_ptr(), x.data_ptr(), F, H, W, out.data_ptr(),
-                                   clr.data_ptr(), unf.data_ptr(), sp()), "fgt_poisson_finish")
-    lib.COUNTERS["launches"] += 1
+    lib.call("fgt_poisson_finish", trg, hole, x, F, H, W, out, clr, unf)
     unf = unf.bool()
     if return_info:
         return out, unf, last[:, 13].to(torch.int64).view(F, C), last[:, 14].to(torch.int64).view(F, C)
@@ -143,8 +129,5 @@ def getUnfilledMask(holeMask, gradientMask):
     gm = _mask(np.asarray(gradientMask)[None], dev, tuple(hole.shape), "gradientMask")
     _, H, W = hole.shape
     clr = torch.empty(2, 1, H, W, dtype=torch.uint8, device=dev)
-    L = lib.load()
-    lib.check(L.fgt_poisson_unfilled(hole.data_ptr(), gm.data_ptr(), 1, H, W, clr.data_ptr(), lib.stream_ptr()),
-              "fgt_poisson_unfilled")
-    lib.COUNTERS["launches"] += 1
+    lib.call("fgt_poisson_unfilled", hole, gm, 1, H, W, clr)
     return ((hole != 0) & (clr[0] == 0) & (clr[1] == 0))[0].cpu().numpy()

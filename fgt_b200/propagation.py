@@ -12,21 +12,15 @@ import torch
 from . import lib
 
 
-def _check(rc, what):
-    lib.check(rc, what)
-
-
 def get_flowNN_gradient(args, gradient_x, gradient_y, mask_RGB, mask, videoFlowF, videoFlowB,
                         videoNonLocalFlowF=None, videoNonLocalFlowB=None, device="cuda:0"):
     if getattr(args, "Nonlocal", False):
         raise ValueError("fgt_b200 implements Nonlocal=False (the driver's setting, video_inpainting.py:796)")
     if not torch.cuda.is_available():
         raise RuntimeError("fgt_b200 get_flowNN_gradient needs a CUDA (sm_90a) device; there is no CPU fallback")
-    L = lib.load()
     dev = torch.device(device)
     H, W, N = mask.shape
     thres, alpha = float(args.consistencyThres), float(args.alpha)
-    st = lib.stream_ptr
     m = torch.from_numpy(np.ascontiguousarray(mask.astype(np.uint8).transpose(2, 0, 1))).to(dev)  # [N,H,W]
     ff = torch.from_numpy(np.ascontiguousarray(videoFlowF.astype(np.float32).transpose(3, 0, 1, 2))).to(dev)
     fb = torch.from_numpy(np.ascontiguousarray(videoFlowB.astype(np.float32).transpose(3, 0, 1, 2))).to(dev)
@@ -39,28 +33,25 @@ def get_flowNN_gradient(args, gradient_x, gradient_y, mask_RGB, mask, videoFlowF
                           nt=torch.full((N, H, W), -1, dtype=torch.int32, device=dev),
                           have=torch.zeros(N, H, W, dtype=torch.uint8, device=dev),
                           cuv=torch.zeros(N, H, W, 2, dtype=torch.float64, device=dev)))
-    p = lambda t: t.data_ptr()  # noqa: E731
     # pass 1: backward-flow neighbours, frames 1..N-1; pass 2: forward-flow neighbours, frames N-2..0
     for t in range(1, N):
         s0 = state[0]
-        _check(L.fgt_prop_step(p(m), p(fb[t - 1]), p(ff[t - 1]), H, W, t, t - 1, thres, p(s0["ny"]), p(s0["nx"]),
-                               p(s0["nt"]), p(s0["have"]), p(s0["cuv"]), st()), "fgt_prop_step")
+        lib.call("fgt_prop_step", m, fb[t - 1], ff[t - 1], H, W, t, t - 1, thres, s0["ny"], s0["nx"], s0["nt"], s0["have"],
+                 s0["cuv"])
     for t in range(N - 2, -1, -1):
         s1 = state[1]
-        _check(L.fgt_prop_step(p(m), p(ff[t]), p(fb[t]), H, W, t, t + 1, thres, p(s1["ny"]), p(s1["nx"]),
-                               p(s1["nt"]), p(s1["have"]), p(s1["cuv"]), st()), "fgt_prop_step")
+        lib.call("fgt_prop_step", m, ff[t], fb[t], H, W, t, t + 1, thres, s1["ny"], s1["nx"], s1["nt"], s1["have"],
+                 s1["cuv"])
     cand = []
     for slot, order in ((0, range(N)), (1, range(N - 1, -1, -1))):
         gx, gy = gx0.clone(), gy0.clone()
         s_ = state[slot]
         for s in order:
-            _check(L.fgt_prop_gather(p(m), p(s_["ny"]), p(s_["nx"]), p(s_["nt"]), N, H, W, s, p(gx), p(gy), st()),
-                   "fgt_prop_gather")
+            lib.call("fgt_prop_gather", m, s_["ny"], s_["nx"], s_["nt"], N, H, W, s, gx, gy)
         cand.append((gx, gy))
     tofill = torch.empty(N, H, W, dtype=torch.uint8, device=dev)
-    _check(L.fgt_prop_fuse(p(m), p(state[0]["have"]), p(state[1]["have"]), p(state[0]["cuv"]), p(state[1]["cuv"]), N, H,
-                           W, alpha, p(cand[0][0]), p(cand[0][1]), p(cand[1][0]), p(cand[1][1]), p(gx0), p(gy0),
-                           p(tofill), st()), "fgt_prop_fuse")
+    lib.call("fgt_prop_fuse", m, state[0]["have"], state[1]["have"], state[0]["cuv"], state[1]["cuv"], N, H, W, alpha,
+             cand[0][0], cand[0][1], cand[1][0], cand[1][1], gx0, gy0, tofill)
     out_x = gx0.permute(1, 2, 3, 0).cpu().numpy()
     out_y = gy0.permute(1, 2, 3, 0).cpu().numpy()
     # the reference fuses into its inputs in place and returns them (get_flowNN_gradient.py:517-534)

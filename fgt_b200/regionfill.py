@@ -30,29 +30,22 @@ def regionfill_batch(images, masks, tol=1e-12, device=None, return_iters=False, 
     if bool(full.any()):
         raise ValueError("regionfill: a mask covers its whole image (singular system; the reference fails too)")
     x, r, p0, p1, ap = (torch.empty_like(img) for _ in range(5))
-    L = lib.load()
-    sp = lib.stream_ptr
     # per-iteration scalars <r,r> and <p,Ap> of every image: one slot per iteration, never reset (csrc/laplace.cu)
     rr = torch.zeros((max_iters + 1) * B, dtype=torch.float64, device=dev)
     pap = torch.zeros(max_iters * B, dtype=torch.float64, device=dev)
-    lib.check(L.fgt_regionfill_init(img.data_ptr(), msk.data_ptr(), B, H, W, x.data_ptr(), r.data_ptr(), p0.data_ptr(),
-                                    rr.data_ptr(), sp()), "fgt_regionfill_init")
+    lib.call("fgt_regionfill_init", img, msk, B, H, W, x, r, p0, rr)
     rr0 = rr[:B].clone()
     k = 0
     while k < max_iters:
         n = min(CHUNK, max_iters - k)
-        lib.check(L.fgt_regionfill_iters(msk.data_ptr(), B, H, W, x.data_ptr(), r.data_ptr(), p0.data_ptr(),
-                                         p1.data_ptr(), ap.data_ptr(), rr.data_ptr(), pap.data_ptr(), k, n, sp()),
-                  "fgt_regionfill_iters")
-        lib.COUNTERS["launches"] += 2 * n - 1
+        lib.call("fgt_regionfill_iters", msk, B, H, W, x, r, p0, p1, ap, rr, pap, k, n, kernels=2 * n)
         k += n
         if bool((rr[k * B:(k + 1) * B] <= (tol * tol) * rr0).all()):   # one host sync per CHUNK iterations
             break
     else:
         raise RuntimeError(f"regionfill: CG did not reach relative residual {tol:g} in {max_iters} iterations")
     out = torch.empty_like(img)
-    lib.check(L.fgt_regionfill_finish(img.data_ptr(), msk.data_ptr(), img.numel(), x.data_ptr(), out.data_ptr(), sp()),
-              "fgt_regionfill_finish")
+    lib.call("fgt_regionfill_finish", img, msk, img.numel(), x, out)
     return (out, k) if return_iters else out
 
 

@@ -49,28 +49,9 @@ from fgt_b200 import lib
 from tests.gemm_emulator import GemmEmulator, _act, _GemmEntry, _r16, _Refused
 from tests.test_launch_trace import recording
 
-NAMES = {
-    "fgt_im2col_nchw": "src0 c0 src1 c1 n H W k stride pad replicate OH OW cpad scale shift out_hi out_plane",
-    "fgt_rownorm": "a ca lda b cb ldb gather rows_per_batch total_rows dst_batch_rows dst_row0 gamma beta out_hi "
-                   "out_plane eps",
-    "fgt_attention": "desc",
-    "fgt_fold_unfold": "hid bt th tw C kh kw stride pad OH OW relu out_hi out_plane",
-    "fgt_fold": "hid bt th tw C kh kw stride pad OH OW normalize add out out_hi out_plane",
-    "fgt_dwconv3x3_res": "x bt h w C weight bias out out_hi out_plane",
-    "fgt_swin_prep": "x fp d df bt h w win_map nl R gd gh gw gk_w gk_b gv_w gv_b qkn_hi qkn_plane vn_hi vn_plane eps",
-    "fgt_conv_tail": "x_hi x_plane n H W cin w_hi w_plane k_pad cout bias act out os_n os_c os_y os_x",
-    "fgt_upsample2x": "in_hi in_plane n H W C out_hi out_plane",
-    "fgt_chan_stats": "x n HW C stats",
-    "fgt_instnorm_act": "x stats n HW C eps relu res out out_hi out_plane",
-    "fgt_avgpool2": "src rows h w out",
-    "fgt_corr_lookup": "level_ptrs level_h level_w levels radius coords n_pix out_pitch out_hi out_plane",
-    "fgt_raft_flow_update": "coords delta delta_f16 n h w flow_nchw x_hi x_plane x_pitch x_chan",
-    "fgt_tapsum": "y n H W cout kx ky pad_x pad_y ycol bias act out os_n os_y os_x os_c",
-    "fgt_convex_upsample": "mask flow n h w out",
-    "fgt_f16_to_split": "src n out_hi out_plane",
-}
-NAMES = {k: v.split() + ["stream"] for k, v in NAMES.items()}
-ENTRIES = tuple(NAMES)
+ENTRIES = ("fgt_im2col_nchw", "fgt_rownorm", "fgt_attention", "fgt_fold_unfold", "fgt_fold", "fgt_dwconv3x3_res",
+           "fgt_swin_prep", "fgt_conv_tail", "fgt_upsample2x", "fgt_chan_stats", "fgt_instnorm_act", "fgt_avgpool2",
+           "fgt_corr_lookup", "fgt_raft_flow_update", "fgt_tapsum", "fgt_convex_upsample", "fgt_f16_to_split")
 
 
 def _k16(p, plane):
@@ -144,7 +125,7 @@ class _KernelEntry:
 
     def __call__(self, *args):
         assert self.argtypes is not None and len(args) == len(self.argtypes), self.name
-        a = {k: _raw(v, t) for k, v, t in zip(NAMES[self.name], args, self.argtypes)}
+        a = {k: _raw(v, t) for k, v, t in zip(lib.PROTOS[self.name].names, args, self.argtypes)}
         self.emu.forms.add((self.name, form(self.name, a)))
         getattr(self.emu, "_" + self.name[4:])(a)
         return 0
@@ -170,7 +151,7 @@ class KernelEmulator(GemmEmulator):
             raise AttributeError(name)
         if name == "fgt_gemm_tc":
             e = _GemmEntry(self)
-        elif name in NAMES:
+        elif name in ENTRIES:
             e = _KernelEntry(self, name)
         else:
             e = _Refused(name)
@@ -502,7 +483,7 @@ class KernelEmulator(GemmEmulator):
 
     def _avgpool2(self, a):
         rows, h, w = a["rows"], a["h"], a["w"]
-        x = self.f32(a["src"], rows * h * w).view(rows, h, w)[:, :h // 2 * 2, :w // 2 * 2]
+        x = self.f32(a["in"], rows * h * w).view(rows, h, w)[:, :h // 2 * 2, :w // 2 * 2]
         v = x.reshape(rows, h // 2, 2, w // 2, 2).sum((2, 4)) * 0.25
         self.st32(a["out"], torch.arange(v.numel()), v)
 
@@ -514,8 +495,8 @@ class KernelEmulator(GemmEmulator):
         p = torch.arange(n_pix)
         out = torch.empty(n_pix, L, win, win, dtype=torch.float64)
         for l in range(L):
-            hl, wl = a["level_h"][l], a["level_w"][l]
-            vol = self.f32(a["level_ptrs"][l], n_pix * hl * wl)
+            hl, wl = a["level_h_host"][l], a["level_w_host"][l]
+            vol = self.f32(a["level_ptrs_host"][l], n_pix * hl * wl)
             c = (co / 2.0 ** l).clamp(-1e6, 1e6)
             X = c[:, 0:1] + dd            # [p, a]: window index a offsets x
             Y = c[:, 1:2] + dd            # [p, b]: window index b offsets y
@@ -554,7 +535,7 @@ class KernelEmulator(GemmEmulator):
     def _convex_upsample(self, a):
         n, h, w = a["n"], a["h"], a["w"]
         m = torch.softmax(self.f32(a["mask"], n * h * w * 576).view(n, h, w, 9, 8, 8), 3)
-        fp = F.pad(self.f32(a["flow"], n * 2 * h * w).view(n, 2, h, w), (1, 1, 1, 1))
+        fp = F.pad(self.f32(a["flow_nchw"], n * 2 * h * w).view(n, 2, h, w), (1, 1, 1, 1))
         nb = torch.stack([8.0 * fp[:, :, k // 3:k // 3 + h, k % 3:k % 3 + w] for k in range(9)], -1)   # [n,2,h,w,9]
         up = torch.einsum("nyxkij,ncyxk->ncyixj", m, nb).reshape(n, 2, 8 * h, 8 * w)
         self.st32(a["out"], torch.arange(up.numel()), up)

@@ -130,7 +130,7 @@ def test_hidden_permutation_matches_fold():
     assert torch.allclose(img, ref, atol=1e-5)
 
 
-def test_c_abi_rejects_bad_arguments_without_touching_the_gpu():
+def test_c_abi_and_lib_call_reject_bad_arguments_without_touching_the_gpu(monkeypatch):
     """Error behaviour of the boundary (SURVEY 8b): a negative FGT_ERR_* code plus a thread-local message, checked
     before any CUDA call — so it can be exercised on a host without a device."""
     L = lib.load()
@@ -156,8 +156,9 @@ def test_c_abi_rejects_bad_arguments_without_touching_the_gpu():
         assert rc == -1, (fn.__name__, rc)          # FGT_ERR_ARG
         assert needle in L.fgt_last_error().decode(), (fn.__name__, L.fgt_last_error())
     assert L.fgt_poisson_graph_destroy(None) == 0   # destroying nothing is not an error
+    monkeypatch.setattr(lib, "stream_ptr", lambda: None)
     with pytest.raises(RuntimeError, match="fgt_plane_max"):
-        lib.check(L.fgt_plane_max(None, 1, 16, None, None), "fgt_plane_max")
+        lib.call("fgt_plane_max", None, 1, 16, None)
 
 
 # ------------------------------------------------------------------------------------------ round 2 host logic

@@ -31,7 +31,7 @@ import torch.nn.functional as F
 
 from fgt_b200 import lib, synth
 from oracle import raft_oracle as RO
-from tests.kernel_emulator import ENTRIES, NAMES, emulating_all, form
+from tests.kernel_emulator import ENTRIES, emulating_all, form
 from tests.test_launch_trace import GOLDEN
 from tests.util import load_golden, max_over_max, rel_l2
 
@@ -567,7 +567,7 @@ def _trace_forms():
     for case_name, calls in g.items():
         for name, args in calls:
             if name != "fgt_gemm_tc":
-                out.setdefault((name, form(name, dict(zip(NAMES[name], args)))), case_name)
+                out.setdefault((name, form(name, dict(zip(lib.PROTOS[name].names, args)))), case_name)
     return out
 
 

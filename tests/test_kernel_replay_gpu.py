@@ -56,7 +56,7 @@ import torch
 import torch.nn.functional as F
 
 from fgt_b200 import lib, synth
-from tests.kernel_emulator import ENTRIES, NAMES, KernelEmulator
+from tests.kernel_emulator import ENTRIES, KernelEmulator
 from tests.util import load_golden
 
 pytestmark = pytest.mark.gpu
@@ -176,8 +176,9 @@ class Replayer:
                 for s, f in _ptr_fields(a._obj):
                     if getattr(s, f):
                         out.append((s, f))
-            elif isinstance(a, ctypes.Array) and a._type_ is ctypes.c_void_p:
-                out += [(a, j) for j in range(len(a)) if a[j]]
+            elif isinstance(a, ctypes.Array):
+                if a._type_ is ctypes.c_void_p:
+                    out += [(a, j) for j in range(len(a)) if a[j]]
             elif t is ctypes.c_void_p and a is not None:
                 out.append((args, i))
         return out
@@ -232,7 +233,7 @@ class Replayer:
         for b, w in work.items():
             wb = emu.written_bytes(w)
             assert torch.equal(after[b][~wb], before[b][~wb]), f"{name}: bytes outside its outputs changed"
-        a = dict(zip(NAMES.get(name, ["desc", "stream"]), cargs))
+        a = dict(zip(lib.PROTOS[name].names, cargs))
         exact = name in EXACT_ENTRIES or (name == "fgt_im2col_nchw" and (a["scale"], a["shift"]) == (1.0, 0.0))
         inorm16 = name == "fgt_instnorm_act" and a["out_hi"] and a["out_plane"] == 0
         stored = {}
@@ -256,7 +257,7 @@ class Replayer:
             assert torch.isfinite(got).all(), f"{name}: non-finite output"
             scale = want.abs().max().item() + 1e-30
             if name == "fgt_avgpool2":
-                x = emu.f32(a["src"], a["rows"] * a["h"] * a["w"]).view(a["rows"], a["h"], a["w"]).abs()
+                x = emu.f32(a["in"], a["rows"] * a["h"] * a["w"]).view(a["rows"], a["h"], a["w"]).abs()
                 mag = F.avg_pool2d(x[:, None], 2, stride=2).reshape(-1)[idx]
                 err = ((got - want).abs() / (3 * 2.0 ** -24 * mag + 1e-38)).max().item()
             elif name == "fgt_gemm_tc":
@@ -367,8 +368,7 @@ PRODUCTION = {
 }
 
 
-@pytest.mark.parametrize("case", sorted(TRACE_CASES))
-def test_replay_trace_cases_every_launch(case):
+def _replay_trace_case(case):
     run = TRACE_CASES[case]()
     with torch.no_grad():
         run()                       # packs the weights and allocates the workspaces outside the replay
@@ -378,8 +378,7 @@ def test_replay_trace_cases_every_launch(case):
     assert sum(r.launches.values()) > 0
 
 
-@pytest.mark.parametrize("case", sorted(PRODUCTION))
-def test_replay_production_non_gemm_launches(case):
+def _replay_production_case(case):
     run = PRODUCTION[case]()
     with torch.no_grad():
         run()
@@ -387,6 +386,28 @@ def test_replay_production_non_gemm_launches(case):
             run()
     r.report(case)
     assert sum(r.launches.values()) > 0
+
+
+@pytest.mark.parametrize("case", sorted(c for c in TRACE_CASES if not c.startswith("raft")))
+def test_replay_trace_cases_every_launch(case):
+    _replay_trace_case(case)
+
+
+@pytest.mark.parametrize("case", sorted(c for c in PRODUCTION if not c.startswith("raft")))
+def test_replay_production_non_gemm_launches(case):
+    _replay_production_case(case)
+
+
+# RAFT's forwards pass fgt_corr_lookup's per-level host tables (device pointers, heights, widths): the replay resolves
+# the pointer table element by element and passes the int tables through as they are.
+@pytest.mark.parametrize("case", sorted(c for c in TRACE_CASES if c.startswith("raft")))
+def test_replay_raft_trace_cases_with_host_level_tables(case):
+    _replay_trace_case(case)
+
+
+@pytest.mark.parametrize("case", sorted(c for c in PRODUCTION if c.startswith("raft")))
+def test_replay_raft_production_non_gemm_launches_with_host_level_tables(case):
+    _replay_production_case(case)
 
 
 # ------------------------------------------------------------------------------------------------------- edge cases
@@ -408,9 +429,10 @@ def test_f16_to_split_every_pattern():
     assert torch.isnan(o[0, nan]).all() and torch.isnan(o[1, nan]).all()
 
 
-def test_corr_lookup_edges_fp16_and_split():
+def test_corr_lookup_edges_with_host_level_tables():
     """Lookup centres on integers, at w - 1 / h - 1, one pixel and half a pixel outside and beyond the +-1e6 clamp, into
-    fp16 and split-bf16 rows of pitch 384 (columns 324-383 untouched), including a 1 x 1 coarsest level."""
+    fp16 and split-bf16 rows of pitch 384 (columns 324-383 untouched), including a 1 x 1 coarsest level. The levels'
+    pointers, heights and widths reach the entry as host tables."""
     from tests.test_kernel_emulator import _edge_coords, _pyramid
     for h, w in ((16, 24), (8, 12)):
         pyr = [t.to(DEV) for t in _pyramid(h, w, 42)]

@@ -108,7 +108,7 @@ def test_rgb_watermark_masks():
     _same(comp, frames, m[2], 3)                                         # one colour mask for every frame
 
 
-def test_argument_errors_surface_the_library_text():
+def test_argument_errors_surface_the_library_text_through_lib_call():
     g = np.random.default_rng(6)
     comp, frames = _inputs(g, 2, 60, 80, 30, 40)
     masks = np.zeros((2, 60, 80), np.uint8)
@@ -120,22 +120,17 @@ def test_argument_errors_surface_the_library_text():
     with pytest.raises(ValueError):
         native.composite_native(comp, frames, np.zeros((2, 60, 81), np.uint8), 0)
     dev = torch.device("cuda:0")
-    L = lib.load()
     c, f = torch.from_numpy(comp).to(dev), torch.from_numpy(frames).to(dev)
-    ws = torch.zeros(int(L.fgt_native_workspace(2, 60, 80, 2)), dtype=torch.uint8, device=dev)
+    ws = torch.zeros(lib.call("fgt_native_workspace", 2, 60, 80, 2), dtype=torch.uint8, device=dev)
     out = torch.empty_like(f)
     with pytest.raises(RuntimeError, match="not the working size"):            # counts built for k = 3, comp gives k = 2
-        lib.check(L.fgt_native_composite(c.data_ptr(), 2, 30, 40, f.data_ptr(), 60, 80, 3, 0, 3, ws.data_ptr(), ws.numel(),
-                                         out.data_ptr(), lib.stream_ptr()), "fgt_native_composite")
+        lib.call("fgt_native_composite", c, 2, 30, 40, f, 60, 80, 3, 0, 3, ws, ws.numel(), out)
     with pytest.raises(RuntimeError, match="workspace of"):
-        lib.check(L.fgt_native_count(f.data_ptr(), 2, 60, 80, 2, ws.data_ptr(), ws.numel() - 1, lib.stream_ptr()),
-                  "fgt_native_count")
+        lib.call("fgt_native_count", f, 2, 60, 80, 2, ws, ws.numel() - 1)
     with pytest.raises(RuntimeError, match="empty size"):
-        lib.check(L.fgt_native_composite(c.data_ptr(), 0, 30, 40, f.data_ptr(), 60, 80, 3, 0, 2, ws.data_ptr(), ws.numel(),
-                                         out.data_ptr(), lib.stream_ptr()), "fgt_native_composite")
+        lib.call("fgt_native_composite", c, 0, 30, 40, f, 60, 80, 3, 0, 2, ws, ws.numel(), out)
     with pytest.raises(RuntimeError, match="alias"):
-        lib.check(L.fgt_native_composite(c.data_ptr(), 2, 30, 40, f.data_ptr(), 60, 80, 3, 0, 2, ws.data_ptr(), ws.numel(),
-                                         f.data_ptr(), lib.stream_ptr()), "fgt_native_composite")
+        lib.call("fgt_native_composite", c, 2, 30, 40, f, 60, 80, 3, 0, 2, ws, ws.numel(), f)
 
 
 def _backend(H, W):
