@@ -64,6 +64,7 @@ struct GemmParams {
   int act;
   float alpha;
   int out_half;  // the 16-bit output is ONE plane of fp16 (input of a 1-term layer) instead of split-bf16
+  int r16;       // FGT_OUT_HALF_AUTOCAST: every fp16 tensor of the layer under autocast is rounded (kExt = 1 or 2)
 };
 
 // Epilogue parameters hoisted into registers once per CTA.
@@ -74,7 +75,7 @@ struct EpiArgs {
   const float* aux2;
   long long out_plane, os_c;
   float alpha;
-  int act, aux_mode, vec_ok, aux_vec, N, out_half;
+  int act, aux_mode, vec_ok, aux_vec, N, out_half, r16;
 };
 
 __device__ __forceinline__ float act_one(float v, int act) {
@@ -106,7 +107,8 @@ __device__ __forceinline__ void load_pair(const float* src, long long o0, long l
 
 // Output channels (col, col + 1) of one output row at element offset `off`: bias + alpha * acc, activation, aux
 // operand, stores. `two`: col + 1 < N. kExt = 1 adds the rarely used modes (pre-activation add, add+ReLU, GRU
-// updates, slope-0.01 LeakyReLU); keeping them out of the common instantiation keeps its register count down.
+// updates, slope-0.01 LeakyReLU); keeping them out of the common instantiation keeps its register count down. kExt = 2
+// (FGT_OUT_HALF_AUTOCAST without those modes) has the activations and the r16 rounding only.
 template <int kExt>
 __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, long long off, int col, bool two) {
   const bool vec = e.vec_ok && two;  // vec_ok implies a unit channel stride and even element offsets
@@ -114,18 +116,26 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
   const long long o1 = o0 + e.os_c;
   const bool avec = vec && e.aux_vec;
   float a0 = 0.f, a1 = 0.f;
-  if (kExt && e.aux_mode == FGT_AUX_ADD_PRE) {  // residual added BEFORE the activation (LAFC edge head)
+  if (kExt && e.r16) {  // autocast (LAFC): the conv's output is an fp16 tensor, also before a pre-activation add
+    v0 = round_f16(v0);
+    v1 = round_f16(v1);
+  }
+  if (kExt == 1 && e.aux_mode == FGT_AUX_ADD_PRE) {  // residual added BEFORE the activation (LAFC edge head)
     load_pair(e.aux, o0, o1, two, avec, a0, a1);
     v0 += a0;
     v1 += a1;
   }
-  if (kExt && e.out_half) {  // mixed precision: the conv's output is an fp16 tensor before its activation (autocast)
+  if (kExt && (e.out_half || e.r16)) {  // mixed precision: the conv's output is an fp16 tensor before its activation (autocast)
     v0 = round_f16(v0);
     v1 = round_f16(v1);
   }
   if (kExt) {
     v0 = act_one(v0, e.act);
     v1 = act_one(v1, e.act);
+    if (e.r16) {  // autocast (LAFC): the activation's output is an fp16 tensor before the residual add
+      v0 = round_f16(v0);
+      v1 = round_f16(v1);
+    }
   } else if (e.act == FGT_ACT_LEAKY02) {
     v0 = v0 > 0.f ? v0 : 0.2f * v0;
     v1 = v1 > 0.f ? v1 : 0.2f * v1;
@@ -133,12 +143,12 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
     v0 = act_one(v0, e.act);
     v1 = act_one(v1, e.act);
   }
-  if (kExt && e.out_half && (e.aux_mode == FGT_AUX_GRU_ZR || e.aux_mode == FGT_AUX_GRU)) {
+  if (kExt == 1 && e.out_half && (e.aux_mode == FGT_AUX_GRU_ZR || e.aux_mode == FGT_AUX_GRU)) {
     // mixed-precision GRU (update.py:45-60 under autocast): the gates z, r and the candidate q are fp16
     v0 = round_f16(v0);
     v1 = round_f16(v1);
   }
-  if (kExt && e.aux_mode == FGT_AUX_GRU_ZR) {  // fused z | r gates: two C-channel outputs (host guarantees vec)
+  if (kExt == 1 && e.aux_mode == FGT_AUX_GRU_ZR) {  // fused z | r gates: two C-channel outputs (host guarantees vec)
     const int half = e.N >> 1;
     if (col < half) {
       *reinterpret_cast<float2*>(e.out_f32 + o0) = make_float2(v0, v1);
@@ -164,7 +174,7 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
     load_pair(e.aux, o0, o1, two, avec, a0, a1);
     v0 *= a0;
     v1 *= a1;
-  } else if (kExt && e.aux_mode == FGT_AUX_ADD_RELU) {
+  } else if (kExt == 1 && e.aux_mode == FGT_AUX_ADD_RELU) {
     load_pair(e.aux, o0, o1, two, avec, a0, a1);
     if (e.out_half) {  // mixed precision: act(v) is an fp16 tensor before the residual add (RAFT/extractor.py:55-56)
       v0 = round_f16(v0);
@@ -172,7 +182,7 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
     }
     v0 = fmaxf(v0 + a0, 0.f);
     v1 = fmaxf(v1 + a1, 0.f);
-  } else if (kExt && e.aux_mode == FGT_AUX_GRU) {  // h' = (1 - z) * h + z * q   (aux = h, aux2 = z, v = q)
+  } else if (kExt == 1 && e.aux_mode == FGT_AUX_GRU) {  // h' = (1 - z) * h + z * q   (aux = h, aux2 = z, v = q)
     float z0, z1;
     load_pair(e.aux, o0, o1, two, avec, a0, a1);
     load_pair(e.aux2, o0, o1, two, avec, z0, z1);
@@ -184,7 +194,7 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
       v1 = (1.f - z1) * a1 + z1 * v1;
     }
   }
-  if (kExt && e.out_half) {  // the fp32 copy (a residual or GRU-state operand) holds the same fp16 value as the 16-bit output
+  if (kExt && (e.out_half || e.r16)) {  // the fp32 copy (a residual or GRU-state operand) holds the same fp16 value as the 16-bit output
     v0 = round_f16(v0);
     v1 = round_f16(v1);
   }
@@ -218,7 +228,7 @@ __device__ __forceinline__ void epi_pair(const EpiArgs& e, float v0, float v1, l
   }
 }
 
-// ---- Batched epilogue (kExt = 0, whole tile inside N, unit channel stride, 16-byte aligned rows: `vec4_ok`).
+// ---- Batched epilogue (kExt = 0 or 2, whole tile inside N, unit channel stride, 16-byte aligned rows: `vec4_ok`).
 // The operands that do not depend on the accumulators (bias, aux) are loaded for a chunk of JC column groups j at once,
 // before the accumulators are final, so the tile waits for global memory once per chunk instead of once per column
 // pair. The quad of threads (qc = 0..3) that holds rows (r, r + 8) x channels [8 j, 8 j + 8) swaps pairs with
@@ -259,7 +269,9 @@ __device__ __forceinline__ float epi_act(float v, int act) {
   return v;
 }
 
-template <int kAct, int JC, int R>
+// kR16: FGT_OUT_HALF_AUTOCAST (the kExt = 2 instantiation): the rounding points of epi_pair's r16 mode, for the modes
+// the batched epilogue runs (activation, FGT_AUX_ADD / MUL).
+template <int kAct, bool kR16, int JC, int R>
 __device__ __forceinline__ void epi_chunk(const EpiArgs& e, const float (&acc)[R], const EpiPre<JC>& pre, int j0,
                                           int n0, int qc, long long off, bool valid) {
   const bool odd = qc & 1;
@@ -279,11 +291,15 @@ __device__ __forceinline__ void epi_chunk(const EpiArgs& e, const float (&acc)[R
     x[2] = odd ? v10 : r0;
     x[3] = odd ? v11 : r1;
 #pragma unroll
-    for (int q = 0; q < 4; ++q) x[q] = epi_act<kAct>(x[q], e.act);
+    for (int q = 0; q < 4; ++q) x[q] = kR16 ? round_f16(epi_act<kAct>(round_f16(x[q]), e.act)) : epi_act<kAct>(x[q], e.act);
     if (e.aux_mode == FGT_AUX_ADD) {
       x[0] += pre.a[jj].x; x[1] += pre.a[jj].y; x[2] += pre.a[jj].z; x[3] += pre.a[jj].w;
     } else if (e.aux_mode == FGT_AUX_MUL) {
       x[0] *= pre.a[jj].x; x[1] *= pre.a[jj].y; x[2] *= pre.a[jj].z; x[3] *= pre.a[jj].w;
+    }
+    if (kR16) {  // the fp32 copy holds the fp16 value of the 16-bit output
+#pragma unroll
+      for (int q = 0; q < 4; ++q) x[q] = round_f16(x[q]);
     }
     if (!valid) continue;
     const long long o = ob + j * 8;
@@ -388,6 +404,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
     ep.out_f32 = p.out_f32; ep.out_hi = p.out_hi; ep.aux = p.aux; ep.aux2 = p.aux2; ep.out_plane = p.out_plane; ep.os_c = p.os_c;
     ep.alpha = p.alpha; ep.act = p.act; ep.aux_mode = p.aux_mode; ep.vec_ok = p.vec_ok; ep.aux_vec = p.aux_vec; ep.N = p.N;
     ep.out_half = p.out_half;
+    ep.r16 = p.r16;
     const int qc = lane & 3;
     int stage = 0;
     uint32_t phase = 0;
@@ -489,7 +506,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       }
       // The batched epilogue stores row (qc & 1) of the quad's two rows. Its first load batch goes out while the tile's
       // last MMA group runs.
-      const bool batched = kExt == 0 && !kSerial && p.vec4_ok && n0 + BN <= p.N;
+      const bool batched = kExt != 1 && !kSerial && p.vec4_ok && n0 + BN <= p.N;
       const long long off_q = (qc & 1) ? off[1] : off[0];
       const bool valid_q = (qc & 1) ? valid[1] : valid[0];
       // column groups per load batch, as registers allow: 4 at BN = 64 next to two accumulator arrays, half the tile
@@ -525,9 +542,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
         for (int j0 = 0; j0 < BN / 8; j0 += JC) {
           if (j0 > 0) epi_prefetch<JC>(pre, ep, p.bias, j0, n0, qc, off_q, valid_q);
-          if (act_kind == 0) epi_chunk<0>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
-          else if (act_kind == 1) epi_chunk<1>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
-          else epi_chunk<2>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
+          if (act_kind == 0) epi_chunk<0, kExt == 2>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
+          else if (act_kind == 1) epi_chunk<1, kExt == 2>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
+          else epi_chunk<2, kExt == 2>(ep, cur, pre, j0, n0, qc, off_q, valid_q);
         }
       } else {
 #pragma unroll
@@ -737,8 +754,12 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
 
   // ---- numerics: 3-term split-bf16 (default) or single-plane fp16 operands (1 MMA per K step)
   const int planes = one_term ? 1 : 2;
-  p.out_half = d.out_half ? 1 : 0;
-  FGT_REQUIRE(!p.out_half || d.out_hi, FGT_ERR_ARG, "gemm_tc: out_half without a 16-bit output");
+  FGT_REQUIRE(d.out_half >= 0 && d.out_half <= FGT_OUT_HALF_AUTOCAST, FGT_ERR_ARG, "gemm_tc: out_half=%d", d.out_half);
+  FGT_REQUIRE(d.out_half != 1 || d.out_hi, FGT_ERR_ARG, "gemm_tc: out_half without a 16-bit output");
+  FGT_REQUIRE(d.out_half != FGT_OUT_HALF_AUTOCAST || one_term, FGT_ERR_ARG,
+              "gemm_tc: FGT_OUT_HALF_AUTOCAST needs a 1-term (fp16) layer");
+  p.out_half = (d.out_half && d.out_hi) ? 1 : 0;
+  p.r16 = d.out_half == FGT_OUT_HALF_AUTOCAST ? 1 : 0;
 
   const uint32_t stage_bytes = static_cast<uint32_t>(planes) * (kAPlaneBytes + static_cast<uint32_t>(bn) * 128u);
   const uint32_t fixed = 1024u /*align*/ + 256u /*barriers*/;
@@ -749,9 +770,13 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(stages) * stage_bytes + fixed;
 
   // out_half with an fp32 copy (mixed-precision RAFT): the fp16 rounding before the activation and of the fp32 copy lives
-  // in the kExt = 1 epilogue, so the common instantiation keeps the previous code
-  const bool ext = d.aux_mode == FGT_AUX_ADD_PRE || d.aux_mode == FGT_AUX_ADD_RELU || d.aux_mode == FGT_AUX_GRU ||
-                   d.aux_mode == FGT_AUX_GRU_ZR || d.act == FGT_ACT_LEAKY001 || (d.out_half && d.out_f32);
+  // in the kExt = 1 epilogue, so the common instantiation keeps the previous code. FGT_OUT_HALF_AUTOCAST (mixed-precision
+  // LAFC) has an instantiation of its own, kExt = 2: the batched epilogue with its rounding points, and epi_pair's r16
+  // mode where the batched one does not apply; the modes only kExt = 1 has take kExt = 1.
+  const bool ext_modes = d.aux_mode == FGT_AUX_ADD_PRE || d.aux_mode == FGT_AUX_ADD_RELU || d.aux_mode == FGT_AUX_GRU ||
+                         d.aux_mode == FGT_AUX_GRU_ZR || d.act == FGT_ACT_LEAKY001;
+  const bool ext = ext_modes || (d.out_half && d.out_f32 && !p.r16) || (p.r16 && g_gemm_serial);
+  const bool r16_batched = p.r16 && !ext;
   if (d.aux_mode == FGT_AUX_GRU_ZR)
     FGT_REQUIRE(d.out_f32 && d.out_hi && p.vec_ok && d.N % 64 == 0 && (d.N / 2) % d.bn == 0 && d.groups == 1, FGT_ERR_ARG,
                 "gemm_tc: FGT_AUX_GRU_ZR needs both outputs, aligned unit-stride channels, N=%d a multiple of 64 and "
@@ -759,7 +784,9 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   void* kern = g_gemm_serial
                    ? (one_term ? (ext ? gemm_kernel_for<true, 1, true>(bn) : gemm_kernel_for<true, 0, true>(bn))
                                : (ext ? gemm_kernel_for<false, 1, true>(bn) : gemm_kernel_for<false, 0, true>(bn)))
-                   : (one_term ? (ext ? gemm_kernel_for<true, 1, false>(bn) : gemm_kernel_for<true, 0, false>(bn))
+                   : (one_term ? (ext           ? gemm_kernel_for<true, 1, false>(bn)
+                                  : r16_batched ? gemm_kernel_for<true, 2, false>(bn)
+                                                : gemm_kernel_for<true, 0, false>(bn))
                                : (ext ? gemm_kernel_for<false, 1, false>(bn) : gemm_kernel_for<false, 0, false>(bn)));
   FGT_REQUIRE(kern, FGT_ERR_ARG, "gemm_tc: no instantiation for a %d-wide tile", bn);
   // raised once per instantiation: the attribute is per kernel

@@ -509,13 +509,15 @@ __global__ void fold_unfold_kernel(const float* __restrict__ hid, int bt, int th
   }
 }
 
-// nearest x2 upsampling of an NHWC split tensor (F.interpolate(scale_factor=2), network_blocks_2d.py:58-60)
+// nearest x2 upsampling of an NHWC split tensor (F.interpolate(scale_factor=2), network_blocks_2d.py:58-60); with both
+// plane offsets 0, of a single-plane fp16 tensor (mixed-precision LAFC). A bit copy of 8 16-bit elements per thread.
 __global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ in, long long in_plane, int n, int H, int W,
                                   int C, __nv_bfloat16* __restrict__ out, long long out_plane) {
   pdl_launch_dependents();
   pdl_wait();
   const int C8 = C / 8;
-  const long long total = 2LL * n * (2 * H) * (2 * W) * C8;
+  const int planes = in_plane == 0 ? 1 : 2;
+  const long long total = planes * static_cast<long long>(n) * (2 * H) * (2 * W) * C8;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(i % C8) * 8;
@@ -742,7 +744,9 @@ extern "C" int fgt_fold_unfold(const float* hid, int bt, int th, int tw, int C, 
 extern "C" int fgt_upsample2x(const void* in_hi, long long in_plane, int n, int H, int W, int C, void* out_hi,
                               long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(in_hi && out_hi && C % 8 == 0, FGT_ERR_ARG, "upsample2x: C=%d", C);
-  const long long total = 2LL * n * (2 * H) * (2 * W) * (C / 8);
+  FGT_REQUIRE((in_plane == 0) == (out_plane == 0) && in_plane >= 0 && out_plane >= 0, FGT_ERR_ARG,
+              "upsample2x: plane offsets %lld -> %lld (both 0: fp16, both > 0: split-bf16)", in_plane, out_plane);
+  const long long total = (in_plane == 0 ? 1LL : 2LL) * n * (2 * H) * (2 * W) * (C / 8);
   launch_k(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
       reinterpret_cast<const __nv_bfloat16*>(in_hi), in_plane, n, H, W, C, reinterpret_cast<__nv_bfloat16*>(out_hi),
       out_plane);

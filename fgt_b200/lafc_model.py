@@ -6,6 +6,10 @@ Drop-in for /root/reference/LAFC/models/lafc.py: `Model(config).forward(flows, m
 convolution runs on the wgmma implicit-GEMM engine (P3D (1,k,k) convs as per-frame 2-D taps,
 (3,1,1) temporal convs as z-taps with TMA zero fill, dilated convs as tap offsets, skip concats as
 K-segments), the input gather and nearest upsampling on HBM-bound helper kernels. No CPU fallback.
+
+Opt-in mixed precision (`P3DNet.enable_mixed_precision()`): the reference module under
+torch.autocast("cuda", dtype=torch.float16), with every conv a 1-term fp16 GEMM (oracle/lafc_mixed_oracle.py is the
+definition; DESIGN.md section 2 the rounding points).
 """
 import torch
 import torch.nn as nn
@@ -58,6 +62,7 @@ class P3DNet(NativeNet):
             raise ValueError("fgt_b200 LAFC expects flows(2)+mask(1) input channels")
         c = num_feats
         self.c, self.T, self.use_residual, self.resNums = c, num_flows, use_residual, res_blocks
+        self._mixed = False
         self.encoder2 = nn.Sequential(nn.ReplicationPad3d((2, 2, 2, 2, 0, 0)), _P3D(in_channels, c, 5), _P3D(c, 2 * c, 3))
         self.encoder4 = nn.Sequential(_P3D(2 * c, 2 * c, 3), _P3D(2 * c, 4 * c, 3))
         base = _P3D(4 * c, 4 * c, 3)
@@ -75,16 +80,22 @@ class P3DNet(NativeNet):
                     nn.init.kaiming_normal_(m.weight.data, a=0, mode='fan_in')
                     nn.init.constant_(m.bias.data, 0.0)
 
-    def _pack(self, dev):
+    def _pack(self, dev, half=False):
+        """half: the mixed-precision set, every conv a 1-term fp16 layer whose weight and bias are rounded to fp16 once
+        (autocast's casts of the conv's parameters)."""
         sd = {k: v.detach().float() for k, v in self.state_dict().items()}
+        if half:
+            sd = {k: v.half().float() for k, v in sd.items()}
         c = self.c
         P = {}
 
         def put(name, key, segs=None, im2col=None):
-            P[name] = ops.packed(name, sd[key + ".featureConv.weight"], sd[key + ".featureConv.bias"], dev, segs, im2col)
+            P[name] = ops.packed(name, sd[key + ".featureConv.weight"], sd[key + ".featureConv.bias"], dev, segs, im2col,
+                                 half=half)
 
         w = sd["encoder2.1.conv1.featureConv.weight"]  # [c,3,1,5,5] -> 2-D filter for the im2col path
-        P["e2a1"] = ops.packed("e2a1", w[:, :, 0], sd["encoder2.1.conv1.featureConv.bias"], dev, im2col_pad=128)
+        P["e2a1"] = ops.packed("e2a1", w[:, :, 0], sd["encoder2.1.conv1.featureConv.bias"], dev, im2col_pad=128,
+                               half=half)
         put("e2a2", "encoder2.1.conv2")
         put("e2b1", "encoder2.2.conv1")
         put("e2b2", "encoder2.2.conv2")
@@ -110,58 +121,62 @@ class P3DNet(NativeNet):
         put("edge_1", "edgeDetector.mid_layer_1")
         put("edge_2", "edgeDetector.mid_layer_2")
         put("edge_o", "edgeDetector.out_layer")
-        self._packed[False] = P
+        self._packed[half] = P
         return P
 
-    def _forward_one(self, x, P, dev):
-        """x: [T, 3, H, W] fp32 (flows + mask per candidate frame) -> (flow [2,H,W], edge [1,H,W])."""
+    def _forward_one(self, x, P, dev, mixed=False):
+        """x: [T, 3, H, W] fp32 (flows + mask per candidate frame) -> (flow [2,H,W], edge [1,H,W]). mixed: fp16
+        activation buffers, fp16 packed weights P, and every GEMM rounds where autocast makes an fp16 tensor."""
         T, _, H, W = x.shape
         c = self.c
         H2, W2, H4, W4 = H // 2, W // 2, H // 4, W // 4
-        bufs = self._geo.setdefault((T, H, W), {})
-        B = lambda n, s, split=True: workspace(bufs, n, s, dev, torch.bfloat16 if split else torch.float32)  # noqa: E731
+        bufs = self._geo.setdefault((T, H, W, mixed), {})
+        a16 = torch.float16 if mixed else torch.bfloat16  # 16-bit activations: fp16 (mixed) or split-bf16
+        B = lambda n, s, split=True: workspace(bufs, n, s, dev, a16 if split else torch.float32)  # noqa: E731
+        conv = (lambda *a, **k: ops.conv(*a, autocast=True, **k)) if mixed else ops.conv  # noqa: E731
+        linear = (lambda *a, **k: ops.linear(*a, autocast=True, **k)) if mixed else ops.linear  # noqa: E731
         L = lib.ACT_LEAKY02
         # encoder2 (lafc.py:23-30): ReplicationPad + (1,5,5) conv via im2col, then the (3,1,1) conv
         col = B("col", (T, H, W, 128))
         lib.im2col_nchw(x, None, col, k=5, stride=1, pad=2, replicate=True, OH=H, OW=W, tag="e2a1")
         a1 = B("a1", (T, H, W, c))
-        ops.linear([(col.view(2, T * H * W, 128), 128)], P["e2a1"], T * H * W, act=L, out_split=a1)
+        linear([(lib.view16(col, T * H * W, 128), 128)], P["e2a1"], T * H * W, act=L, out_split=a1)
         a2 = B("a2", (T, H, W, c))
-        ops.conv([(a1, c)], P["e2a2"], kz=3, pad_z=1, out_split=a2)
+        conv([(a1, c)], P["e2a2"], kz=3, pad_z=1, out_split=a2)
         a3 = B("a3", (T, H2, W2, 2 * c))
-        ops.conv([(a2, c)], P["e2b1"], kx=3, ky=3, stride=2, pad_x=1, pad_y=1, out_split=a3)
+        conv([(a2, c)], P["e2b1"], kx=3, ky=3, stride=2, pad_x=1, pad_y=1, out_split=a3)
         e2 = B("e2", (T, H2, W2, 2 * c))
         e2f = B("e2f", (T, H2, W2, 2 * c), split=False)
-        ops.conv([(a3, 2 * c)], P["e2b2"], kz=3, pad_z=1, out_split=e2, out_f32=e2f)
+        conv([(a3, 2 * c)], P["e2b2"], kz=3, pad_z=1, out_split=e2, out_f32=e2f)
         ce2 = B("ce2", (1, H2, W2, 2 * c))
-        ops.conv([(e2, 2 * c)], P["cond2"], kz=T, pad_z=0, out_z=1, out_split=ce2)
+        conv([(e2, 2 * c)], P["cond2"], kz=T, pad_z=0, out_z=1, out_split=ce2)
         # encoder4 (lafc.py:31-36)
         t1 = B("t1", (T, H2, W2, 2 * c))
-        ops.conv([(e2, 2 * c)], P["e4a1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=t1)
+        conv([(e2, 2 * c)], P["e4a1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=t1)
         e4a = B("e4a", (T, H2, W2, 2 * c))
         if self.use_residual:
-            ops.conv([(t1, 2 * c)], P["e4a2"], kz=3, pad_z=1, out_split=e4a, aux=e2f, aux_mode=lib.AUX_ADD)
+            conv([(t1, 2 * c)], P["e4a2"], kz=3, pad_z=1, out_split=e4a, aux=e2f, aux_mode=lib.AUX_ADD)
         else:
-            ops.conv([(t1, 2 * c)], P["e4a2"], kz=3, pad_z=1, out_split=e4a)
+            conv([(t1, 2 * c)], P["e4a2"], kz=3, pad_z=1, out_split=e4a)
         t2 = B("t2", (T, H4, W4, 4 * c))
-        ops.conv([(e4a, 2 * c)], P["e4b1"], kx=3, ky=3, stride=2, pad_x=1, pad_y=1, out_split=t2)
+        conv([(e4a, 2 * c)], P["e4b1"], kx=3, ky=3, stride=2, pad_x=1, pad_y=1, out_split=t2)
         e4 = B("e4", (T, H4, W4, 4 * c))
         e4f = B("e4f", (T, H4, W4, 4 * c), split=False)
-        ops.conv([(t2, 4 * c)], P["e4b2"], kz=3, pad_z=1, out_split=e4, out_f32=e4f)
+        conv([(t2, 4 * c)], P["e4b2"], kz=3, pad_z=1, out_split=e4, out_f32=e4f)
         ce4 = B("ce4", (1, H4, W4, 4 * c))
-        ops.conv([(e4, 4 * c)], P["cond4pre"], kz=T, pad_z=0, out_z=1, out_split=ce4)
+        conv([(e4, 4 * c)], P["cond4pre"], kz=T, pad_z=0, out_z=1, out_split=ce4)
         # residual blocks: one shared block applied resNums times (lafc.py:38-43,94-95)
         t3 = B("t3", (T, H4, W4, 4 * c))
         for _ in range(self.resNums):
-            ops.conv([(e4, 4 * c)], P["res1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=t3)
-            ops.conv([(t3, 4 * c)], P["res2"], kz=3, pad_z=1, out_split=e4, out_f32=e4f, aux=e4f, aux_mode=lib.AUX_ADD)
+            conv([(e4, 4 * c)], P["res1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=t3)
+            conv([(t3, 4 * c)], P["res2"], kz=3, pad_z=1, out_split=e4, out_f32=e4f, aux=e4f, aux_mode=lib.AUX_ADD)
         y0 = B("y0", (1, H4, W4, 4 * c))
         y1 = B("y1", (1, H4, W4, 4 * c))
-        ops.conv([(e4, 4 * c)], P["cond4post"], kz=T, pad_z=0, out_z=1, out_split=y0)
+        conv([(e4, 4 * c)], P["cond4post"], kz=T, pad_z=0, out_z=1, out_split=y0)
         # dilated middle (lafc.py:54-63)
         src, dst = y0, y1
         for i, d in enumerate((8, 4, 2, 1)):
-            ops.conv([(src, 4 * c)], P[f"mid{i}"], kx=3, ky=3, dil=d, pad_x=d, pad_y=d, out_split=dst)
+            conv([(src, 4 * c)], P[f"mid{i}"], kx=3, ky=3, dil=d, pad_x=d, pad_y=d, out_split=dst)
             src, dst = dst, src
         # decoder2 (lafc.py:64-71): nearest x2 of [filled ; pre] then conv
         u1 = B("u1", (1, H2, W2, 4 * c))
@@ -170,10 +185,10 @@ class P3DNet(NativeNet):
         lib.upsample2x(ce4, 1, H4, W4, 4 * c, u2)
         d20 = B("d20", (1, H2, W2, 2 * c))
         d21 = B("d21", (1, H2, W2, 2 * c))
-        ops.conv([(u1, 4 * c), (u2, 4 * c)], P["dec2_0"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d20,
-                 seg_counts=[4 * c, 4 * c])
-        ops.conv([(d20, 2 * c)], P["dec2_1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d21)
-        ops.conv([(d21, 2 * c)], P["dec2_2"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d20)
+        conv([(u1, 4 * c), (u2, 4 * c)], P["dec2_0"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d20,
+             seg_counts=[4 * c, 4 * c])
+        conv([(d20, 2 * c)], P["dec2_1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d21)
+        conv([(d21, 2 * c)], P["dec2_2"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d20)
         # decoder (lafc.py:72-79)
         u3 = B("u3", (1, H, W, 2 * c))
         u4 = B("u4", (1, H, W, 2 * c))
@@ -181,43 +196,55 @@ class P3DNet(NativeNet):
         lib.upsample2x(ce2, 1, H2, W2, 2 * c, u4)
         d0 = B("d0", (1, H, W, c))
         d1 = B("d1", (1, H, W, c // 2))
-        ops.conv([(u3, 2 * c), (u4, 2 * c)], P["dec_0"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d0,
-                 seg_counts=[2 * c, 2 * c])
-        ops.conv([(d0, c)], P["dec_1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d1)
+        conv([(u3, 2 * c), (u4, 2 * c)], P["dec_0"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d0,
+             seg_counts=[2 * c, 2 * c])
+        conv([(d0, c)], P["dec_1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=d1)
         flow = torch.empty(1, 2, H, W, device=dev, dtype=torch.float32)
-        ops.conv([(d1, c // 2)], P["dec_2"], kx=3, ky=3, pad_x=1, pad_y=1, act=lib.ACT_NONE, out_f32=flow, nchw_out=True)
+        conv([(d1, c // 2)], P["dec_2"], kx=3, ky=3, pad_x=1, pad_y=1, act=lib.ACT_NONE, out_f32=flow, nchw_out=True)
         # edge head (lafc.py:141-148)
         ecol = B("ecol", (1, H, W, 64))
         lib.im2col_nchw(flow, None, ecol, k=3, stride=1, pad=1, replicate=False, OH=H, OW=W, tag="edge_p")
         ep = B("ep", (1, H, W, 16))
         epf = B("epf", (1, H, W, 16), split=False)
-        ops.linear([(ecol.view(2, H * W, 64), 64)], P["edge_p"], H * W, act=L, out_split=ep, out_f32=epf)
+        linear([(lib.view16(ecol, H * W, 64), 64)], P["edge_p"], H * W, act=L, out_split=ep, out_f32=epf)
         e1 = B("e1", (1, H, W, 16))
         e2_ = B("e2_", (1, H, W, 16))
-        ops.conv([(ep, 16)], P["edge_1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=e1)
-        ops.conv([(e1, 16)], P["edge_2"], kx=3, ky=3, pad_x=1, pad_y=1, act=lib.ACT_LEAKY001, aux=epf,
-                 aux_mode=lib.AUX_ADD_PRE, out_split=e2_)
+        conv([(ep, 16)], P["edge_1"], kx=3, ky=3, pad_x=1, pad_y=1, out_split=e1)
+        conv([(e1, 16)], P["edge_2"], kx=3, ky=3, pad_x=1, pad_y=1, act=lib.ACT_LEAKY001, aux=epf,
+             aux_mode=lib.AUX_ADD_PRE, out_split=e2_)
         edge = torch.empty(1, 1, H, W, device=dev, dtype=torch.float32)
-        ops.conv([(e2_, 16)], P["edge_o"], act=lib.ACT_SIGMOID, out_f32=edge, nchw_out=True)
+        conv([(e2_, 16)], P["edge_o"], act=lib.ACT_SIGMOID, out_f32=edge, nchw_out=True)
         return flow, edge
+
+    def enable_mixed_precision(self, on=True):
+        """Mixed precision, opt-in: the network runs as the reference does under
+        torch.autocast("cuda", dtype=torch.float16). Every conv is a 1-term fp16 tensor-core GEMM (fp16 weights, biases
+        and activation rows, fp32 accumulation) that rounds to fp16 wherever autocast makes an fp16 tensor. Autocast's
+        outputs are fp16; these stay fp32 tensors holding the fp16-rounded values, so callers keep their dtypes. The
+        fp16 weights, workspaces and CUDA graphs are kept apart from the fp32 path's, so the flag may change between
+        calls; off (the default) gives the fp32 path's outputs bit for bit. DESIGN.md section 2 lists where the
+        rounding points differ from autocast."""
+        self._mixed = bool(on)
 
     def forward(self, flows, masks, edges=None):
         if edges is not None:
             raise ValueError("fgt_b200 LAFC: the `edges` input is unused by the shipped driver (always None)")
         if not flows.is_cuda:
             raise RuntimeError("fgt_b200 LAFC runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+        mixed = self._mixed
         if self._graphs is not None:
-            return self._graphed((), self._forward_impl, flows.float().contiguous(), masks.float().contiguous())
-        return self._forward_impl(flows, masks)
+            fn = (lambda *a: self._forward_impl(*a, mixed=True)) if mixed else self._forward_impl
+            return self._graphed((True,) if mixed else (), fn, flows.float().contiguous(), masks.float().contiguous())
+        return self._forward_impl(flows, masks, mixed=mixed)
 
-    def _forward_impl(self, flows, masks):
+    def _forward_impl(self, flows, masks, mixed=False):
         b, _, T, H, W = flows.shape
         if T != self.T or H % 4 or W % 4:
             raise ValueError(f"LAFC input [T={T},{H}x{W}]: T must be {self.T} and H, W divisible by 4")
         dev = flows.device
-        P = self._packed.get(False) or self._pack(dev)
+        P = self._packed.get(mixed) or self._pack(dev, mixed)
         x = torch.cat([flows.float(), masks.float()], 1).permute(0, 2, 1, 3, 4).contiguous()  # [b,T,3,H,W]
-        outs = [self._forward_one(x[i], P, dev) for i in range(b)]
+        outs = [self._forward_one(x[i], P, dev, mixed) for i in range(b)]
         return torch.cat([o[0] for o in outs], 0), torch.cat([o[1] for o in outs], 0)
 
 

@@ -222,13 +222,16 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
             out_w, out_h=1, out_z=1, box_w=128, box_h=1, bn=128, bias=None, alpha=1.0, act=ACT_NONE,
             aux=None, aux_mode=AUX_NONE, out_f32=None, out_split=None, out_elem_offset=0,
             os_z=0, os_y=0, os_x=None, os_c=1, rowmap=None, lin_batch=0, aux2=None, terms=None, out_f16=None,
-            alg_k=None, tag=""):
+            alg_k=None, autocast=False, tag=""):
     """Generic launcher for fgt_gemm_tc. Output strides are in elements; see include/fgt_b200.h.
     The weight's dtype selects the MMA form: a split-bf16 weight takes split-bf16 A segments (3 terms), an fp16 weight
     plain fp16 ones (1 term). out_split, the optional 16-bit output, is split-bf16 or plain fp16. Optional checks of
-    the caller's expectation: terms, the MMA form; out_f16, a 16-bit output that must be fp16."""
+    the caller's expectation: terms, the MMA form; out_f16, a 16-bit output that must be fp16. autocast (fp16 weights
+    only): round at every point where the layer under torch.autocast makes an fp16 tensor (FGT_OUT_HALF_AUTOCAST), so
+    that every output, out_f32 included, holds fp16 values."""
     f16 = w_split.dtype == torch.float16
     assert terms is None or terms == (1 if f16 else 3), "terms=1 takes fp16 weights, terms=3 split-bf16 ones"
+    assert not autocast or f16, "autocast rounding takes fp16 weights"
     if out_f16 is not None:
         assert out_split is None and out_f16.dtype == torch.float16
         out_split = out_f16
@@ -264,6 +267,9 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
         d.out_hi = out_split.data_ptr() + 2 * out_elem_offset
         d.out_plane = _plane16(out_split)
         d.out_half = 1 if out_split.dtype == torch.float16 else 0
+        assert not autocast or d.out_half, "autocast rounding: the 16-bit output is fp16"
+    if autocast:
+        d.out_half = OUT_HALF_AUTOCAST
     d.os_z, d.os_y, d.os_c = os_z, os_y, os_c
     d.os_x = N if os_x is None else os_x
     d.rowmap = rowmap.data_ptr() if rowmap is not None else None
@@ -423,8 +429,9 @@ def fold_unfold(hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu
 
 
 def upsample2x(in_split, n, H, W, C, out_split, tag=""):
-    with _Prof("upsample2x", tag, 0, 4.0 * n * H * W * C * 5):
-        call("fgt_upsample2x", in_split, plane_elems(in_split), n, H, W, C, out_split, plane_elems(out_split))
+    """Nearest x2 of NHWC [n, H, W, C]: split-bf16 in and out, or plain fp16 in and out."""
+    with _Prof("upsample2x", tag, 0, (2.5 if in_split.dtype == torch.float16 else 5.0) * n * H * W * C * 4):
+        call("fgt_upsample2x", in_split, _plane16(in_split), n, H, W, C, out_split, _plane16(out_split))
 
 
 # ------------------------------------------------------------------------------------------ RAFT helpers

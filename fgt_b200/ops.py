@@ -63,11 +63,12 @@ def packed(name, weight, bias, dev, seg_counts=None, im2col_pad=None, half=False
 
 def conv(xs, wp, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad_y=0, pad_z=0, out_z=None, act=lib.ACT_LEAKY02,
          out_split=None, out_f32=None, aux=None, aux_mode=lib.AUX_NONE, groups=1, seg_counts=None, nchw_out=False,
-         alpha=1.0, aux2=None, out_c_total=None, out_c_offset=0, out_phase=None, tile=conv_tile, bn=None, alg_k=None):
+         alpha=1.0, aux2=None, out_c_total=None, out_c_offset=0, out_phase=None, tile=conv_tile, bn=None, alg_k=None,
+         autocast=False):
     """xs: list of (split tensor [2, Z, Y, X, C], C) sharing Z/Y/X, or of fp16 tensors [Z, Y, X, C] for a layer with
     fp16 weights. Output NHWC [Z', Y', X', N] (or NCHW fp32 when nchw_out). out_phase=(py, px): the output is one
     phase of a 2x upsampled map, pixel (y, x) stored at (2y+py, 2x+px) of [Z, 2Y, 2X, N]. The channel tile is `bn`,
-    or the caller's policy `tile`. Returns (oz, oy, ox)."""
+    or the caller's policy `tile`. autocast: lib.gemm_tc's autocast rounding (fp16 weights only). Returns (oz, oy, ox)."""
     x0, c0 = xs[0]
     Z, Y, X = x0.shape[-4], x0.shape[-3], x0.shape[-2]
     if out_phase is None:
@@ -94,7 +95,7 @@ def conv(xs, wp, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad_y=0, pad_z=0
                 groups=groups, out_w=ox, out_h=oy, out_z=oz, box_w=bw, box_h=bh,
                 bn=tile(N, groups, ox * oy * oz) if bn is None else bn,
                 bias=wp["b"], alpha=alpha, act=act, aux=aux, aux_mode=aux_mode, aux2=aux2, out_f32=out_f32, out_split=out_split,
-                tag=wp["name"], alg_k=alg_k, **strides)
+                tag=wp["name"], alg_k=alg_k, autocast=autocast, **strides)
     return oz, oy, ox
 
 

@@ -578,11 +578,13 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
 
 
 # ------------------------------------------------------------------------------------------------ command line
-def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False, fgt_mixed_precision=False):
+def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False, fgt_mixed_precision=False,
+                lafc_mixed_precision=False):
     """initialize_RAFT / initialize_LAFC / initialize_FGT (:186-230) with the drop-in modules: the same checkpoint
     layout (a `module.`-prefixed RAFT state dict; directories holding one *.tar with `model_state_dict` and one
     *.yaml config). mixed_precision: RAFT's fp16 mode (the reference's --mixed_precision, RAFT only).
-    fgt_mixed_precision: the FGT generator's fp16 mode (FGT.enable_mixed_precision). Returns
+    fgt_mixed_precision: the FGT generator's fp16 mode (FGT.enable_mixed_precision). lafc_mixed_precision: the LAFC
+    flow-completion network's fp16 mode (P3DNet.enable_mixed_precision). The three are independent. Returns
     (GpuBackend, lafc_config)."""
     import glob
     import os
@@ -607,6 +609,7 @@ def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False
     lafc_sd, lafc_cfg = ckpt_dir(lafc_ckpts)
     lafc = LAFCModel(lafc_cfg)
     lafc.load_state_dict(lafc_sd)
+    lafc.net.enable_mixed_precision(bool(lafc_mixed_precision))
     fgt_sd, fgt_cfg = ckpt_dir(fgt_ckpts)
     fgt = FGTModel(fgt_cfg)
     fgt.load_state_dict(fgt_sd)
@@ -634,6 +637,9 @@ def arg_parser():
     ap.add_argument("--fgt_mixed_precision", action="store_true",
                     help="run the FGT generator with fp16 tensor-core operands, as the reference under CUDA autocast "
                          "(faster, not fp32-accurate; independent of --mixed_precision)")
+    ap.add_argument("--lafc_mixed_precision", action="store_true",
+                    help="run the LAFC flow-completion network with fp16 tensor-core operands, as the reference under "
+                         "CUDA autocast (faster, not fp32-accurate; independent of the other two switches)")
     for k, v in DEFAULTS.items():
         if k == "mode":
             ap.add_argument("--mode", default=v, choices=list(MODES))
@@ -652,6 +658,8 @@ def main(argv=None):
         ap.error("--native: video_extrapolation has no original frame to paste the result into")
     dev = torch.device("cuda", ns.gpu)
     fgt_kw = dict(fgt_mixed_precision=True) if ns.fgt_mixed_precision else {}
+    if ns.lafc_mixed_precision:
+        fgt_kw["lafc_mixed_precision"] = True
     backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev, ns.mixed_precision, **fgt_kw)
     args = make_args(**{k: getattr(ns, k) for k in DEFAULTS if hasattr(ns, k)})
     frames = IO.read_frames(ns.path)

@@ -53,6 +53,7 @@ enum { FGT_ACT_NONE = 0, FGT_ACT_LEAKY02 = 1, FGT_ACT_RELU = 2, FGT_ACT_SIGMOID 
  *      stores r*h as fp16, and GRU rounds each of (1 - z), (1 - z) * h, z * q and their sum to fp16. */
 enum { FGT_AUX_NONE = 0, FGT_AUX_ADD = 1, FGT_AUX_MUL = 2, FGT_AUX_ADD_PRE = 3, FGT_AUX_ADD_RELU = 4,
        FGT_AUX_GRU = 5, FGT_AUX_GRU_ZR = 6 };
+enum { FGT_OUT_HALF_AUTOCAST = 2 /* FgtGemmDesc.out_half: autocast's rounding points, see there */ };
 
 int fgt_version(void);
 const char* fgt_last_error(void);
@@ -115,7 +116,11 @@ typedef struct {
                                 plane offsets are ignored), one MMA per K step — for layers whose error budget allows */
   int out_half;              /* 1: out_hi receives ONE plane of fp16 (the input format of a terms == 1 layer). With
                                 out_f32 as well (mixed-precision RAFT, autocast semantics), the value is rounded to
-                                fp16 before the activation and again after it, and out_f32 receives that fp16 value */
+                                fp16 before the activation and again after it, and out_f32 receives that fp16 value.
+                                FGT_OUT_HALF_AUTOCAST (terms == 1 only; out_hi optional): every tensor the layer makes
+                                under autocast is fp16 (mixed-precision LAFC) — the conv output is rounded before a
+                                pre-activation add and the activation, the activation's output before FGT_AUX_ADD, and
+                                the result; out_f32 alone (an fp32-only output) then also holds fp16 values */
 } FgtGemmDesc;
 
 int fgt_gemm_tc(const FgtGemmDesc* desc, fgt_stream_t stream);
