@@ -439,6 +439,41 @@ def pipeline_clip(seed=5, N=7, H=64, W=96):
 
 
 # ----------------------------------------------------------------------------------------------
+# clip scoring (fgt_b200/metrics.py)
+# ----------------------------------------------------------------------------------------------
+def _box(x, r):
+    """Integer box sum of half-width r along axes 1 and 2 of an int64 [N,H,W,C] array (valid part only)."""
+    import numpy as np
+    for ax in (1, 2):
+        c = np.cumsum(np.pad(x, [(1, 0) if a == ax else (0, 0) for a in range(4)]), axis=ax)
+        n = x.shape[ax] - 2 * r
+        x = np.take(c, range(2 * r + 1, 2 * r + 1 + n), axis=ax) - np.take(c, range(n), axis=ax)
+    return x
+
+
+def metric_pair(seed, N, H, W, C, kind, dtype):
+    """(results, gts) [N,H,W,C] numpy arrays of `dtype` ('u8' or 'f32') on the 0..255 scale for scoring
+    (fgt_b200/metrics.py): a smooth integer texture as the ground truth, and as the result the ground truth plus
+    quarter-level noise (kind "noise"), its 3x3 box blur ("blur") or the ground truth itself ("same"). Integer
+    arithmetic and exact float64 divisions only, so every machine regenerates the arrays bit for bit."""
+    import numpy as np
+    g = np.random.default_rng(seed)
+    tex = _box(g.integers(0, 256, (N, H + 10, W + 10, C)), 4)[:, 1:-1, 1:-1]       # [N, H, W, C] box sums of 81
+    lo, hi = tex.min(), tex.max()
+    gt = (tex - lo) * 255 // max(hi - lo, 1)
+    if kind == "noise":
+        res = gt + g.integers(-48, 49, gt.shape) / 4.0
+    elif kind == "blur":
+        res = _box(np.pad(gt, [(0, 0), (1, 1), (1, 1), (0, 0)], mode="edge"), 1) / 9.0
+    else:
+        res = gt.astype(np.float64)
+    res = np.clip(res, 0, 255)
+    if dtype == "u8":
+        return np.floor(res + 0.5).astype(np.uint8), gt.astype(np.uint8)
+    return res.astype(np.float32), gt.astype(np.float32)
+
+
+# ----------------------------------------------------------------------------------------------
 # forward flow splatting (LAFC/models/utils/flow_warp.py)
 # ----------------------------------------------------------------------------------------------
 def flow_warp_inputs(seed=0, b=2, c=5, h=20, w=28):

@@ -410,6 +410,27 @@ int fgt_native_composite(const unsigned char* comp, int B, int cH, int cW, const
                          int C, int shared_mask, int k, const void* workspace, long long workspace_bytes,
                          unsigned char* out, fgt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Quality metrics of N result frames against N ground-truth frames, both [N,H,W,C] with C = 1 or 3 and values on the
+ * 0..255 scale, as the reference defines them (FGT/metrics/psnr.py, ssim.py and the L1 / L2 errors of
+ * FGT/metrics/__init__.py calculate_metrics); every input is converted to float64 first. a_dtype / b_dtype are
+ * FGT_METRIC_U8 or FGT_METRIC_F32. Per frame, with d = a - b over all H*W*C values:
+ *   l1 = mean|d|,  l2 = sqrt(sum d^2) / (H*W*C),  psnr = 100 if mean d^2 == 0 else 20 log10(255 / sqrt(mean d^2)),
+ *   ssim = the mean over channels of the MATLAB-style SSIM of each plane: 11x11 Gaussian window (sigma 1.5, cv2's
+ *          getGaussianKernel) at the (H-10) x (W-10) valid positions, C1 = (0.01*255)^2, C2 = (0.03*255)^2,
+ *          sigma^2 = w*(x^2) - mu^2 as written in ssim.py.
+ * H and W must be at least 11 (the reference returns NaN below), N * C at most 65535.
+ *   fgt_metrics_workspace  bytes of workspace for N frames of H x W x C (negative FGT_ERR_* on bad sizes).
+ *   fgt_metrics            out float64 [N][4] = (l1, l2, psnr, ssim); ssim_c float64 [N][C] = the per-channel SSIM
+ *                          (NULL: not written). Two kernels: per-(frame, channel, 32x32 tile) partial sums into the
+ *                          workspace, then a fixed-order reduction per frame, so each frame's values do not depend on
+ *                          N or on the other frames.
+ * ------------------------------------------------------------------------------------------ */
+enum { FGT_METRIC_U8 = 0, FGT_METRIC_F32 = 1 };
+long long fgt_metrics_workspace(int N, int H, int W, int C);
+int fgt_metrics(const void* a, int a_dtype, const void* b, int b_dtype, int N, int H, int W, int C, void* workspace,
+                long long workspace_bytes, double* out, double* ssim_c, fgt_stream_t stream);
+
 /* 3x3 convolution (zero padding 1, stride 1) with cout <= 3 output channels + bias + activation in one kernel: the
  * nine taps become the N dimension of a wgmma GEMM over the input positions (activation read once) and are summed
  * per output pixel in shared memory — the decoder's final conv + tanh (FGT/models/model.py:185-193). x: NHWC
