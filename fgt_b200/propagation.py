@@ -19,20 +19,38 @@ def get_flowNN_gradient(args, gradient_x, gradient_y, mask_RGB, mask, videoFlowF
     if not torch.cuda.is_available():
         raise RuntimeError("fgt_b200 get_flowNN_gradient needs a CUDA (sm_90a) device; there is no CPU fallback")
     dev = torch.device(device)
-    H, W, N = mask.shape
     thres, alpha = float(args.consistencyThres), float(args.alpha)
     m = torch.from_numpy(np.ascontiguousarray(mask.astype(np.uint8).transpose(2, 0, 1))).to(dev)  # [N,H,W]
     ff = torch.from_numpy(np.ascontiguousarray(videoFlowF.astype(np.float32).transpose(3, 0, 1, 2))).to(dev)
     fb = torch.from_numpy(np.ascontiguousarray(videoFlowB.astype(np.float32).transpose(3, 0, 1, 2))).to(dev)
     gx0 = torch.from_numpy(np.ascontiguousarray(gradient_x.astype(np.float32).transpose(3, 0, 1, 2))).to(dev)
     gy0 = torch.from_numpy(np.ascontiguousarray(gradient_y.astype(np.float32).transpose(3, 0, 1, 2))).to(dev)
-    state = []
-    for slot in (0, 1):
-        state.append(dict(ny=torch.zeros(N, H, W, dtype=torch.float64, device=dev),
-                          nx=torch.zeros(N, H, W, dtype=torch.float64, device=dev),
-                          nt=torch.full((N, H, W), -1, dtype=torch.int32, device=dev),
-                          have=torch.zeros(N, H, W, dtype=torch.uint8, device=dev),
-                          cuv=torch.zeros(N, H, W, 2, dtype=torch.float64, device=dev)))
+    tofill = propagate(m, ff, fb, gx0, gy0, thres, alpha)
+    out_x = gx0.permute(1, 2, 3, 0).cpu().numpy()
+    out_y = gy0.permute(1, 2, 3, 0).cpu().numpy()
+    # the reference fuses into its inputs in place and returns them (get_flowNN_gradient.py:517-534)
+    if isinstance(gradient_x, np.ndarray) and gradient_x.dtype == np.float32 and gradient_x.flags.writeable:
+        np.copyto(gradient_x, out_x)
+        np.copyto(gradient_y, out_y)
+        out_x, out_y = gradient_x, gradient_y
+    return out_x, out_y, tofill.permute(1, 2, 0).cpu().numpy().astype(bool)
+
+
+def slot_state(N, H, W, dev):
+    """One NN slot's dense state (include/fgt_b200.h), with no neighbour anywhere."""
+    return dict(ny=torch.zeros(N, H, W, dtype=torch.float64, device=dev),
+                nx=torch.zeros(N, H, W, dtype=torch.float64, device=dev),
+                nt=torch.full((N, H, W), -1, dtype=torch.int32, device=dev),
+                have=torch.zeros(N, H, W, dtype=torch.uint8, device=dev),
+                cuv=torch.zeros(N, H, W, 2, dtype=torch.float64, device=dev))
+
+
+def propagate(m, ff, fb, gx0, gy0, thres, alpha):
+    """The launch sequence on tensors in the kernels' layouts: mask m uint8 [N,H,W], flows [N-1,H,W,2], gradients
+    [N,H,W,3] (fused in place). Returns mask_tofill, uint8 [N,H,W]."""
+    N, H, W = m.shape
+    dev = m.device
+    state = [slot_state(N, H, W, dev) for _ in (0, 1)]
     # pass 1: backward-flow neighbours, frames 1..N-1; pass 2: forward-flow neighbours, frames N-2..0
     for t in range(1, N):
         s0 = state[0]
@@ -52,11 +70,4 @@ def get_flowNN_gradient(args, gradient_x, gradient_y, mask_RGB, mask, videoFlowF
     tofill = torch.empty(N, H, W, dtype=torch.uint8, device=dev)
     lib.call("fgt_prop_fuse", m, state[0]["have"], state[1]["have"], state[0]["cuv"], state[1]["cuv"], N, H, W, alpha,
              cand[0][0], cand[0][1], cand[1][0], cand[1][1], gx0, gy0, tofill)
-    out_x = gx0.permute(1, 2, 3, 0).cpu().numpy()
-    out_y = gy0.permute(1, 2, 3, 0).cpu().numpy()
-    # the reference fuses into its inputs in place and returns them (get_flowNN_gradient.py:517-534)
-    if isinstance(gradient_x, np.ndarray) and gradient_x.dtype == np.float32 and gradient_x.flags.writeable:
-        np.copyto(gradient_x, out_x)
-        np.copyto(gradient_y, out_y)
-        out_x, out_y = gradient_x, gradient_y
-    return out_x, out_y, tofill.permute(1, 2, 0).cpu().numpy().astype(bool)
+    return tofill

@@ -131,7 +131,10 @@ def _instnorm_f16_interval(emu, a, idx):
 class Replayer:
     """Stands in for the ctypes library: the entries in `entries` run on the GPU and are then replayed by the
     interpreter and compared; every other entry goes straight to the real library. `maxima[(entry, kind)]` holds the
-    largest error seen, in the unit of the entry's bar."""
+    largest error seen, in the unit of the entry's bar. Subclasses replay other entries by naming another interpreter in
+    `emulator` and overriding `_compare` (tests/test_prop_kernels_gpu.py)."""
+
+    emulator = KernelEmulator
 
     def __init__(self, real, entries, attn_budget=None, device_type="cuda"):
         self.real, self.entries, self.attn_budget = real, set(entries), attn_budget
@@ -218,7 +221,7 @@ class Replayer:
                 setattr(h[0], h[1], q)
             else:
                 h[0][h[1]] = q
-        emu = KernelEmulator()
+        emu = self.emulator()
         emu.attn_budget = self.attn_budget
         emu._storages = [[w.data_ptr(), w.data_ptr() + w.numel(), w] for w in work.values()]
         entry = getattr(emu, name)
@@ -228,11 +231,15 @@ class Replayer:
         self.launches[name] += 1
         return rc
 
-    def _compare(self, name, cargs, emu, before, after, work):
-        key = {w.untyped_storage().data_ptr(): b for b, w in work.items()}
+    @staticmethod
+    def _check_untouched(name, emu, before, after, work):
         for b, w in work.items():
             wb = emu.written_bytes(w)
             assert torch.equal(after[b][~wb], before[b][~wb]), f"{name}: bytes outside its outputs changed"
+
+    def _compare(self, name, cargs, emu, before, after, work):
+        key = {w.untyped_storage().data_ptr(): b for b, w in work.items()}
+        self._check_untouched(name, emu, before, after, work)
         a = dict(zip(lib.PROTOS[name].names, cargs))
         exact = name in EXACT_ENTRIES or (name == "fgt_im2col_nchw" and (a["scale"], a["shift"]) == (1.0, 0.0))
         inorm16 = name == "fgt_instnorm_act" and a["out_hi"] and a["out_plane"] == 0
