@@ -320,6 +320,12 @@ class GpuBackend:
         return morph.resize_bilinear(x, (H, W), channel_scale=(float(W) / float(w), float(H) / float(h)),
                                      device=self.dev).cpu().numpy()
 
+    def flow_images(self, flows, convert_to_bgr=False):
+        """flow_viz.flow_to_image of every flow in [n,H,W,2] float32 in one batched device call -> numpy uint8
+        [n,H,W,3] (fgt_b200/flowviz.py)."""
+        from . import flowviz
+        return flowviz.flow_to_image(np.ascontiguousarray(flows, dtype=np.float32), convert_to_bgr, device=self.dev)
+
     def _inpaint_telea(self, images, masks):
         """cv2.inpaint(..., 3, INPAINT_TELEA) of uint8 [B,H,W,3] with masks [B,H,W] or one [H,W] -> numpy uint8."""
         from . import inpaint
@@ -534,7 +540,7 @@ def composite_native(backend, comp, frames_u8, masks_u8, args):
 
 
 def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_interval=3, return_stages=False,
-                     native=False):
+                     native=False, vis_out=None):
     """The driver on arrays: frames_u8 [N,h,w,3] RGB uint8 (the PNGs the driver reads), masks_u8 [N,h,w] (non-zero =
     remove; ignored by video_extrapolation) -> list of N uint8 RGB frames (what the driver writes to result.mp4).
     `args`: make_args(...), `args.mode` one of object_removal (default), watermark_removal (frames are masked before
@@ -542,7 +548,12 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
     :516-537); num_flows / flow_interval are the LAFC config entries the driver reads (:352).
     native=True returns the frames at the input size h x w instead of imgH x imgW: the result is upscaled and pasted
     into the input frames around the mask by `backend.composite_native` (object and watermark removal; every frame and
-    mask of one size). With return_stages the working-resolution frames are then in stages["comp"]."""
+    mask of one size). With return_stages the working-resolution frames are then in stages["comp"].
+    vis_out: a dict that receives what the driver's visualisation switches write (write_visualisations): "flow_f" /
+    "flow_b", the RAFT flows at imgH x imgW before video_extrapolation places them on its canvas (--vis_flows);
+    "done_f" / "done_b", the completed flows (--vis_completed_flows); "prop_frames", the list of BGR frames after
+    propagation, each with its own dtype (float64 where the Poisson blend ran, float32 elsewhere), and "masks_left",
+    the [H,W,N] mask of what propagation could not fill (--vis_prop)."""
     args = args or make_args()
     if args.mode not in MODES:
         raise ValueError(f"Accepted modes: {MODES}, but input is {args.mode}")
@@ -551,6 +562,8 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
     video, video_flow = load_clip(frames_u8, args, masks_u8 if args.mode == "watermark_removal" else None)
     flow_f = compute_flows(backend, video_flow, args, "forward")
     flow_b = compute_flows(backend, video_flow, args, "backward")
+    if vis_out is not None:
+        vis_out.update(flow_f=flow_f, flow_b=flow_b)
     # [H,W,3(BGR),N] in 0..1 (:499-501), stored frame-major so that every per-frame view is contiguous
     video = np.moveaxis(np.ascontiguousarray(video.permute(0, 2, 3, 1).numpy()[..., ::-1]) / 255.0, 0, -1)
     assert video.dtype == np.float32
@@ -566,6 +579,8 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
     gx, gy = prepare_gradients(video, mask, mask_dilated, backend)
     gx, gy, mask_gradient = backend.propagate(args, gx, gy, mask, mask_dilated, done_f, done_b)
     frame_blends = blend_frames(backend, video, gx, gy, mask, np.array(mask_gradient, dtype=bool))
+    if vis_out is not None:
+        vis_out.update(done_f=done_f, done_b=done_b, prop_frames=list(frame_blends), masks_left=mask.copy())
     comp = backend.fgt_stage(frame_blends, mask, done_f, args.step, args.num_ref, args.neighbor_stride)
     out = composite_native(backend, comp, frames_u8, masks_u8, args) if native else comp
     if return_stages:
@@ -575,6 +590,72 @@ def video_inpainting(frames_u8, masks_u8, backend, args=None, num_flows=3, flow_
             stages["comp"] = np.stack(comp)
         return out, stages
     return out
+
+
+# ------------------------------------------------------------------------------------------------ visualisations
+def _write_flow_sets(outroot, sub, sets, backend):
+    """One directory pair per flow set, as the driver names them: {sub}/{mode}_flo/%05d.flo (Middlebury) and
+    {sub}/{mode}_png/%05d.png (flow_viz colours, RGB, written by PIL). sets: [(mode, flows [H,W,2,n])]. Each set is
+    coloured in one batched backend call; the files are encoded on the host pool."""
+    from . import io as IO
+    from PIL import Image
+    written = []
+    for mode, flows in sets:
+        fl = np.ascontiguousarray(np.moveaxis(np.asarray(flows, dtype=np.float32), -1, 0))     # [n,H,W,2]
+        fdir, pdir = os.path.join(outroot, sub, mode + "_flo"), os.path.join(outroot, sub, mode + "_png")
+        os.makedirs(fdir, exist_ok=True)
+        os.makedirs(pdir, exist_ok=True)
+        if not fl.shape[0]:
+            continue
+        imgs = backend.flow_images(fl)
+
+        def one(i):
+            IO.write_flo(os.path.join(fdir, "%05d.flo" % i), fl[i])
+            Image.fromarray(imgs[i]).save(os.path.join(pdir, "%05d.png" % i))
+            return [os.path.join(fdir, "%05d.flo" % i), os.path.join(pdir, "%05d.png" % i)]
+
+        written += sum(_per_frame(one, fl.shape[0]), [])
+    return written
+
+
+def _write_prop(outroot, frames, masks):
+    """save_fgcp (:157-177): prop_frames/ and masks_left/ PNGs through cv2.imwrite of the float arrays times 255 (cv2
+    rounds them), and the same arrays as .npy files in prop_frames_npy/ and masks_left_npy/."""
+    dirs = [os.path.join(outroot, d) for d in ("prop_frames", "masks_left", "prop_frames_npy", "masks_left_npy")]
+    for d in dirs:
+        os.makedirs(d, exist_ok=True)
+    if len(frames) != masks.shape[2]:
+        raise ValueError(f"{len(frames)} propagated frames but {masks.shape[2]} masks")
+
+    def one(i):
+        fr, mk = frames[i] * 255.0, masks[:, :, i] * 255.0
+        paths = [os.path.join(dirs[0], "%05d.png" % i), os.path.join(dirs[1], "%05d.png" % i),
+                 os.path.join(dirs[2], "%05d.npy" % i), os.path.join(dirs[3], "%05d.npy" % i)]
+        for ok in (cv2.imwrite(paths[0], fr), cv2.imwrite(paths[1], mk)):
+            if not ok:
+                raise OSError(f"cv2.imwrite could not write {paths[0]} / {paths[1]}")
+        np.save(paths[2], fr)
+        np.save(paths[3], mk)
+        return paths
+
+    return sum(_per_frame(one, len(frames)), [])
+
+
+def write_visualisations(outroot, vis, backend, vis_flows=False, vis_completed_flows=False, vis_prop=False):
+    """The driver's visualisation outputs under `outroot`, from the dict `vis` that video_inpainting(..., vis_out=vis)
+    filled: --vis_flows (calculate_flow :241-287) flow/{forward,backward}_{flo,png}/; --vis_completed_flows
+    (save_flows :120-155) completed_flow/{forward,backward}_{flo,png}/, coloured like --vis_flows where the driver
+    uses cvbase.flow2rgb; --vis_prop (save_fgcp :157-177) prop_frames/, masks_left/ and their _npy twins. The flow
+    colours come from backend.flow_images. Returns the paths written."""
+    written = []
+    if vis_flows:
+        written += _write_flow_sets(outroot, "flow", [("forward", vis["flow_f"]), ("backward", vis["flow_b"])], backend)
+    if vis_completed_flows:
+        written += _write_flow_sets(outroot, "completed_flow", [("forward", vis["done_f"]), ("backward", vis["done_b"])],
+                                    backend)
+    if vis_prop:
+        written += _write_prop(outroot, vis["prop_frames"], vis["masks_left"])
+    return written
 
 
 # ------------------------------------------------------------------------------------------------ command line
@@ -640,6 +721,16 @@ def arg_parser():
     ap.add_argument("--lafc_mixed_precision", action="store_true",
                     help="run the LAFC flow-completion network with fp16 tensor-core operands, as the reference under "
                          "CUDA autocast (faster, not fp32-accurate; independent of the other two switches)")
+    ap.add_argument("--vis_flows", action="store_true",
+                    help="write the RAFT flows as flow/{forward,backward}_flo/*.flo and, coloured on the GPU, "
+                         "flow/{forward,backward}_png/*.png")
+    ap.add_argument("--vis_completed_flows", action="store_true",
+                    help="write the completed flows as completed_flow/{forward,backward}_{flo,png}/")
+    ap.add_argument("--vis_prop", action="store_true",
+                    help="write the frames after flow-guided propagation (prop_frames/, green where it could not "
+                         "fill) and what is left to fill (masks_left/), as PNG and .npy")
+    ap.add_argument("--vis_frame", action="store_true",
+                    help="accepted for the driver's command line; frames/ is always written")
     for k, v in DEFAULTS.items():
         if k == "mode":
             ap.add_argument("--mode", default=v, choices=list(MODES))
@@ -650,7 +741,7 @@ def arg_parser():
 
 def main(argv=None):
     """`python -m fgt_b200.pipeline --path frames/ --path_mask masks/ --outroot out/ [--mode ...] ...` — the driver's
-    command line (:764-855; the visualisation switches are not offered)."""
+    command line (:764-855), visualisation switches included (write_visualisations)."""
     from . import io as IO
     ap = arg_parser()
     ns = ap.parse_args(argv)
@@ -666,8 +757,11 @@ def main(argv=None):
     masks = IO.read_masks(ns.path_mask, rgb=ns.mode == "watermark_removal") if ns.mode != "video_extrapolation" else [None] * len(frames)
     if len(frames) != len(masks):
         raise ValueError(f"{len(frames)} frames but {len(masks)} masks")
+    vis = {} if ns.vis_flows or ns.vis_completed_flows or ns.vis_prop else None
     comp = video_inpainting(frames, masks, backend, args, lafc_cfg["num_flows"], lafc_cfg["flow_interval"],
-                            native=ns.native)
+                            native=ns.native, vis_out=vis)
+    if vis is not None:
+        write_visualisations(ns.outroot, vis, backend, ns.vis_flows, ns.vis_completed_flows, ns.vis_prop)
     written = IO.write_frames(ns.outroot, comp)
     print(f"Done, {len(comp)} frames written to {ns.outroot} ({len(written)} files)")
     return comp

@@ -485,3 +485,26 @@ def flow_warp_inputs(seed=0, b=2, c=5, h=20, w=28):
     flow[:, :, :, -2:] += 40.0                                         # pushed out of the image
     flow[0, :, h // 2, : w // 2] = 0.0                                 # identity
     return feat, flow
+
+
+# ----------------------------------------------------------------------------------------------
+# flow colour coding (fgt_b200/flowviz.py)
+# ----------------------------------------------------------------------------------------------
+def vis_flows(seed, B, H, W, scale=8.0):
+    """Flows [B,H,W,2] float32 shaped like RAFT's: per image a sum of three random plane waves of `scale` pixels
+    (different in u and v), a constant drift and a little pixel noise, so every direction of the colour wheel occurs
+    and each image has its own maximum."""
+    import numpy as np
+    g = np.random.default_rng(seed)
+    ys, xs = np.arange(H, dtype=np.float32)[:, None], np.arange(W, dtype=np.float32)[None, :]
+    out = np.empty((B, H, W, 2), np.float32)
+    for b in range(B):
+        s = np.float32(scale * g.uniform(0.25, 2.0))
+        for c in range(2):
+            acc = np.full((H, W), g.normal(0.0, 0.5) * s, np.float32)
+            for _ in range(3):
+                fy, fx, ph = g.uniform(-0.05, 0.05), g.uniform(-0.05, 0.05), g.uniform(0, 2 * np.pi)
+                acc += s * np.float32(g.uniform(0.3, 1.0)) * np.sin(ys * np.float32(fy) + xs * np.float32(fx) +
+                                                                    np.float32(ph))
+            out[b, :, :, c] = acc + np.float32(0.05) * s * g.standard_normal((H, W), dtype=np.float32)
+    return out

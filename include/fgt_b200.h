@@ -431,6 +431,23 @@ long long fgt_metrics_workspace(int N, int H, int W, int C);
 int fgt_metrics(const void* a, int a_dtype, const void* b, int b_dtype, int N, int H, int W, int C, void* workspace,
                 long long workspace_bytes, double* out, double* ssim_c, fgt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Flow colour coding of the driver's --vis_flows (RAFT/utils/flow_viz.py flow_to_image :109-132 with
+ * flow_uv_to_colors :70-106 and the 55-entry Middlebury wheel of make_colorwheel :20-67): flows fp32 [B,H,W,2]
+ * (8-byte aligned) -> out uint8 [B,H,W,3], RGB (bgr = 0) or BGR (bgr != 0). Each image is divided by its own maximum
+ * radius + 1e-5. Every operation is rounded as numpy 2 (NEP 50) rounds the reference's: float32 up to the wheel
+ * coordinate, float64 from the interpolation weight on, no contraction. The angle is atan2f, which may differ from the
+ * host's float32 arctan2 by an ulp, so a few values in a million can differ by one level.
+ *   fgt_flow_to_image_workspace  bytes of workspace for B flows of H x W (negative FGT_ERR_* on bad sizes).
+ *   fgt_flow_to_image            two kernels: per-image maximum radius (partial maxima into the workspace; exact in any
+ *                                order), then the colour pass. maxima float [B] (NULL: not written) receives each
+ *                                image's maximum radius, or NaN when the image holds a NaN or Inf, where the reference
+ *                                raises; such an image's output is left unwritten. B at most 65535.
+ * ------------------------------------------------------------------------------------------ */
+long long fgt_flow_to_image_workspace(int B, int H, int W);
+int fgt_flow_to_image(const float* flow, int B, int H, int W, int bgr, void* workspace, long long workspace_bytes,
+                      unsigned char* out, float* maxima, fgt_stream_t stream);
+
 /* 3x3 convolution (zero padding 1, stride 1) with cout <= 3 output channels + bias + activation in one kernel: the
  * nine taps become the N dimension of a wgmma GEMM over the input positions (activation read once) and are summed
  * per output pixel in shared memory — the decoder's final conv + tanh (FGT/models/model.py:185-193). x: NHWC
