@@ -14,19 +14,26 @@
 
 namespace fgt {
 
+// torch.max's maximum, in any reduction order: a NaN anywhere gives NaN (fmaxf would drop it); +0 ranks above -0
+// (torch's own sign of a zero maximum depends on its reduction order).
+__device__ __forceinline__ float max_nan(float a, float b) {
+  if (isnan(a) || isnan(b)) return __int_as_float(0x7fffffff);
+  return (a > b || (a == b && !signbit(a))) ? a : b;
+}
+
 __global__ void plane_max_kernel(const float* __restrict__ x, long long plane, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float red[8];
   const float* p = x + static_cast<long long>(blockIdx.x) * plane;
   float m = -INFINITY;
-  for (long long i = threadIdx.x; i < plane; i += blockDim.x) m = fmaxf(m, p[i]);
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_down_sync(0xffffffffu, m, o));
+  for (long long i = threadIdx.x; i < plane; i += blockDim.x) m = max_nan(m, p[i]);
+  for (int o = 16; o > 0; o >>= 1) m = max_nan(m, __shfl_down_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
   __syncthreads();
   if (threadIdx.x < 32) {
     m = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : -INFINITY;
-    for (int o = 4; o > 0; o >>= 1) m = fmaxf(m, __shfl_down_sync(0xffffffffu, m, o));
+    for (int o = 4; o > 0; o >>= 1) m = max_nan(m, __shfl_down_sync(0xffffffffu, m, o));
     if (threadIdx.x == 0) out[blockIdx.x] = m;
   }
 }

@@ -1,9 +1,9 @@
 // Device-side versions of the driver's mask / resize glue (SURVEY 8f rank 3; tool/video_inpainting.py:264-268, 546-561,
 // 637): scipy.ndimage.binary_dilation (default cross structuring element, `iterations` repeats), binary_fill_holes,
 // cv2.resize INTER_NEAREST on uint8 masks and INTER_LINEAR on float32 images (= F.interpolate bilinear with
-// align_corners=False). Byte / index work: bit-exact for the masks; the bilinear kernel follows OpenCV's arithmetic
-// (horizontal pass, then vertical, float32) and agrees to 1 ulp. HBM-bound helpers: one thread per output element,
-// coalesced along x.
+// align_corners=False). Byte / index work: bit-exact for the masks; the bilinear kernel performs OpenCV's float32
+// operations in OpenCV's order (explicit _rn intrinsics, no FMA contraction), so it is bit-identical to cv2.resize on
+// the driver's two-channel flows. HBM-bound helpers: one thread per output element, coalesced along x.
 #include "common.h"
 #include "ptx.cuh"
 
@@ -121,14 +121,20 @@ __global__ void resize_nearest_u8_kernel(const uint8_t* __restrict__ in, uint8_t
   }
 }
 
-// cv2.resize INTER_LINEAR on float32 [B,H,W,C] (channels last): source coordinate (d + 0.5) * scale - 0.5, clamped
-// to the image with the weight collapsing onto the edge sample (OpenCV's resizeGeneric_: sx < 0 -> (0, fx = 0);
-// sx >= W-1 -> (W-1, fx = 0)); horizontal interpolation of the two source rows first, then vertical, in float32.
-// The same arithmetic is F.interpolate(mode="bilinear", align_corners=False) when `nchw` (planes instead of
-// interleaved channels).
+// cv2.resize INTER_LINEAR on float32 [B,H,W,C] (channels last), as OpenCV's resizeGeneric_ computes it: source
+// coordinate fp32((d + 0.5) * scale - 0.5) in double, s = floor, f = coordinate - s. Along x the weight collapses onto
+// the edge sample (s < 0 -> (0, f = 0); s >= W-1 -> (W-1, f = 0)); along y f is kept and only the two rows are clamped
+// to [0, H-1] (so an edge row is r * (1 - f) + r * f). Each row is a0 * left + a1 * right, then (1 - fy) * r0 + fy * r1,
+// every product and sum rounded to float32 (no FMA). When H = 2 OH and W = 2 OW exactly, cv2 switches to INTER_AREA:
+// (0 + (((a + b) + c) + d)) * 0.25 of the 2x2 block, a b the upper row. cv2 hands C = 1, 3 and 4 to IPP, whose arithmetic
+// differs; the driver resizes flows (C = 2). With `nchw` (planes instead of interleaved channels) the arithmetic is
+// ATen's CPU kernel as built with FMA (UpSample.h, align_corners = False): fp32 fma(scale, d + 0.5, -0.5), negative
+// -> 0, s = trunc, the second tap clamped; rows fma(a0, left, a1 * right), then fma(1 - fy, r0, fy * r1). That is
+// F.interpolate on the CPU bit for bit except on small images, where ATen takes a scalar path (within 1e-7 relative).
 __global__ void resize_bilinear_f32_kernel(const float* __restrict__ in, float* __restrict__ out, int B, int H, int W,
                                            int C, int OH, int OW, int nchw, float out_scale_c0, float out_scale_c1) {
   const double sxs = 1.0 / (static_cast<double>(OW) / W), sys = 1.0 / (static_cast<double>(OH) / H);
+  const bool area2 = !nchw && W == 2 * OW && H == 2 * OH;
   const long long total = static_cast<long long>(B) * OH * OW * C;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -146,39 +152,52 @@ __global__ void resize_bilinear_f32_kernel(const float* __restrict__ in, float* 
       dy = static_cast<int>((t / OW) % OH);
       b = t / (static_cast<long long>(OW) * OH);
     }
-    float fx, fy;
-    int sx, sy;
-    if (nchw) {
-      // ATen (UpSample.h area_pixel_compute_source_index, align_corners = False): float32 throughout, negative -> 0
-      const float scx = static_cast<float>(W) / OW, scy = static_cast<float>(H) / OH;
-      fx = fmaxf(scx * (dx + 0.5f) - 0.5f, 0.f);
-      fy = fmaxf(scy * (dy + 0.5f) - 0.5f, 0.f);
-      sx = min(static_cast<int>(fx), W - 1);
-      sy = min(static_cast<int>(fy), H - 1);
-      fx -= sx;
-      fy -= sy;
-    } else {
-      fx = static_cast<float>((dx + 0.5) * sxs - 0.5);
-      sx = static_cast<int>(floorf(fx));
-      fx -= sx;
-      if (sx < 0) { sx = 0; fx = 0.f; }
-      if (sx >= W - 1) { sx = W - 1; fx = 0.f; }
-      fy = static_cast<float>((dy + 0.5) * sys - 0.5);
-      sy = static_cast<int>(floorf(fy));
-      fy -= sy;
-      if (sy < 0) { sy = 0; fy = 0.f; }
-      if (sy >= H - 1) { sy = H - 1; fy = 0.f; }
-    }
-    const int sx1 = min(sx + 1, W - 1), sy1 = min(sy + 1, H - 1);
     auto at = [&](int y, int x) -> float {
       return nchw ? in[((b * C + c) * H + y) * W + x] : in[((b * H + y) * W + x) * C + c];
     };
-    const float a0 = 1.f - fx, a1 = fx;
-    const float r0 = at(sy, sx) * a0 + at(sy, sx1) * a1;
-    const float r1 = at(sy1, sx) * a0 + at(sy1, sx1) * a1;
-    float v = r0 * (1.f - fy) + r1 * fy;
-    if (c == 0) v *= out_scale_c0;
-    else if (c == 1) v *= out_scale_c1;
+    float v;
+    if (area2) {
+      const int x0 = 2 * dx, y0 = 2 * dy;
+      v = __fadd_rn(__fadd_rn(__fadd_rn(at(y0, x0), at(y0, x0 + 1)), at(y0 + 1, x0)), at(y0 + 1, x0 + 1));
+      v = __fmul_rn(__fadd_rn(0.f, v), 0.25f);
+    } else {
+      float fx, fy;
+      int sx, sy, sy0, sy1;
+      if (nchw) {
+        const float scx = static_cast<float>(W) / OW, scy = static_cast<float>(H) / OH;
+        fx = fmaxf(__fmaf_rn(scx, __fadd_rn(static_cast<float>(dx), 0.5f), -0.5f), 0.f);
+        fy = fmaxf(__fmaf_rn(scy, __fadd_rn(static_cast<float>(dy), 0.5f), -0.5f), 0.f);
+        sx = min(static_cast<int>(fx), W - 1);
+        sy0 = min(static_cast<int>(fy), H - 1);
+        fx = __fsub_rn(fx, static_cast<float>(sx));
+        fy = __fsub_rn(fy, static_cast<float>(sy0));
+        sy1 = min(sy0 + 1, H - 1);
+      } else {
+        fx = static_cast<float>(__dsub_rn(__dmul_rn(dx + 0.5, sxs), 0.5));
+        sx = static_cast<int>(floorf(fx));
+        fx = __fsub_rn(fx, static_cast<float>(sx));
+        if (sx < 0) { sx = 0; fx = 0.f; }
+        if (sx >= W - 1) { sx = W - 1; fx = 0.f; }
+        fy = static_cast<float>(__dsub_rn(__dmul_rn(dy + 0.5, sys), 0.5));
+        sy = static_cast<int>(floorf(fy));
+        fy = __fsub_rn(fy, static_cast<float>(sy));
+        sy0 = min(max(sy, 0), H - 1);
+        sy1 = min(max(sy + 1, 0), H - 1);
+      }
+      const int sx1 = min(sx + 1, W - 1);
+      const float a0 = __fsub_rn(1.f, fx), a1 = fx, b0 = __fsub_rn(1.f, fy);
+      if (nchw) {   // ATen's CPU kernel as built with FMA: fma(a0, left, a1 * right), likewise vertically
+        const float r0 = __fmaf_rn(at(sy0, sx), a0, __fmul_rn(at(sy0, sx1), a1));
+        const float r1 = __fmaf_rn(at(sy1, sx), a0, __fmul_rn(at(sy1, sx1), a1));
+        v = __fmaf_rn(r0, b0, __fmul_rn(r1, fy));
+      } else {
+        const float r0 = __fadd_rn(__fmul_rn(at(sy0, sx), a0), __fmul_rn(at(sy0, sx1), a1));
+        const float r1 = __fadd_rn(__fmul_rn(at(sy1, sx), a0), __fmul_rn(at(sy1, sx1), a1));
+        v = __fadd_rn(__fmul_rn(r0, b0), __fmul_rn(r1, fy));
+      }
+    }
+    if (c == 0) v = __fmul_rn(v, out_scale_c0);
+    else if (c == 1) v = __fmul_rn(v, out_scale_c1);
     out[i] = v;
   }
 }

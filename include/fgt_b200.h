@@ -337,8 +337,9 @@ int fgt_dwpool(const float* a, int ca, const float* b, int cb, int bt, int h, in
  *   fgt_resize_nearest_u8 cv2.resize(..., INTER_NEAREST) on [B,H,W,C] uint8.
  *   fgt_resize_bilinear_f32  cv2.resize(..., INTER_LINEAR) on float32 [B,H,W,C] (nchw = 0) — optionally scaling channel
  *                         0 / 1 of the result (the driver rescales resized flow vectors, :266-267) — or
- *                         F.interpolate(mode="bilinear", align_corners=False) on [B,C,H,W] (nchw = 1); agrees with the
- *                         libraries to float32 rounding of the two 1-D interpolations.
+ *                         F.interpolate(mode="bilinear", align_corners=False) on [B,C,H,W] (nchw = 1). Bit-identical
+ *                         to cv2 for C = 2 (cv2's INTER_AREA when exactly 2x smaller; C = 1, 3, 4 go to IPP in cv2) and
+ *                         to ATen's vectorised CPU kernel (its FMAs included) for nchw.
  * ------------------------------------------------------------------------------------------ */
 int fgt_binary_dilate(const unsigned char* in, int B, int H, int W, int iterations, unsigned char* tmp, unsigned char* out,
                       fgt_stream_t stream);
