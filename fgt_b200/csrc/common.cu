@@ -24,6 +24,13 @@ int set_err(int code, const char* fmt, ...) {
   return code;
 }
 
+int check_act16(const char* who, const void* hi, long long plane, int vec, bool f16_ok) {
+  if (!hi || (reinterpret_cast<uintptr_t>(hi) % (2 * vec) == 0 && plane % vec == 0 && plane >= (f16_ok ? 0 : 1)))
+    return FGT_OK;
+  return set_err(FGT_ERR_ARG, "%s: 16-bit buffer misaligned or plane offset %lld not a %s multiple of %d", who, plane,
+                 f16_ok ? "non-negative" : "positive", vec);
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,

@@ -27,6 +27,12 @@ int set_err(int code, const char* fmt, ...);
                           cudaGetErrorString(e__), __FILE__, __LINE__);                 \
   } while (0)
 
+// A 16-bit activation argument: split-bf16 with the lo plane `plane` elements after `hi` (plane > 0) or, where
+// `f16_ok`, single-plane fp16 (plane == 0). Its kernel accesses `vec` consecutive elements at a time, so hi must be
+// 2*vec-byte aligned and plane a multiple of vec. A NULL hi (no such output) passes. FGT_OK, or FGT_ERR_ARG with the
+// error text set.
+int check_act16(const char* who, const void* hi, long long plane, int vec, bool f16_ok);
+
 // Encode a bf16 tiled tensor map (rank <= 5) with the 128B swizzle and zero OOB fill.
 // dims[0] is the contiguous dimension; strides_bytes has rank-1 entries (dims 1..rank-1).
 int encode_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,

@@ -205,7 +205,8 @@ extern "C" int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, 
   FGT_REQUIRE(cout >= 1 && cout <= 3, FGT_ERR_ARG, "conv_tail: cout=%d (1..3: nine taps times cout must fit 32 columns)", cout);
   FGT_REQUIRE(k_pad == cin, FGT_ERR_ARG, "conv_tail: weights must be packed [32, cin] (k_pad=%d, cin=%d)", k_pad, cin);
   FGT_REQUIRE(n >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "conv_tail: empty problem");
-  FGT_REQUIRE(x_plane % 8 == 0 && w_plane % 8 == 0 && x_plane >= 0 && w_plane >= 0, FGT_ERR_ARG, "conv_tail: plane offsets");
+  if (const int rc = fgt::check_act16("conv_tail: x", x_hi, x_plane, 8, true)) return rc;
+  if (const int rc = fgt::check_act16("conv_tail: weights", w_hi, w_plane, 8, true)) return rc;
   FGT_REQUIRE((x_plane == 0) == (w_plane == 0), FGT_ERR_ARG,
               "conv_tail: activation and weights are both split-bf16 (plane > 0) or both single-plane fp16 (plane 0), "
               "got x_plane=%lld w_plane=%lld", x_plane, w_plane);

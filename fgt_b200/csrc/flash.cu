@@ -302,7 +302,7 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   FGT_REQUIRE(d.q_ld % 8 == 0 && d.k_ld % 8 == 0 && d.v_ld % 8 == 0 && d.out_ld % 8 == 0, FGT_ERR_ARG,
               "attention: leading dimensions must be multiples of 8 elements");
   FGT_REQUIRE(d.q_batch_stride % 8 == 0 && d.k_batch_stride % 8 == 0 && d.v_batch_stride % 8 == 0 &&
-                  d.out_batch_stride % 8 == 0 && d.out_plane % 8 == 0,
+                  d.out_batch_stride % 8 == 0,
               FGT_ERR_ARG, "attention: batch strides must be multiples of 8 elements");
   FGT_REQUIRE(d.mode == 0 || d.mode == 1, FGT_ERR_ARG, "attention: mode=%d", d.mode);
   FGT_REQUIRE(d.f16 == 0 || d.f16 == 1, FGT_ERR_ARG, "attention: f16=%d (0 split-bf16, 1 single-plane fp16)", d.f16);
@@ -310,12 +310,14 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   FGT_REQUIRE(!f16 || (d.q_plane == 0 && d.k_plane == 0 && d.v_plane == 0 && d.out_plane == 0), FGT_ERR_ARG,
               "attention: f16 operands are single-plane (plane offsets must be 0)");
   FGT_REQUIRE(d.q_hi && d.k_hi && d.v_hi && d.out_hi, FGT_ERR_ARG, "attention: null operand");
+  if (const int rc = check_act16("attention: Q", d.q_hi, d.q_plane, 8, f16)) return rc;
+  if (const int rc = check_act16("attention: K", d.k_hi, d.k_plane, 8, f16)) return rc;
+  if (const int rc = check_act16("attention: V", d.v_hi, d.v_plane, 8, f16)) return rc;
+  if (const int rc = check_act16("attention: output", d.out_hi, d.out_plane, 8, f16)) return rc;
   FlashParams p;
   memset(&p, 0, sizeof(p));
   const uint64_t hd = static_cast<uint64_t>(d.heads) * 128;
   const uint64_t planes = f16 ? 1 : 2;
-  FGT_REQUIRE((reinterpret_cast<uintptr_t>(d.q_hi) & 15) == 0 && d.q_plane % 8 == 0, FGT_ERR_ARG,
-              "attention: Q misaligned");
   p.q_hi = reinterpret_cast<const __nv_bfloat16*>(d.q_hi);
   p.q_plane = d.q_plane;
   p.q_batch_stride = d.q_batch_stride;
@@ -357,7 +359,6 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   p.out_batch_stride = d.out_batch_stride;
   p.out_ld = d.out_ld;
   p.out_rowmap = d.out_rowmap;
-  FGT_REQUIRE((reinterpret_cast<uintptr_t>(d.out_hi) & 15) == 0, FGT_ERR_ARG, "attention: output misaligned");
 
   static bool attr_set[2] = {false, false};
   auto kern = f16 ? flash_kernel<true> : flash_kernel<false>;

@@ -89,10 +89,6 @@ __device__ __forceinline__ float act_one(float v, int act) {
   }
 }
 
-// Nearest fp16 value, as fp32. Mixed-precision RAFT (out_half): the fp32 copy of an output equals its fp16 output, as
-// autocast's fp16 tensors do.
-__device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
-
 __device__ __forceinline__ void load_pair(const float* src, long long o0, long long o1, bool two, bool vec, float& x0,
                                           float& x1) {
   if (vec) {
@@ -756,6 +752,7 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
   const int planes = one_term ? 1 : 2;
   FGT_REQUIRE(d.out_half >= 0 && d.out_half <= FGT_OUT_HALF_AUTOCAST, FGT_ERR_ARG, "gemm_tc: out_half=%d", d.out_half);
   FGT_REQUIRE(d.out_half != 1 || d.out_hi, FGT_ERR_ARG, "gemm_tc: out_half without a 16-bit output");
+  if (const int rc = check_act16("gemm_tc: output", d.out_hi, d.out_plane, 1, d.out_half != 0)) return rc;
   FGT_REQUIRE(d.out_half != FGT_OUT_HALF_AUTOCAST || one_term, FGT_ERR_ARG,
               "gemm_tc: FGT_OUT_HALF_AUTOCAST needs a 1-term (fp16) layer");
   p.out_half = (d.out_half && d.out_hi) ? 1 : 0;

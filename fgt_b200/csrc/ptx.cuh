@@ -175,9 +175,80 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
-  return static_cast<uint32_t>(__bfloat16_as_ushort(a)) |
-         (static_cast<uint32_t>(__bfloat16_as_ushort(b)) << 16);
+// Nearest fp16 value, as fp32: where the reference under autocast makes an fp16 tensor.
+__device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// ---------------------------------------------------------------- 16-bit activation stores
+// A 16-bit activation is split-bf16 when plane > 0 (hi[i] = bf16(v), hi[plane + i] = bf16(v - hi)) and single-plane
+// fp16 when plane == 0 (hi[i] = fp16(v)). store16* write 1, 2, 4 or 8 consecutive values at hi[0..]; a store of n
+// values takes 2n-byte aligned addresses (the host's check_act16). Stores of two or more fp16 values saturate to the
+// finite range (pack_f16x2), the single one rounds as __float2half_rn.
+__device__ __forceinline__ void store16(__nv_bfloat16* hi, long long plane, float v) {
+  if (plane == 0) {
+    *reinterpret_cast<__half*>(hi) = __float2half_rn(v);
+  } else {
+    __nv_bfloat16 h, l;
+    split_bf16(v, h, l);
+    hi[0] = h;
+    hi[plane] = l;
+  }
+}
+
+__device__ __forceinline__ void store16x2(__nv_bfloat16* hi, long long plane, float a, float b) {
+  if (plane == 0) {
+    *reinterpret_cast<uint32_t*>(hi) = pack_f16x2(a, b);
+  } else {
+    uint32_t h, l;
+    split_bf16x2(a, b, h, l);
+    *reinterpret_cast<uint32_t*>(hi) = h;
+    *reinterpret_cast<uint32_t*>(hi + plane) = l;
+  }
+}
+
+// Four values converted once, for a store to several places (lo is zero when plane == 0).
+struct Packed16x4 {
+  uint2 hi, lo;
+};
+
+__device__ __forceinline__ Packed16x4 pack16x4(long long plane, float a, float b, float c, float d) {
+  Packed16x4 p = {};
+  if (plane == 0) {
+    p.hi = make_uint2(pack_f16x2(a, b), pack_f16x2(c, d));
+  } else {
+    split_bf16x2(a, b, p.hi.x, p.lo.x);
+    split_bf16x2(c, d, p.hi.y, p.lo.y);
+  }
+  return p;
+}
+
+__device__ __forceinline__ void store16x4(__nv_bfloat16* hi, long long plane, const Packed16x4& p) {
+  *reinterpret_cast<uint2*>(hi) = p.hi;
+  if (plane) *reinterpret_cast<uint2*>(hi + plane) = p.lo;
+}
+
+__device__ __forceinline__ void store16x4(__nv_bfloat16* hi, long long plane, float a, float b, float c, float d) {
+  store16x4(hi, plane, pack16x4(plane, a, b, c, d));
+}
+
+__device__ __forceinline__ void zero16x4(__nv_bfloat16* hi, long long plane) { store16x4(hi, plane, Packed16x4{}); }
+
+__device__ __forceinline__ void store16x8(__nv_bfloat16* hi, long long plane, const float (&v)[8]) {
+  if (plane == 0) {
+    *reinterpret_cast<uint4*>(hi) =
+        make_uint4(pack_f16x2(v[0], v[1]), pack_f16x2(v[2], v[3]), pack_f16x2(v[4], v[5]), pack_f16x2(v[6], v[7]));
+  } else {
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) split_bf16x2(v[2 * t], v[2 * t + 1], h[t], l[t]);
+    *reinterpret_cast<uint4*>(hi) = make_uint4(h[0], h[1], h[2], h[3]);
+    *reinterpret_cast<uint4*>(hi + plane) = make_uint4(l[0], l[1], l[2], l[3]);
+  }
 }
 
 }  // namespace fgt

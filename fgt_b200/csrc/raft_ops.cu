@@ -105,7 +105,7 @@ __global__ void instnorm_act_kernel(const float* __restrict__ x, const double* _
     if (res) {
       if (f16) {  // relu(norm(x)) is an fp16 tensor before the residual add (extractor.py:55-56)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) o[j] = __half2float(__float2half_rn(o[j]));
+        for (int j = 0; j < 4; ++j) o[j] = round_f16(o[j]);
       }
       const float4 r = __ldg(reinterpret_cast<const float4*>(res + off));
       o[0] = fmaxf(o[0] + r.x, 0.f); o[1] = fmaxf(o[1] + r.y, 0.f);
@@ -113,18 +113,10 @@ __global__ void instnorm_act_kernel(const float* __restrict__ x, const double* _
     }
     if (f16) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) o[j] = __half2float(__float2half_rn(o[j]));
+      for (int j = 0; j < 4; ++j) o[j] = round_f16(o[j]);
     }
     if (out) *reinterpret_cast<float4*>(out + off) = make_float4(o[0], o[1], o[2], o[3]);
-    if (f16) {
-      *reinterpret_cast<uint2*>(hi + off) = make_uint2(pack_f16x2(o[0], o[1]), pack_f16x2(o[2], o[3]));
-    } else if (hi) {
-      uint32_t h0, l0, h1, l1;
-      split_bf16x2(o[0], o[1], h0, l0);
-      split_bf16x2(o[2], o[3], h1, l1);
-      *reinterpret_cast<uint2*>(hi + off) = make_uint2(h0, h1);
-      *reinterpret_cast<uint2*>(hi + plane + off) = make_uint2(l0, l1);
-    }
+    if (hi) store16x4(hi + off, plane, o[0], o[1], o[2], o[3]);
   }
 }
 
@@ -193,15 +185,7 @@ __global__ void corr_lookup_kernel(LookupLevels lv, int levels, int radius, cons
       const int a = o / win, b = o - a * win;  // a -> x offset, b -> y offset
       const float v = w00 * patch[b * pw + a] + w01 * patch[b * pw + a + 1] + w10 * patch[(b + 1) * pw + a] +
                       w11 * patch[(b + 1) * pw + a + 1];
-      const long long off = static_cast<long long>(p) * out_pitch + l * win * win + o;
-      if (plane == 0) {  // single-plane fp16 row (input of a 1-term convc1)
-        reinterpret_cast<__half*>(hi)[off] = __float2half_rn(v);
-      } else {
-        __nv_bfloat16 hh, ll;
-        split_bf16(v, hh, ll);
-        hi[off] = hh;
-        hi[plane + off] = ll;
-      }
+      store16(hi + static_cast<long long>(p) * out_pitch + l * win * win + o, plane, v);
     }
     __syncwarp();
   }
@@ -213,15 +197,12 @@ __global__ void corr_lookup_kernel(LookupLevels lv, int levels, int radius, cons
 // x_plane == 0: x is single-plane fp16 (mixed precision), the flow channels are stored as fp16. delta_f16: delta is
 // the flow head's output, an fp16 tensor under autocast, so it is rounded to fp16 before the fp32 add (raft.py:132).
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
-
 __global__ void flow_update_kernel(float* __restrict__ coords, const float* __restrict__ delta, int delta_f16, int n_img,
                                    int h, int w, float* __restrict__ flow_nchw, __nv_bfloat16* __restrict__ x_hi,
                                    long long x_plane, int x_pitch, int x_chan) {
   pdl_launch_dependents();
   pdl_wait();
   const int n = h * w;
-  const bool f16 = x_hi && x_plane == 0;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n_img * n; p += gridDim.x * blockDim.x) {
     const int img = p / n, q = p - img * n;
     float cx = coords[2 * p], cy = coords[2 * p + 1];
@@ -235,17 +216,10 @@ __global__ void flow_update_kernel(float* __restrict__ coords, const float* __re
     const float fx = cx - static_cast<float>(q % w), fy = cy - static_cast<float>(q / w);
     flow_nchw[static_cast<long long>(img) * 2 * n + q] = fx;
     flow_nchw[static_cast<long long>(img) * 2 * n + n + q] = fy;
-    if (f16) {
-      __half* xh = reinterpret_cast<__half*>(x_hi) + static_cast<long long>(p) * x_pitch + x_chan;
-      xh[0] = __float2half_rn(fx);
-      xh[1] = __float2half_rn(fy);
-    } else if (x_hi) {
-      __nv_bfloat16 h0, l0, h1, l1;
-      split_bf16(fx, h0, l0);
-      split_bf16(fy, h1, l1);
-      const long long off = static_cast<long long>(p) * x_pitch + x_chan;
-      x_hi[off] = h0; x_hi[off + 1] = h1;
-      x_hi[x_plane + off] = l0; x_hi[x_plane + off + 1] = l1;
+    if (x_hi) {
+      __nv_bfloat16* xh = x_hi + static_cast<long long>(p) * x_pitch + x_chan;
+      store16(xh, x_plane, fx);
+      store16(xh + 1, x_plane, fy);
     }
   }
 }
@@ -264,14 +238,14 @@ __global__ void f16_to_split_kernel(const __half* __restrict__ src, long long n8
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const uint4 v = __ldg(reinterpret_cast<const uint4*>(src) + i);
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    uint32_t hw[4], lw[4];
+    float f[8];
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
-      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[t]));
-      split_bf16x2(f.x, f.y, hw[t], lw[t]);
+      const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&w[t]));
+      f[2 * t] = f2.x;
+      f[2 * t + 1] = f2.y;
     }
-    reinterpret_cast<uint4*>(hi)[i] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-    reinterpret_cast<uint4*>(hi + plane)[i] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+    store16x8(hi + 8 * i, plane, f);
   }
 }
 
@@ -344,6 +318,7 @@ extern "C" int fgt_instnorm_act(const float* x, const double* stats, int n, int 
                                 fgt_stream_t stream) {
   FGT_REQUIRE(x && stats && C % 4 == 0 && (out || out_hi), FGT_ERR_ARG, "instnorm_act: C=%d", C);
   FGT_REQUIRE(C <= 256, FGT_ERR_ARG, "instnorm_act: C=%d > 256", C);
+  if (const int rc = check_act16("instnorm_act", out_hi, out_plane, 4, true)) return rc;
   const long long total = static_cast<long long>(HW) * (C / 4);
   const dim3 grid(grid_cap(total, 256), n);
   launch_k(instnorm_act_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
@@ -367,6 +342,7 @@ extern "C" int fgt_corr_lookup(const float* const* level_ptrs_host, const int* l
               levels, radius);
   const int win = 2 * radius + 1;
   FGT_REQUIRE(out_pitch >= levels * win * win, FGT_ERR_ARG, "corr_lookup: out_pitch=%d", out_pitch);
+  if (const int rc = check_act16("corr_lookup", out_hi, out_plane, 1, true)) return rc;
   LookupLevels lv;
   for (int i = 0; i < 4; ++i) {
     lv.ptr[i] = i < levels ? level_ptrs_host[i] : nullptr;
@@ -387,6 +363,7 @@ extern "C" int fgt_raft_flow_update(float* coords, const float* delta, int delta
                                     fgt_stream_t stream) {
   FGT_REQUIRE(coords && flow_nchw && n >= 1, FGT_ERR_ARG, "raft_flow_update: null argument");
   FGT_REQUIRE(delta_f16 == 0 || delta_f16 == 1, FGT_ERR_ARG, "raft_flow_update: delta_f16=%d (0 or 1)", delta_f16);
+  if (const int rc = check_act16("raft_flow_update", x_hi, x_plane, 1, true)) return rc;
   launch_k(flow_update_kernel, dim3(grid_cap(static_cast<long long>(n) * h * w, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
       coords, delta, delta_f16, n, h, w, flow_nchw, reinterpret_cast<__nv_bfloat16*>(x_hi), x_plane, x_pitch, x_chan);
   FGT_CUDA(cudaGetLastError());
@@ -394,9 +371,9 @@ extern "C" int fgt_raft_flow_update(float* coords, const float* delta, int delta
 }
 
 extern "C" int fgt_f16_to_split(const void* src, long long n, void* out_hi, long long out_plane, fgt_stream_t stream) {
-  const auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  FGT_REQUIRE(src && out_hi && n >= 0 && n % 8 == 0 && out_plane % 8 == 0 && out_plane >= n && al16(src) && al16(out_hi),
+  FGT_REQUIRE(src && out_hi && n >= 0 && n % 8 == 0 && out_plane >= n && (reinterpret_cast<uintptr_t>(src) & 15) == 0,
               FGT_ERR_ARG, "f16_to_split: n=%lld plane=%lld (multiples of 8, 16-byte aligned buffers)", n, out_plane);
+  if (const int rc = check_act16("f16_to_split", out_hi, out_plane, 8, false)) return rc;
   if (n == 0) return FGT_OK;
   launch_k(f16_to_split_kernel, dim3(grid_cap(n / 8, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
       reinterpret_cast<const __half*>(src), n / 8, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);

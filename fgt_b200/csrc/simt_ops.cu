@@ -6,30 +6,6 @@
 
 namespace fgt {
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* lo, float a, float b, float c,
-                                             float d) {
-  __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
-  split_bf16(a, h0, l0);
-  split_bf16(b, h1, l1);
-  split_bf16(c, h2, l2);
-  split_bf16(d, h3, l3);
-  *reinterpret_cast<uint2*>(hi) = make_uint2(pack_bf16x2(h0, h1), pack_bf16x2(h2, h3));
-  *reinterpret_cast<uint2*>(lo) = make_uint2(pack_bf16x2(l0, l1), pack_bf16x2(l2, l3));
-}
-
-// Four consecutive 16-bit outputs: split-bf16 with the lo plane `plane` elements after hi, or single-plane fp16 rows
-// (the A operand of a 1-term layer, mixed precision) when plane == 0.
-__device__ __forceinline__ void store16x4(__nv_bfloat16* hi, long long plane, float a, float b, float c, float d) {
-  if (plane == 0) *reinterpret_cast<uint2*>(hi) = make_uint2(pack_f16x2(a, b), pack_f16x2(c, d));
-  else store_split4(hi, hi + plane, a, b, c, d);
-}
-
 // ------------------------------------------------------------------------------------------
 // pack: NCHW fp32 (two sources concatenated on C) -> NHWC split-bf16 with channel padding and
 // optional replication padding (ReplicationPad2d of the flow encoder, model.py:207).
@@ -38,6 +14,7 @@ __global__ void pack_nchw_kernel(const float* __restrict__ s0, int c0, const flo
                                  int H, int W, int pad, int cpad, __nv_bfloat16* __restrict__ hi, long long plane) {
   pdl_launch_dependents();
   pdl_wait();
+  __builtin_assume(plane > 0);  // split-bf16 only: the host rejects plane <= 0
   const int Wp = W + 2 * pad, Hp = H + 2 * pad;
   const long long total = static_cast<long long>(n) * Hp * Wp;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -50,10 +27,7 @@ __global__ void pack_nchw_kernel(const float* __restrict__ s0, int c0, const flo
       float v = 0.f;
       if (c < c0) v = s0[((static_cast<long long>(b) * c0 + c) * H + sy) * W + sx];
       else if (c < c0 + c1) v = s1[((static_cast<long long>(b) * c1 + (c - c0)) * H + sy) * W + sx];
-      __nv_bfloat16 h, l;
-      split_bf16(v, h, l);
-      hi[i * cpad + c] = h;
-      hi[plane + i * cpad + c] = l;
+      store16(hi + i * cpad + c, plane, v);
     }
   }
 }
@@ -117,17 +91,7 @@ __global__ void im2col_nchw_kernel(const float* __restrict__ s0, int c0, const f
     float v[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) v[j] = off[j] >= 0 ? srow[off[j] + x0] : 0.f;
-    const long long o = ((static_cast<long long>(b) * OH + oy) * OW + ox) * cpad + g * 8;
-    if (plane == 0) {  // single-plane fp16 rows (input of a 1-term layer)
-      *reinterpret_cast<uint4*>(hi + o) = make_uint4(pack_f16x2(v[0], v[1]), pack_f16x2(v[2], v[3]),
-                                                     pack_f16x2(v[4], v[5]), pack_f16x2(v[6], v[7]));
-    } else {
-      uint32_t hw[4], lw[4];
-#pragma unroll
-      for (int t = 0; t < 4; ++t) split_bf16x2(v[2 * t], v[2 * t + 1], hw[t], lw[t]);
-      *reinterpret_cast<uint4*>(hi + o) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-      *reinterpret_cast<uint4*>(hi + plane + o) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-    }
+    store16x8(hi + ((static_cast<long long>(b) * OH + oy) * OW + ox) * cpad + g * 8, plane, v);
   }
 }
 
@@ -169,12 +133,8 @@ __global__ void __launch_bounds__(256, 4) rownorm_kernel(const float* __restrict
     long long src = d;
     if (gather) src = gather[d];
     if (src < 0) {
-      for (int q = 0; q < dst.n; ++q) {
-        for (int v = lane; v < nvec; v += 32) {
-          *reinterpret_cast<uint2*>(dst.hi[q] + ooff + v * 4) = make_uint2(0u, 0u);
-          if (plane) *reinterpret_cast<uint2*>(dst.hi[q] + ooff + plane + v * 4) = make_uint2(0u, 0u);
-        }
-      }
+      for (int q = 0; q < dst.n; ++q)
+        for (int v = lane; v < nvec; v += 32) zero16x4(dst.hi[q] + ooff + v * 4, plane);
       continue;
     }
     float4 val[kNormMaxVec];
@@ -210,18 +170,8 @@ __global__ void __launch_bounds__(256, 4) rownorm_kernel(const float* __restrict
           const float4 bt = __ldg(reinterpret_cast<const float4*>(beta + v * 4));
           o.x = o.x * gm.x + bt.x; o.y = o.y * gm.y + bt.y; o.z = o.z * gm.z + bt.z; o.w = o.w * gm.w + bt.w;
         }
-        if (plane == 0) {  // single-plane fp16 rows (mixed precision)
-          const uint2 hv = make_uint2(pack_f16x2(o.x, o.y), pack_f16x2(o.z, o.w));
-          for (int q = 0; q < dst.n; ++q) *reinterpret_cast<uint2*>(dst.hi[q] + ooff + v * 4) = hv;
-          continue;
-        }
-        uint32_t h0, l0, h1, l1;
-        split_bf16x2(o.x, o.y, h0, l0);
-        split_bf16x2(o.z, o.w, h1, l1);
-        for (int q = 0; q < dst.n; ++q) {
-          *reinterpret_cast<uint2*>(dst.hi[q] + ooff + v * 4) = make_uint2(h0, h1);
-          *reinterpret_cast<uint2*>(dst.hi[q] + ooff + plane + v * 4) = make_uint2(l0, l1);
-        }
+        const Packed16x4 pk = pack16x4(plane, o.x, o.y, o.z, o.w);
+        for (int q = 0; q < dst.n; ++q) store16x4(dst.hi[q] + ooff + v * 4, plane, pk);
       }
     }
   }
@@ -410,6 +360,7 @@ __global__ void unfold_kernel(const float* __restrict__ img, int bt, int th, int
                               int pd, int OH, int OW, int relu, __nv_bfloat16* __restrict__ hi, long long plane) {
   pdl_launch_dependents();
   pdl_wait();
+  __builtin_assume(plane > 0);  // split-bf16 only: the host rejects plane <= 0
   const int C4 = C / 4;
   if (threadIdx.x >= C4) return;
   const int P = kh * kw;
@@ -428,8 +379,7 @@ __global__ void unfold_kernel(const float* __restrict__ img, int bt, int th, int
     if (relu) {
       v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
     }
-    const long long o = (static_cast<long long>(tok) * P + pidx) * C + c;
-    store_split4(hi + o, hi + plane + o, v.x, v.y, v.z, v.w);
+    store16x4(hi + (static_cast<long long>(tok) * P + pidx) * C + c, plane, v.x, v.y, v.z, v.w);
     ky += dky;
     kx += dkx;
     if (kx >= kw) { kx -= kw; ++ky; }
@@ -485,14 +435,7 @@ __global__ void fold_unfold_kernel(const float* __restrict__ hid, int bt, int th
         acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f);
       }
     }
-    uint32_t h0, l0 = 0u, h1, l1 = 0u;
-    if (plane == 0) {  // single-plane fp16 patches (mixed precision)
-      h0 = pack_f16x2(acc.x, acc.y);
-      h1 = pack_f16x2(acc.z, acc.w);
-    } else {
-      split_bf16x2(acc.x, acc.y, h0, l0);
-      split_bf16x2(acc.z, acc.w, h1, l1);
-    }
+    const Packed16x4 pk = pack16x4(plane, acc.x, acc.y, acc.z, acc.w);
     for (int ty = ty_hi; ty >= 0; --ty) {
       const int ky = y + pd - st * ty;
       if (ky >= kh) break;
@@ -501,9 +444,7 @@ __global__ void fold_unfold_kernel(const float* __restrict__ hid, int bt, int th
         const int kx = x + pd - st * tx;
         if (kx >= kw) break;
         if (kx < 0) continue;
-        const long long o = ((static_cast<long long>(b) * th + ty) * tw + tx) * hidden + (ky * kw + kx) * C + c;
-        *reinterpret_cast<uint2*>(hi + o) = make_uint2(h0, h1);
-        if (plane) *reinterpret_cast<uint2*>(hi + plane + o) = make_uint2(l0, l1);
+        store16x4(hi + ((static_cast<long long>(b) * th + ty) * tw + tx) * hidden + (ky * kw + kx) * C + c, plane, pk);
       }
     }
   }
@@ -532,12 +473,6 @@ __global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ in, long lon
         in + pl * in_plane + ((static_cast<long long>(b) * H + (y >> 1)) * W + (x >> 1)) * C + c));
     *reinterpret_cast<uint4*>(out + pl * out_plane + ((static_cast<long long>(b) * 2 * H + y) * 2 * W + x) * C + c) = v;
   }
-}
-
-// 16-bit output of the CUDA-core producers: split-bf16 (lo plane `plane` elements after hi, plane > 0) or single-plane
-// fp16 (plane == 0); both are stored 4 elements (8 bytes) at a time.
-static bool out16_ok(const void* hi, long long plane) {
-  return hi == nullptr || (plane >= 0 && plane % 4 == 0 && (reinterpret_cast<uintptr_t>(hi) & 7) == 0);
 }
 
 static int grid_for(long long work_items, int block) {
@@ -605,6 +540,7 @@ extern "C" int fgt_pack_nchw(const float* src0, int c0, const float* src1, int c
                              int cpad, void* out_hi, long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(src0 && c0 >= 1 && c0 + c1 <= cpad && cpad % 8 == 0 && (c1 == 0 || src1), FGT_ERR_ARG,
               "pack_nchw: c0=%d c1=%d cpad=%d", c0, c1, cpad);
+  if (const int rc = check_act16("pack_nchw", out_hi, out_plane, 1, false)) return rc;
   const long long total = static_cast<long long>(n) * (H + 2 * pad) * (W + 2 * pad);
   launch_k(pack_nchw_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
       src0, c0, src1, c1, n, H, W, pad, cpad, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
@@ -623,6 +559,7 @@ extern "C" int fgt_im2col_nchw(const float* src0, int c0, const float* src1, int
   const size_t smem = static_cast<size_t>(k) * (c0 + c1) * ((OW - 1) * stride + k) * sizeof(float);
   constexpr size_t kIm2colSmemMax = 160 * 1024;
   FGT_REQUIRE(smem <= kIm2colSmemMax, FGT_ERR_ARG, "im2col_nchw: %zu bytes of staged input rows exceed %zu", smem, kIm2colSmemMax);
+  if (const int rc = check_act16("im2col_nchw", out_hi, out_plane, 8, true)) return rc;
   static bool attr_set = false;
   if (!attr_set) {
     FGT_CUDA(cudaFuncSetAttribute(im2col_nchw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kIm2colSmemMax)));
@@ -656,8 +593,7 @@ extern "C" int fgt_rownorm_bcast(const float* a, int ca, int lda, const float* b
   dst.n = n_out;
   for (int q = 0; q < n_out; ++q) {
     FGT_REQUIRE(dst.hi[q], FGT_ERR_ARG, "rownorm: destination %d is NULL", q);
-    FGT_REQUIRE(out16_ok(dst.hi[q], out_plane), FGT_ERR_ARG,
-                "rownorm: destination %d misaligned or plane offset %lld not a non-negative multiple of 4", q, out_plane);
+    if (const int rc = check_act16("rownorm", dst.hi[q], out_plane, 4, true)) return rc;
   }
   FGT_REQUIRE(out_plane != 0 || n_out == 1, FGT_ERR_ARG,
               "rownorm: single-plane fp16 output (out_plane = 0) takes one destination, got %d", n_out);
@@ -687,8 +623,7 @@ extern "C" int fgt_dwconv3x3_res(const float* x, int bt, int h, int w, int C, co
                                  float* out, void* out_hi, long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(x && weight && bias && out, FGT_ERR_ARG, "dwconv3x3_res: null argument");
   FGT_REQUIRE(C % 4 == 0, FGT_ERR_ARG, "dwconv3x3_res: C=%d must be a multiple of 4", C);
-  FGT_REQUIRE(out16_ok(out_hi, out_plane), FGT_ERR_ARG,
-              "dwconv3x3_res: 16-bit output misaligned or plane offset %lld not a non-negative multiple of 4", out_plane);
+  if (const int rc = check_act16("dwconv3x3_res", out_hi, out_plane, 4, true)) return rc;
   const int tx = (C / 4) < 128 ? (C / 4 + 31) / 32 * 32 : 128;   // threads along channels (x), tokens of the row along y
   launch_k(dwconv3_res_kernel, dim3(bt * h, w >= 16 ? 4 : 1), dim3(tx, 256 / tx > 0 ? 256 / tx : 1), 0, reinterpret_cast<cudaStream_t>(stream), 
       x, bt, h, w, C, weight, bias, out, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
@@ -701,8 +636,7 @@ extern "C" int fgt_fold(const float* hid, int bt, int th, int tw, int C, int kh,
                         fgt_stream_t stream) {
   FGT_REQUIRE(hid && C % 4 == 0 && (out || out_hi), FGT_ERR_ARG, "fold: C=%d", C);
   FGT_REQUIRE(C / 4 <= 64, FGT_ERR_ARG, "fold: C=%d > 256", C);
-  FGT_REQUIRE(out16_ok(out_hi, out_plane), FGT_ERR_ARG,
-              "fold: 16-bit output misaligned or plane offset %lld not a non-negative multiple of 4", out_plane);
+  if (const int rc = check_act16("fold", out_hi, out_plane, 4, true)) return rc;
   const int gx = (C / 4 + 1) / 2 * 2;  // channel groups per row of the thread block
   const dim3 blk(gx, 256 / gx);
   launch_k(fold_kernel, dim3(bt * OH), dim3(blk), 0, reinterpret_cast<cudaStream_t>(stream), 
@@ -716,6 +650,7 @@ extern "C" int fgt_unfold(const float* img, int bt, int th, int tw, int C, int k
                           int OH, int OW, int relu, void* out_hi, long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(img && out_hi && C % 4 == 0, FGT_ERR_ARG, "unfold: C=%d", C);
   FGT_REQUIRE(C / 4 <= 64, FGT_ERR_ARG, "unfold: C=%d > 256", C);
+  if (const int rc = check_act16("unfold", out_hi, out_plane, 4, false)) return rc;
   const int gx = (C / 4 + 1) / 2 * 2;
   const dim3 blk(gx, 256 / gx);
   launch_k(unfold_kernel, dim3(bt * th * tw), dim3(blk), 0, reinterpret_cast<cudaStream_t>(stream), 
@@ -728,8 +663,7 @@ extern "C" int fgt_fold_unfold(const float* hid, int bt, int th, int tw, int C, 
                                int OH, int OW, int relu, void* out_hi, long long out_plane, fgt_stream_t stream) {
   FGT_REQUIRE(hid && out_hi && C % 4 == 0 && C / 4 <= 64, FGT_ERR_ARG, "fold_unfold: C=%d", C);
   FGT_REQUIRE(kh >= stride && kw >= stride, FGT_ERR_ARG, "fold_unfold: kernel %dx%d must cover the stride %d", kh, kw, stride);
-  FGT_REQUIRE(out16_ok(out_hi, out_plane), FGT_ERR_ARG,
-              "fold_unfold: output misaligned or plane offset %lld not a non-negative multiple of 4", out_plane);
+  if (const int rc = check_act16("fold_unfold", out_hi, out_plane, 4, true)) return rc;
   // every pixel of the map must lie under at least one patch (last patch ends at (th-1)*stride + kh - 1 - pad)
   FGT_REQUIRE((th - 1) * stride + kh - pad >= OH && (tw - 1) * stride + kw - pad >= OW && pad < kh && pad < kw, FGT_ERR_ARG,
               "fold_unfold: patches do not cover the %dx%d map", OH, OW);
@@ -746,6 +680,8 @@ extern "C" int fgt_upsample2x(const void* in_hi, long long in_plane, int n, int 
   FGT_REQUIRE(in_hi && out_hi && C % 8 == 0, FGT_ERR_ARG, "upsample2x: C=%d", C);
   FGT_REQUIRE((in_plane == 0) == (out_plane == 0) && in_plane >= 0 && out_plane >= 0, FGT_ERR_ARG,
               "upsample2x: plane offsets %lld -> %lld (both 0: fp16, both > 0: split-bf16)", in_plane, out_plane);
+  if (const int rc = check_act16("upsample2x", in_hi, in_plane, 8, true)) return rc;
+  if (const int rc = check_act16("upsample2x", out_hi, out_plane, 8, true)) return rc;
   const long long total = (in_plane == 0 ? 1LL : 2LL) * n * (2 * H) * (2 * W) * (C / 8);
   launch_k(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
       reinterpret_cast<const __nv_bfloat16*>(in_hi), in_plane, n, H, W, C, reinterpret_cast<__nv_bfloat16*>(out_hi),

@@ -21,13 +21,7 @@ namespace fgt {
 constexpr int kMaxVec = 6;  // float4 per lane: up to 768 channels per row (FGT: 512 + 256)
 constexpr int kMaxVecV = 4; // value rows: up to 512 channels
 
-__device__ __forceinline__ float swin_wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// LayerNorm (no affine) of the first `nvec` float4 of val[] per lane (channels 4*(lane + 32 i)), stored split-bf16.
+// LayerNorm (no affine) of the first `nvec` float4 of val[] per lane (channels 4*(lane + 32 i)), stored 16-bit.
 template <int NV>
 __device__ __forceinline__ void swin_norm_store(const float4 (&val)[kMaxVec], int nvec, int C, float eps,
                                            __nv_bfloat16* __restrict__ hi, long long plane, int lane) {
@@ -35,7 +29,7 @@ __device__ __forceinline__ void swin_norm_store(const float4 (&val)[kMaxVec], in
 #pragma unroll
   for (int i = 0; i < NV; ++i)
     if (lane + 32 * i < nvec) sum += (val[i].x + val[i].y) + (val[i].z + val[i].w);
-  const float mean = swin_wsum(sum) / static_cast<float>(C);
+  const float mean = warp_sum(sum) / static_cast<float>(C);
   float sq = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i)
@@ -43,29 +37,18 @@ __device__ __forceinline__ void swin_norm_store(const float4 (&val)[kMaxVec], in
       const float a = val[i].x - mean, b = val[i].y - mean, c = val[i].z - mean, d = val[i].w - mean;
       sq += (a * a + b * b) + (c * c + d * d);
     }
-  const float rstd = rsqrtf(swin_wsum(sq) / static_cast<float>(C) + eps);
+  const float rstd = rsqrtf(warp_sum(sq) / static_cast<float>(C) + eps);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int v = lane + 32 * i;
-    if (v < nvec && plane == 0) {  // single-plane fp16 rows (mixed precision)
-      *reinterpret_cast<uint2*>(hi + v * 4) =
-          make_uint2(pack_f16x2((val[i].x - mean) * rstd, (val[i].y - mean) * rstd),
-                     pack_f16x2((val[i].z - mean) * rstd, (val[i].w - mean) * rstd));
-    } else if (v < nvec) {
-      uint32_t h0, l0, h1, l1;
-      split_bf16x2((val[i].x - mean) * rstd, (val[i].y - mean) * rstd, h0, l0);
-      split_bf16x2((val[i].z - mean) * rstd, (val[i].w - mean) * rstd, h1, l1);
-      *reinterpret_cast<uint2*>(hi + v * 4) = make_uint2(h0, h1);
-      *reinterpret_cast<uint2*>(hi + plane + v * 4) = make_uint2(l0, l1);
-    }
+    if (v < nvec)
+      store16x4(hi + v * 4, plane, (val[i].x - mean) * rstd, (val[i].y - mean) * rstd, (val[i].z - mean) * rstd,
+                (val[i].w - mean) * rstd);
   }
 }
 
 __device__ __forceinline__ void swin_zero_row(__nv_bfloat16* __restrict__ hi, long long plane, int nvec, int lane) {
-  for (int v = lane; v < nvec; v += 32) {
-    *reinterpret_cast<uint2*>(hi + v * 4) = make_uint2(0u, 0u);
-    if (plane) *reinterpret_cast<uint2*>(hi + plane + v * 4) = make_uint2(0u, 0u);
-  }
+  for (int v = lane; v < nvec; v += 32) zero16x4(hi + v * 4, plane);
 }
 
 struct SwinPrepArgs {
@@ -212,12 +195,11 @@ extern "C" int fgt_swin_prep(const float* x, const float* fp, int d, int df, int
               FGT_ERR_ARG, "swin_prep: d=%d df=%d (d <= 512, d + df <= 768)", d, df);
   FGT_REQUIRE(bt >= 1 && h >= 1 && w >= 1 && nl >= 1 && gd >= 1 && gh >= 1 && gw >= 1 && R >= nl + gh * gw, FGT_ERR_ARG,
               "swin_prep: geometry bt=%d h=%d w=%d nl=%d R=%d gd=%d gh=%d gw=%d", bt, h, w, nl, R, gd, gh, gw);
-  FGT_REQUIRE(qkn_plane % 4 == 0 && vn_plane % 4 == 0, FGT_ERR_ARG, "swin_prep: plane offsets");
-  FGT_REQUIRE(qkn_plane >= 0 && vn_plane >= 0 && (qkn_plane == 0) == (vn_plane == 0), FGT_ERR_ARG,
+  if (const int rc = fgt::check_act16("swin_prep: qkn", qkn_hi, qkn_plane, 4, true)) return rc;
+  if (const int rc = fgt::check_act16("swin_prep: vn", vn_hi, vn_plane, 4, true)) return rc;
+  FGT_REQUIRE((qkn_plane == 0) == (vn_plane == 0), FGT_ERR_ARG,
               "swin_prep: qkn and vn are both split-bf16 (plane > 0) or both single-plane fp16 (plane 0), got %lld / %lld",
               qkn_plane, vn_plane);
-  FGT_REQUIRE(((reinterpret_cast<uintptr_t>(qkn_hi) | reinterpret_cast<uintptr_t>(vn_hi)) & 7) == 0, FGT_ERR_ARG,
-              "swin_prep: outputs must be 8-byte aligned");
   fgt::SwinPrepArgs a;
   a.x = x; a.fp = fp; a.d = d; a.df = df; a.bt = bt; a.h = h; a.w = w; a.win_map = win_map; a.nl = nl; a.R = R;
   a.gd = gd; a.gh = gh; a.gw = gw; a.gk_w = gk_w; a.gk_b = gk_b; a.gv_w = gv_w; a.gv_b = gv_b;

@@ -347,7 +347,7 @@ class FGT(NativeNet):
         if H % 4 or W % 4:
             raise ValueError(f"FGT input {H}x{W} must be divisible by 4 (model.py:55-63 views features as H//4 x W//4)")
         g = type("Geo", (), {})()
-        g.a16 = torch.float16 if mixed else torch.bfloat16  # 16-bit activations: fp16 (mixed) or split-bf16
+        g.a16 = lib.act16_dtype(mixed)
         bt = b * t
         g.b, g.t, g.bt, g.H, g.W = b, t, bt, H, W
         g.OH, g.OW = H // 4, W // 4

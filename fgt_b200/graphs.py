@@ -44,14 +44,11 @@ class GraphedCall:
 
 
 def workspace(bufs, name, shape, dev, dtype=torch.float32, zero=False):
-    """Buffer `name` of the workspace dict `bufs`, allocated on first use. A bfloat16 buffer is split-bf16, [2, *shape]
-    (hi and lo planes); fp16 and fp32 buffers are [*shape]."""
-    t = bufs.get(name)
-    if t is None:
-        if dtype == torch.bfloat16:
-            shape = (2,) + tuple(shape)
-        t = bufs[name] = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=dev)
-    return t
+    """Buffer `name` of the workspace dict `bufs`, allocated on first use: bfloat16 as lib.empty_split, else [*shape]."""
+    if name not in bufs:
+        t = lib.empty_split(shape, dev) if dtype == torch.bfloat16 else torch.empty(shape, dtype=dtype, device=dev)
+        bufs[name] = t.zero_() if zero else t
+    return bufs[name]
 
 
 def _drop_weights(net, incompatible_keys):

@@ -131,8 +131,7 @@ class P3DNet(NativeNet):
         c = self.c
         H2, W2, H4, W4 = H // 2, W // 2, H // 4, W // 4
         bufs = self._geo.setdefault((T, H, W, mixed), {})
-        a16 = torch.float16 if mixed else torch.bfloat16  # 16-bit activations: fp16 (mixed) or split-bf16
-        B = lambda n, s, split=True: workspace(bufs, n, s, dev, a16 if split else torch.float32)  # noqa: E731
+        B = lambda n, s, split=True: workspace(bufs, n, s, dev, lib.act16_dtype(mixed) if split else torch.float32)  # noqa: E731
         conv = (lambda *a, **k: ops.conv(*a, autocast=True, **k)) if mixed else ops.conv  # noqa: E731
         linear = (lambda *a, **k: ops.linear(*a, autocast=True, **k)) if mixed else ops.linear  # noqa: E731
         L = lib.ACT_LEAKY02

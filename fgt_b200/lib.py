@@ -193,14 +193,26 @@ def empty_split(shape, device):
     return torch.empty((2,) + tuple(shape), dtype=torch.bfloat16, device=device)
 
 
+def act16_dtype(mixed):
+    """dtype of the 16-bit activations: fp16 in mixed precision, split-bf16 otherwise."""
+    return torch.float16 if mixed else torch.bfloat16
+
+
 def view16(t, *shape):
     """A 16-bit activation tensor viewed as `shape`: [2, *shape] when split-bf16, [*shape] when fp16."""
     return t.view(*shape) if t.dtype == torch.float16 else t.view(2, *shape)
 
 
-def plane_elems(s):
-    """Element offset from the hi plane to the lo plane (works for row-sliced views too)."""
-    return s.stride(0)
+def plane16(t, split_only=False):
+    """The C ABI's plane offset of a 16-bit activation: hi-to-lo element offset of a split-bf16 tensor (row-sliced views
+    too), 0 for an fp16 tensor or None. split_only: the entry takes split-bf16 only, and fp16 raises TypeError."""
+    if t is None or (t.dtype == torch.float16 and not split_only):
+        return 0
+    if t.dtype != torch.bfloat16:
+        raise TypeError(f"a {'split-bf16' if split_only else 'split-bf16 or fp16'} tensor is required, got {t.dtype}")
+    if t.dim() == 0 or t.shape[0] != 2:
+        raise ValueError(f"a split-bf16 tensor has a leading plane dimension of 2, got shape {tuple(t.shape)}")
+    return t.stride(0)
 
 
 class ASeg:
@@ -242,7 +254,7 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
         assert (s.split.dtype == torch.float16) == f16, "A segments and weight: both split-bf16 or both fp16"
         a = d.seg[i]
         a.hi = s.split.data_ptr() + 2 * s.elem_offset
-        a.plane = 0 if f16 else plane_elems(s.split)
+        a.plane = plane16(s.split)
         a.C, a.DX, a.DY, a.DZ = s.C, s.DX, s.DY, s.DZ
         a.sx, a.sy, a.sz = s.sx, s.sy, s.sz
         a.c_base, a.c_per_group, a.c_count = s.c_base, s.c_per_group, s.c_count
@@ -250,7 +262,7 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
     d.kx, d.ky, d.kz, d.stride, d.dil = kx, ky, kz, stride, dil
     d.pad_x, d.pad_y, d.pad_z = pad_x, pad_y, pad_z
     d.w_hi = w_split.data_ptr()
-    d.w_plane = 0 if f16 else plane_elems(w_split)
+    d.w_plane = plane16(w_split)
     d.N = N
     d.k_pad = w_split.shape[-1]
     d.groups = groups
@@ -265,7 +277,7 @@ def gemm_tc(segs, w_split, N, *, kx=1, ky=1, kz=1, stride=1, dil=1, pad_x=0, pad
     d.out_f32 = (out_f32.data_ptr() + 4 * out_elem_offset) if out_f32 is not None else None
     if out_split is not None:
         d.out_hi = out_split.data_ptr() + 2 * out_elem_offset
-        d.out_plane = _plane16(out_split)
+        d.out_plane = plane16(out_split)
         d.out_half = 1 if out_split.dtype == torch.float16 else 0
         assert not autocast or d.out_half, "autocast rounding: the 16-bit output is fp16"
     if autocast:
@@ -294,10 +306,10 @@ def attention(q, k, v, out, *, batches, heads, Lq, Lk, Lk_rows=None, q_ld, k_ld,
     K and V share one [rows, 3*C] projection buffer)."""
     d = FgtAttnDesc()
     d.f16 = 1 if q.dtype == torch.float16 else 0
-    d.q_hi, d.q_plane, d.q_batch_stride, d.q_ld = q.data_ptr() + 2 * q_off, _plane16(q), q_batch_stride, q_ld
-    d.k_hi, d.k_plane, d.k_batch_stride, d.k_ld = k.data_ptr() + 2 * k_off, _plane16(k), k_batch_stride, k_ld
-    d.v_hi, d.v_plane, d.v_batch_stride, d.v_ld = v.data_ptr() + 2 * v_off, _plane16(v), v_batch_stride, v_ld
-    d.out_hi, d.out_plane, d.out_batch_stride, d.out_ld = out.data_ptr(), _plane16(out), out_batch_stride, out_ld
+    d.q_hi, d.q_plane, d.q_batch_stride, d.q_ld = q.data_ptr() + 2 * q_off, plane16(q), q_batch_stride, q_ld
+    d.k_hi, d.k_plane, d.k_batch_stride, d.k_ld = k.data_ptr() + 2 * k_off, plane16(k), k_batch_stride, k_ld
+    d.v_hi, d.v_plane, d.v_batch_stride, d.v_ld = v.data_ptr() + 2 * v_off, plane16(v), v_batch_stride, v_ld
+    d.out_hi, d.out_plane, d.out_batch_stride, d.out_ld = out.data_ptr(), plane16(out), out_batch_stride, out_ld
     d.batches, d.heads, d.head_dim = batches, heads, 128
     d.Lq, d.Lk = Lq, Lk
     d.Lk_rows = Lk if Lk_rows is None else Lk_rows
@@ -316,7 +328,7 @@ def pack_nchw(src0, src1, out_split, pad=0, tag=""):
     c1 = src1.shape[1] if src1 is not None else 0
     cpad = out_split.shape[-1]
     with _Prof("pack_nchw", tag, 0, 4.0 * n * (c0 + c1) * H * W + 4.0 * out_split[0].numel()):
-        call("fgt_pack_nchw", src0, c0, src1, c1, n, H, W, pad, cpad, out_split, plane_elems(out_split))
+        call("fgt_pack_nchw", src0, c0, src1, c1, n, H, W, pad, cpad, out_split, plane16(out_split, split_only=True))
 
 
 def im2col_nchw(src0, src1, out_split, *, k, stride, pad, replicate, OH, OW, scale=1.0, shift=0.0, tag=""):
@@ -324,11 +336,10 @@ def im2col_nchw(src0, src1, out_split, *, k, stride, pad, replicate, OH, OW, sca
     n, c0, H, W = src0.shape
     c1 = src1.shape[1] if src1 is not None else 0
     cpad = out_split.shape[-1]
-    half = out_split.dtype == torch.float16  # plain fp16 rows [n, OH, OW, cpad] for a 1-term layer
-    nbytes = 4.0 * n * (c0 + c1) * H * W + (2.0 * out_split.numel() if half else 4.0 * out_split[0].numel())
+    nbytes = 4.0 * n * (c0 + c1) * H * W + 2.0 * out_split.numel()
     with _Prof("im2col_nchw", tag, 0, nbytes):
         call("fgt_im2col_nchw", src0, c0, src1, c1, n, H, W, k, stride, pad, 1 if replicate else 0, OH, OW, cpad, scale,
-             shift, out_split, 0 if half else plane_elems(out_split))
+             shift, out_split, plane16(out_split))
 
 
 def rownorm(a, b, out_split, *, gather=None, rows_per_batch, total_rows, dst_batch_rows, dst_row0=0, eps=1e-5,
@@ -338,7 +349,7 @@ def rownorm(a, b, out_split, *, gather=None, rows_per_batch, total_rows, dst_bat
     cb, ldb = (b.shape[-1], b.shape[-1]) if b is not None else (0, 0)
     with _Prof("rownorm", tag, 0, 8.0 * total_rows * (ca + cb)):
         call("fgt_rownorm", a, ca, lda, b, cb, ldb, gather, rows_per_batch, total_rows, dst_batch_rows, dst_row0, gamma, beta,
-             out_split, _plane16(out_split), eps)
+             out_split, plane16(out_split), eps)
 
 
 def rownorm_bcast(a, dst_ptrs, plane, *, gather=None, rows_per_batch, total_rows, dst_batch_rows, dst_row0=0, eps=1e-5,
@@ -386,7 +397,7 @@ def conv_tail(x_split, n, H, W, cin, w_split, cout, bias, act, out, *, nchw, tag
     # 2*9*cout*cin FLOP per 4*(cin+cout) bytes = ~13 FLOP/B at 64 -> 3: HBM-bound, reported against the copy roofline
     nbytes = 4.0 * n * H * W * (cin + cout)
     with _Prof("conv_tail", tag, 0.0, nbytes):
-        call("fgt_conv_tail", x_split, _plane16(x_split), n, H, W, cin, w_split, _plane16(w_split), w_split.shape[-1], cout,
+        call("fgt_conv_tail", x_split, plane16(x_split), n, H, W, cin, w_split, plane16(w_split), w_split.shape[-1], cout,
              bias, act, out, os_n, os_c, os_y, os_x)
 
 
@@ -397,27 +408,27 @@ def swin_prep(x, fp, bt, h, w, win_map, nl, R, gd, gh, gw, gk_w, gk_b, gv_w, gv_
     G = gh * gw
     nbytes = 4.0 * bt * ((nl + 2 * h * w) * (d + df) + (nl + G) * (2 * d + df))  # reads (rows + pooling) + split writes
     with _Prof("swin_prep", tag, 0, nbytes):
-        call("fgt_swin_prep", x, fp, d, df, bt, h, w, win_map, nl, R, gd, gh, gw, gk_w, gk_b, gv_w, gv_b, qkn, _plane16(qkn),
-             vn, _plane16(vn), eps)
+        call("fgt_swin_prep", x, fp, d, df, bt, h, w, win_map, nl, R, gd, gh, gw, gk_w, gk_b, gv_w, gv_b, qkn, plane16(qkn),
+             vn, plane16(vn), eps)
 
 
 def dwconv3x3_res(x, bt, h, w, C, weight, bias, out, out_split=None, tag=""):
     """out_split (optional 16-bit copy): split-bf16 or plain fp16."""
     with _Prof("dwconv3x3_res", tag, 0, 12.0 * bt * h * w * C):
-        call("fgt_dwconv3x3_res", x, bt, h, w, C, weight, bias, out, out_split, _plane16(out_split))
+        call("fgt_dwconv3x3_res", x, bt, h, w, C, weight, bias, out, out_split, plane16(out_split))
 
 
 def fold(hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, *, normalize, add=None, out=None, out_split=None, tag=""):
     """out_split (optional 16-bit output): split-bf16 or plain fp16."""
     with _Prof("fold", tag, 0, 4.0 * bt * (th * tw * kh * kw * C + OH * OW * C * (2 if add is not None else 1))):
         call("fgt_fold", hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, 1 if normalize else 0, add, out, out_split,
-             _plane16(out_split))
+             plane16(out_split))
 
 
 def unfold(img, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu=True, tag=""):
     with _Prof("unfold", tag, 0, 4.0 * bt * (th * tw * kh * kw * C + OH * OW * C)):
         call("fgt_unfold", img, bt, th, tw, C, kh, kw, stride, pad, OH, OW, 1 if relu else 0, out_split,
-             plane_elems(out_split))
+             plane16(out_split, split_only=True))
 
 
 def fold_unfold(hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu=True, tag=""):
@@ -425,13 +436,13 @@ def fold_unfold(hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, out_split, relu
     (or plain fp16)."""
     with _Prof("fold_unfold", tag, 0, 8.0 * bt * th * tw * kh * kw * C):
         call("fgt_fold_unfold", hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, 1 if relu else 0, out_split,
-             _plane16(out_split))
+             plane16(out_split))
 
 
 def upsample2x(in_split, n, H, W, C, out_split, tag=""):
     """Nearest x2 of NHWC [n, H, W, C]: split-bf16 in and out, or plain fp16 in and out."""
     with _Prof("upsample2x", tag, 0, (2.5 if in_split.dtype == torch.float16 else 5.0) * n * H * W * C * 4):
-        call("fgt_upsample2x", in_split, _plane16(in_split), n, H, W, C, out_split, _plane16(out_split))
+        call("fgt_upsample2x", in_split, plane16(in_split), n, H, W, C, out_split, plane16(out_split))
 
 
 # ------------------------------------------------------------------------------------------ RAFT helpers
@@ -440,16 +451,10 @@ def chan_stats(x, n, HW, C, stats, tag=""):
         call("fgt_chan_stats", x, n, HW, C, stats)
 
 
-def _plane16(t):
-    """Plane offset of a 16-bit kernel output: 0 selects single-plane fp16 (a torch.float16 tensor), otherwise the
-    split-bf16 lo-plane offset."""
-    return 0 if t is None or t.dtype == torch.float16 else plane_elems(t)
-
-
 def instnorm_act(x, stats, n, HW, C, *, relu=True, res=None, out=None, out_split=None, eps=1e-5, tag=""):
     """out_split: split-bf16 [2, ...] or a plain fp16 tensor (single-plane rows of a 1-term layer)."""
     with _Prof("instnorm_act", tag, 0, 4.0 * n * HW * C * (3 if res is not None else 2)):
-        call("fgt_instnorm_act", x, stats, n, HW, C, eps, 1 if relu else 0, res, out, out_split, _plane16(out_split))
+        call("fgt_instnorm_act", x, stats, n, HW, C, eps, 1 if relu else 0, res, out, out_split, plane16(out_split))
 
 
 def avgpool2(src, rows, h, w, dst, tag=""):
@@ -466,13 +471,13 @@ def corr_lookup(levels, coords, n_pix, radius, out_split, tag=""):
     win = 2 * radius + 1
     with _Prof("corr_lookup", tag, 0, 4.0 * n_pix * nl * ((win + 1) ** 2 + win * win)):
         call("fgt_corr_lookup", ptrs, hs, ws, nl, radius, coords, n_pix, out_split.shape[-1], out_split,
-             _plane16(out_split))
+             plane16(out_split))
 
 
 def raft_flow_update(coords, delta, h, w, flow_nchw, x_split=None, x_chan=0, n=1, delta_f16=False, tag=""):
     """x_split: split-bf16 GRU input, or fp16 for the mixed-precision path; delta_f16: round delta to fp16 first."""
     with _Prof("raft_flow_update", tag, 0, 32.0 * n * h * w):
-        call("fgt_raft_flow_update", coords, delta, 1 if delta_f16 else 0, n, h, w, flow_nchw, x_split, _plane16(x_split),
+        call("fgt_raft_flow_update", coords, delta, 1 if delta_f16 else 0, n, h, w, flow_nchw, x_split, plane16(x_split),
              x_split.shape[-1] if x_split is not None else 0, x_chan)
 
 
@@ -484,4 +489,4 @@ def convex_upsample(mask, flow_nchw, h, w, out, n=1, tag=""):
 def f16_to_split(src, out_split, tag=""):
     """fp16 tensor -> split-bf16 [2, ...] of the same element count (exact)."""
     with _Prof("f16_to_split", tag, 0, 6.0 * src.numel()):
-        call("fgt_f16_to_split", src, src.numel(), out_split, plane_elems(out_split))
+        call("fgt_f16_to_split", src, src.numel(), out_split, plane16(out_split, split_only=True))

@@ -172,9 +172,8 @@ class RAFT(NativeNet):
         """(B, A) workspace allocators of geometry `key`: B(name, shape, dtype=fp32) and A(name, shape) for the 16-bit
         activations of the path, split-bf16 (fp32 path) or fp16 (mixed)."""
         bufs = self._geo.setdefault(key, {})
-        a16 = torch.float16 if mixed else torch.bfloat16
         return ((lambda nm, s, dtype=torch.float32: workspace(bufs, nm, s, dev, dtype)),
-                (lambda nm, s, zero=False: workspace(bufs, nm, s, dev, a16, zero)))
+                (lambda nm, s, zero=False: workspace(bufs, nm, s, dev, lib.act16_dtype(mixed), zero)))
 
     # ------------------------------------------------------------------ encoders
     def _encoder(self, img, net, P, dev, n, mixed=False):
