@@ -205,6 +205,8 @@ extern "C" int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, 
   FGT_REQUIRE(cout >= 1 && cout <= 3, FGT_ERR_ARG, "conv_tail: cout=%d (1..3: nine taps times cout must fit 32 columns)", cout);
   FGT_REQUIRE(k_pad == cin, FGT_ERR_ARG, "conv_tail: weights must be packed [32, cin] (k_pad=%d, cin=%d)", k_pad, cin);
   FGT_REQUIRE(n >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "conv_tail: empty problem");
+  FGT_REQUIRE(act == FGT_ACT_NONE || act == FGT_ACT_TANH || act == FGT_ACT_RELU || act == FGT_ACT_SIGMOID ||
+                  act == FGT_ACT_LEAKY02, FGT_ERR_ARG, "conv_tail: act=%d", act);
   if (const int rc = fgt::check_act16("conv_tail: x", x_hi, x_plane, 8, true)) return rc;
   if (const int rc = fgt::check_act16("conv_tail: weights", w_hi, w_plane, 8, true)) return rc;
   FGT_REQUIRE((x_plane == 0) == (w_plane == 0), FGT_ERR_ARG,

@@ -483,55 +483,6 @@ static int grid_for(long long work_items, int block) {
   return static_cast<int>(g);
 }
 
-// ------------------------------------------------------------------------------------------
-// tapsum: second half of a k x k convolution with a handful of output channels (FGT decoder's final
-// 64->3 conv, RAFT's flow head 256->2), computed "taps as N": a 1x1 GEMM first produces
-// Y[p, tap*cout + c] = <W[c,:,tap], in[p,:]> for every input pixel p (the A tile is read ONCE instead of
-// once per tap, which is what bounds a tiny-N implicit GEMM), then
-//   out[n, y, x, c] = act(bias[c] + sum_tap Y[tap*cout + c][(n, y + ty - py, x + tx - px)])   (zero outside).
-// Y is column-planar ([column][pixel], the GEMM's strided-store epilogue writes it coalesced), so every one
-// of the k*k*cout reads of a warp is one contiguous 128-byte run of pixels.
-// ------------------------------------------------------------------------------------------
-constexpr int kTapsumMaxC = 4;
-
-__global__ void tapsum_kernel(const float* __restrict__ Y, int H, int W, int cout, int kx, int ky, int px, int py,
-                              long long ycol, const float* __restrict__ bias, int act, float* __restrict__ out,
-                              long long os_n, long long os_y, long long os_x, long long os_c) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int x = blockIdx.x * 32 + threadIdx.x;
-  const int y = blockIdx.y * 8 + threadIdx.y;
-  const int n = blockIdx.z;
-  if (x >= W || y >= H) return;
-  float acc[kTapsumMaxC];
-#pragma unroll
-  for (int c = 0; c < kTapsumMaxC; ++c) acc[c] = (c < cout && bias) ? __ldg(bias + c) : 0.f;
-  for (int ty = 0; ty < ky; ++ty) {
-    const int yy = y + ty - py;
-    if (yy < 0 || yy >= H) continue;
-    for (int tx = 0; tx < kx; ++tx) {
-      const int xx = x + tx - px;
-      if (xx < 0 || xx >= W) continue;
-      const float* col = Y + (ty * kx + tx) * cout * ycol + (static_cast<long long>(n) * H + yy) * W + xx;
-#pragma unroll
-      for (int c = 0; c < kTapsumMaxC; ++c)
-        if (c < cout) acc[c] += __ldg(col + c * ycol);
-    }
-  }
-  float* o = out + n * os_n + y * os_y + x * os_x;
-#pragma unroll
-  for (int c = 0; c < kTapsumMaxC; ++c) {
-    if (c < cout) {
-      float v = acc[c];
-      if (act == FGT_ACT_TANH) v = tanhf(v);
-      else if (act == FGT_ACT_RELU) v = fmaxf(v, 0.f);
-      else if (act == FGT_ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
-      else if (act == FGT_ACT_LEAKY02) v = v > 0.f ? v : 0.2f * v;
-      o[c * os_c] = v;
-    }
-  }
-}
-
 }  // namespace fgt
 
 using namespace fgt;
@@ -686,21 +637,6 @@ extern "C" int fgt_upsample2x(const void* in_hi, long long in_plane, int n, int 
   launch_k(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
       reinterpret_cast<const __nv_bfloat16*>(in_hi), in_plane, n, H, W, C, reinterpret_cast<__nv_bfloat16*>(out_hi),
       out_plane);
-  FGT_CUDA(cudaGetLastError());
-  return FGT_OK;
-}
-
-extern "C" int fgt_tapsum(const float* y, int n, int H, int W, int cout, int kx, int ky, int pad_x, int pad_y,
-                          long long ycol, const float* bias, int act, float* out, long long os_n, long long os_y,
-                          long long os_x, long long os_c, fgt_stream_t stream) {
-  FGT_REQUIRE(y && out && n >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "tapsum: null / empty argument");
-  FGT_REQUIRE(cout >= 1 && cout <= kTapsumMaxC && kx >= 1 && ky >= 1 && ycol >= static_cast<long long>(n) * H * W,
-              FGT_ERR_ARG, "tapsum: cout=%d (max %d) taps %dx%d column stride %lld", cout, kTapsumMaxC, kx, ky, ycol);
-  FGT_REQUIRE(act == FGT_ACT_NONE || act == FGT_ACT_TANH || act == FGT_ACT_RELU || act == FGT_ACT_SIGMOID ||
-                  act == FGT_ACT_LEAKY02, FGT_ERR_ARG, "tapsum: act=%d", act);
-  const dim3 grid((W + 31) / 32, (H + 7) / 8, n);
-  launch_k(tapsum_kernel, grid, dim3(32, 8), 0, reinterpret_cast<cudaStream_t>(stream), y, H, W, cout, kx, ky, pad_x,
-           pad_y, ycol, bias, act, out, os_n, os_y, os_x, os_c);
   FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }

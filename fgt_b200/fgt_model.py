@@ -332,10 +332,8 @@ class FGT(NativeNet):
         deconv("dec1", "decoder.layer1.conv.featureConv")
         layer("dec2", "decoder.layer2.featureConv")
         deconv("dec3", "decoder.layer3.conv.featureConv")
-        layer("dec4", "decoder.final.featureConv")
-        # final 64->3 conv as "taps as N": a 1x1 GEMM with N = 9*3 (padded to 32) + fgt_tapsum (shift, add, bias, tanh)
-        w4 = sd["decoder.final.featureConv.weight"]
-        put("dec4t", lib.pack_taps_as_n(w4), torch.zeros(32))
+        # final 64->3 conv for fgt_conv_tail: the taps as the N of its GEMM (9*3 rows, zero-padded to 32)
+        put("dec4", lib.pack_taps_as_n(sd["decoder.final.featureConv.weight"]), sd["decoder.final.featureConv.bias"])
         self._packed[half] = P
         return P
 
@@ -723,7 +721,7 @@ class FGT(NativeNet):
         conv([(d1, c2)], P["dec2"], out_split=d2, **k3)
         self._deconv(d2, c2 // 2, P, "dec3", d3)
         # final 64 -> 3 conv + tanh: taps-as-N tensor-core GEMM and the 9-tap sum in one kernel (no HBM intermediate)
-        lib.conv_tail(d3, bt, H, W, c2 // 2, P["dec4t"]["w"], 3, P["dec4"]["b"], lib.ACT_TANH, out, nchw=True, tag="dec4")
+        lib.conv_tail(d3, bt, H, W, c2 // 2, P["dec4"]["w"], 3, P["dec4"]["b"], lib.ACT_TANH, out, nchw=True, tag="dec4")
         lib._scope[1:] = []
         return out
 

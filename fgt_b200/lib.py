@@ -363,15 +363,6 @@ def rownorm_bcast(a, dst_ptrs, plane, *, gather=None, rows_per_batch, total_rows
              beta, arr, len(dst_ptrs), plane, eps)
 
 
-def tapsum(y, n, H, W, cout, k, bias, act, out, *, nchw, tag=""):
-    """out = act(bias + sum over the k*k taps of the shifted columns of the column-planar y [cols, n*H*W]);
-    out is [n,cout,H,W] (nchw) or [n,H,W,cout] fp32. The producing GEMM stores with os_x=1, os_c=n*H*W."""
-    ycol = y.shape[-1]
-    os_n, os_y, os_x, os_c = (cout * H * W, W, 1, H * W) if nchw else (H * W * cout, W * cout, cout, 1)
-    with _Prof("tapsum", tag, 0, 4.0 * n * H * W * (k * k * cout + cout)):
-        call("fgt_tapsum", y, n, H, W, cout, k, k, k // 2, k // 2, ycol, bias, act, out, os_n, os_y, os_x, os_c)
-
-
 def pack_taps_as_n(w, n_pad=32):
     """[cout, cin, k, k] conv weight -> [n_pad, cin, 1, 1] weight of the equivalent 1x1 'taps as N' GEMM
     (row tap*cout + c = W[c, :, ty, tx]; zero rows up to n_pad so that the epilogue takes the vector path)."""

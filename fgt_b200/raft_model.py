@@ -156,9 +156,8 @@ class RAFT(NativeNet):
             P[f"gru.zr{s}"] = ops.packed(f"gru.zr{s}", torch.cat([wz, wr], 0), torch.cat([bz, br], 0), dev, [128, 256],
                                          half=half)
         put("fh1", u + "flow_head.conv1")
-        put("fh2", u + "flow_head.conv2")
-        w2 = rnd(sd[u + "flow_head.conv2.weight"])
-        P["fh2t"] = ops.packed("fh2t", lib.pack_taps_as_n(w2), torch.zeros(32), dev, half=half)
+        w2, b2 = wb(u + "flow_head.conv2")  # 256 -> 2 conv for fgt_conv_tail: the taps as the N of its GEMM
+        P["fh2"] = ops.packed("fh2", lib.pack_taps_as_n(w2), b2, dev, half=half)
         put("mask0", u + "mask.0")
         put("mask2", u + "mask.2")
         P["mask2"]["b"] = P["mask2"]["b"] * 0.25  # mask = 0.25 * conv(x) (update.py:135): alpha scales W x
@@ -306,7 +305,6 @@ class RAFT(NativeNet):
         rh = A("rh", (n, h, w, 128))
         fh = A("fh", (n, h, w, 256))
         delta = B("delta", (tot, 2))
-        fh2y = B("fh2y", (32, tot))  # column-planar partial products of the flow head
         m0 = A("m0", (n, h, w, 256))
         mask = B("mask", (tot, 576))
         h4 = lib.view16(hsp, n, h, w, 128)
@@ -334,9 +332,8 @@ class RAFT(NativeNet):
                          out_f32=hf.view(n, h, w, 128), out_split=h4, **kw)
             # flow head (update.py:13-14)
             ops.conv([(h4, 128)], P["fh1"], kx=3, ky=3, pad_x=1, pad_y=1, act=RELU, out_split=fh)
-            # 256->2 conv as "taps as N" (1x1 GEMM with N = 18 -> 32, then shift-and-add): A is read once, not 9x
-            ops.linear([(lib.view16(fh, tot, 256), 256)], P["fh2t"], tot, out_f32=fh2y, os_x=1, os_c=tot)
-            lib.tapsum(fh2y, n, h, w, 2, 3, P["fh2"]["b"], NONE, delta, nchw=False, tag="fh2")
+            # 256->2 conv: taps-as-N tensor-core GEMM and the 9-tap sum in one kernel (no HBM intermediate)
+            lib.conv_tail(fh, n, h, w, 256, P["fh2"]["w"], 2, P["fh2"]["b"], NONE, delta, nchw=False, tag="fh2")
             lib.raft_flow_update(coords, delta, h, w, flow_nchw, xbuf, 254, n=n, delta_f16=mixed)
             if not test_mode or it == iters - 1:
                 # mask head scaled by 0.25 (update.py:122-125,135) + convex upsampling (raft.py:73-84)

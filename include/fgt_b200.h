@@ -310,16 +310,6 @@ int fgt_peer_import(const unsigned char handle[64], void** ptr);
 int fgt_peer_unimport(void* ptr);
 int fgt_peer_barrier(void* const* flags_host, int n, int rank, void* epoch_ctr, fgt_stream_t stream);
 
-/* Second half of a k x k convolution with <= 4 output channels computed "taps as N": y is column-planar
- * fp32, y[(tap*cout + c) * ycol + p] = <W[c,:,tap], in[p,:]> for every INPUT pixel p of [n,H,W] (one 1x1
- * fgt_gemm_tc launch with os_x = 1, os_c = ycol: A read once instead of once per tap); this kernel forms
- * out[n,y,x,c] = act(bias[c] + sum_tap y[(tap*cout + c) * ycol + (n, y+ty-pad_y, x+tx-pad_x)]) with zero padding and
- * arbitrary output strides (NCHW or NHWC). Replaces the output side of nn.Conv2d(64, 3, 3) + tanh at
- * FGT/models/model.py:185-193 and of FlowHead.conv2 at RAFT/update.py:10-14. */
-int fgt_tapsum(const float* y, int n, int H, int W, int cout, int kx, int ky, int pad_x, int pad_y, long long ycol,
-               const float* bias, int act, float* out, long long os_n, long long os_y, long long os_x,
-               long long os_c, fgt_stream_t stream);
-
 /* Depthwise k x k, stride k convolution (+bias) of the token grid [bt,h,w,ca+cb], zero-padded to
  * (gh*k, gw*k) -> fp32 [bt, gh*gw, ca+cb]. weight is the torch layout [C,1,k,k].
  * Replaces global_extract_k / global_extract_v, attention_flow.py:135,145. */
@@ -451,10 +441,10 @@ int fgt_flow_to_image(const float* flow, int B, int H, int W, int bgr, void* wor
 
 /* 3x3 convolution (zero padding 1, stride 1) with cout <= 3 output channels + bias + activation in one kernel: the
  * nine taps become the N dimension of a wgmma GEMM over the input positions (activation read once) and are summed
- * per output pixel in shared memory — the decoder's final conv + tanh (FGT/models/model.py:185-193). x: NHWC
- * split-bf16 [n,H,W,cin], cin a multiple of 64 (<= 256); w: split-bf16 [32, cin], row tap*cout + c = W[c,:,ty,tx]
- * (zero rows up to 32); out: fp32 with element strides (os_n, os_c, os_y, os_x). Replaces fgt_gemm_tc "taps as N" +
- * fgt_tapsum and their column-planar intermediate. */
+ * per output pixel in shared memory. x: NHWC split-bf16 [n,H,W,cin], cin a multiple of 64 (<= 256); w: split-bf16
+ * [32, cin], row tap*cout + c = W[c,:,ty,tx] (zero rows up to 32); act: FGT_ACT_NONE, _LEAKY02, _RELU, _SIGMOID or
+ * _TANH; out: fp32 with element strides (os_n, os_c, os_y, os_x). Replaces the decoder's final nn.Conv2d(64, 3, 3) +
+ * tanh (FGT/models/model.py:185-193) and FlowHead.conv2, nn.Conv2d(256, 2, 3) (RAFT/update.py:10,14). */
 int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, int W, int cin, const void* w_hi, long long w_plane,
                   int k_pad, int cout, const float* bias, int act, float* out, long long os_n, long long os_c,
                   long long os_y, long long os_x, fgt_stream_t stream);

@@ -2,7 +2,7 @@
 
 `emulating_all()` installs a `KernelEmulator` as the library `lib.load()` returns, the way tests/gemm_emulator.py
 installs its `fgt_gemm_tc` interpreter (which this class extends), so the production launchers fill their arguments as
-they do on the GPU and every launch of a forward is executed here instead: the 17 entries of `ENTRIES` and
+they do on the GPU and every launch of a forward is executed here instead: the 16 entries of `ENTRIES` and
 `fgt_gemm_tc`. Any other entry is refused. `gemm_emulator.emulating()` stays strict (GEMM only).
 
 Semantics are restated from include/fgt_b200.h and from the reference operations the header names (through oracle/),
@@ -20,7 +20,7 @@ not from the kernels' code paths:
 - fgt_swin_prep: window rows through win_map (< 0: zero rows) and pooled rows (depthwise gd x gd / stride gd + bias over
   the zero-padded grid, weights tap-major), LayerNorm of [x ; f'] into qkn and of x into vn; rows [nl + G, R) of each
   frame are not written.
-- fgt_conv_tail / fgt_tapsum: act(bias + 3x3 (k x k) convolution with zero padding) at arbitrary output strides.
+- fgt_conv_tail: act(bias + 3x3 convolution with zero padding) at arbitrary output strides.
 - fgt_chan_stats: per (image, channel) sum and sum of squares. fgt_instnorm_act: (x - mean) / sqrt(var + eps) with the
   biased variance from those sums, ReLU, residual relu(y + res); an fp16 output rounds y before the residual add and
   again after it, and the fp32 copy holds the fp16 value.
@@ -51,7 +51,7 @@ from tests.test_launch_trace import recording
 
 ENTRIES = ("fgt_im2col_nchw", "fgt_rownorm", "fgt_attention", "fgt_fold_unfold", "fgt_fold", "fgt_dwconv3x3_res",
            "fgt_swin_prep", "fgt_conv_tail", "fgt_upsample2x", "fgt_chan_stats", "fgt_instnorm_act", "fgt_avgpool2",
-           "fgt_corr_lookup", "fgt_raft_flow_update", "fgt_tapsum", "fgt_convex_upsample", "fgt_f16_to_split")
+           "fgt_corr_lookup", "fgt_raft_flow_update", "fgt_convex_upsample", "fgt_f16_to_split")
 
 
 def _k16(p, plane):
@@ -91,8 +91,6 @@ def form(name, a):
         return (_k16(a["out_hi"], a["out_plane"]), a["levels"], a["radius"])
     if name == "fgt_raft_flow_update":
         return (_on(a["delta"]), bool(a["delta_f16"]), _k16(a["x_hi"], a["x_plane"]))
-    if name == "fgt_tapsum":
-        return (a["act"], _on(a["bias"]), a["os_x"] == 1)
     assert name in ENTRIES, name
     return ()
 
@@ -417,24 +415,6 @@ class KernelEmulator(GemmEmulator):
             for tx in range(3):
                 t = ty * 3 + tx
                 v += xp[:, ty:ty + H, tx:tx + W, :] @ wt[t * cout:(t + 1) * cout].t()
-        v = _act(v, a["act"])
-        idx = (torch.arange(n)[:, None, None, None] * a["os_n"] + torch.arange(H)[None, :, None, None] * a["os_y"]
-               + torch.arange(W)[None, None, :, None] * a["os_x"] + torch.arange(cout)[None, None, None, :] * a["os_c"])
-        self.st32(a["out"], idx, v)
-
-    def _tapsum(self, a):
-        n, H, W, cout, kx, ky = (a[x] for x in "n H W cout kx ky".split())
-        Y = self.flat(a["y"], torch.float32)
-        v = torch.zeros(n, H, W, cout, dtype=torch.float64)
-        if a["bias"]:
-            v += self.f32(a["bias"], cout)
-        for ty in range(ky):
-            for tx in range(kx):
-                for c in range(cout):
-                    o = ((ty * kx + tx) * cout + c) * a["ycol"]
-                    col = F.pad(Y[o:o + n * H * W].double().view(n, H, W),
-                                (a["pad_x"], kx - 1 - a["pad_x"], a["pad_y"], ky - 1 - a["pad_y"]))
-                    v[..., c] += col[:, ty:ty + H, tx:tx + W]
         v = _act(v, a["act"])
         idx = (torch.arange(n)[:, None, None, None] * a["os_n"] + torch.arange(H)[None, :, None, None] * a["os_y"]
                + torch.arange(W)[None, None, :, None] * a["os_x"] + torch.arange(cout)[None, None, None, :] * a["os_c"])

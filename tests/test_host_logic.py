@@ -241,6 +241,8 @@ def test_c_abi_rejects_bad_arguments_round2_entry_points():
     assert rc == -1 and "cout=4" in L.fgt_last_error().decode()
     rc = L.fgt_conv_tail(one, ll(0), 1, 8, 8, 48, one, ll(0), 48, 3, one, 0, one, ll(0), ll(0), ll(0), ll(0), None)
     assert rc == -1 and "conv_tail" in L.fgt_last_error().decode()          # cin must be a multiple of 64
+    rc = L.fgt_conv_tail(one, ll(0), 1, 8, 8, 64, one, ll(0), 64, 3, one, 5, one, ll(0), ll(0), ll(0), ll(0), None)
+    assert rc == -1 and "act=5" in L.fgt_last_error().decode()              # LeakyReLU(0.01) has no tail epilogue
     rc = L.fgt_binary_dilate(one, 1, 4, 4, 1, one, one, None)
     assert rc == -1 and "alias" in L.fgt_last_error().decode()
     rc = L.fgt_binary_dilate(one, 1, 4, 4, 0, ctypes.c_void_p(16), ctypes.c_void_p(24), None)

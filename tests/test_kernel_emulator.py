@@ -6,7 +6,7 @@ through them on the CPU against the reference goldens and oracles.
   discrete options of one call) that occurs in the six golden traces has a case here. A forward that starts calling a
   new kernel, or a kernel with a new option, fails `test_every_trace_form_has_a_case`.
 - Cases: each launches the production launcher (`lib.*`) under `emulating_all()` and compares the interpreter's float64
-  values with `F.layer_norm`, `F.fold` / `F.unfold`, `F.conv2d` (depthwise, and taps as channels), `F.instance_norm`,
+  values with `F.layer_norm`, `F.fold` / `F.unfold`, `F.conv2d` (depthwise and 3x3), `F.instance_norm`,
   `F.avg_pool2d`, `F.interpolate`, `oracle.raft_oracle.corr_lookup` / `upsample_flow`, or a float64 softmax attention
   written per zone and per window. Bar EXACT (1e-12 of the largest value): the reference is fed the operands as stored.
   The stored elements must be exactly the operation's own (rows past nl + G of swin_prep, columns past 324 of the
@@ -352,39 +352,23 @@ def _swin_prep(fmt):
     return emu.forms
 
 
-# ----------------------------------------------------------------------------------------------- conv_tail / tapsum
-@case(("split",), ("f16",), ids=["split", "f16"])
-def _conv_tail(fmt):
-    n, H, W, cin, cout = 2, 9, 21, 64, 3
+# -------------------------------------------------------------------------------------------------------- conv_tail
+@case(("split", True), ("f16", True), ("split", False), ("f16", False), ids=["split", "f16", "split-nhwc", "f16-nhwc"])
+def _conv_tail(fmt, nchw):
+    """FGT's decoder tail (64 -> 3, tanh, NCHW output) and RAFT's flow head tail (256 -> 2, no activation, NHWC)."""
+    n, H, W = 2, 9, 21
+    cin, cout, act = (64, 3, lib.ACT_TANH) if nchw else (256, 2, lib.ACT_NONE)
     x, xv = _act16(_randn(n, H, W, cin, seed=24), fmt)
     w = _randn(cout, cin, 3, 3, seed=25, scale=0.1)
     wp = lib.pack_taps_as_n(w).view(32, cin)
     wt, wv = _act16(wp, fmt)
     bias = _randn(cout, seed=26)
-    out = _buf((n, cout, H, W), "f32")
-    emu = _run(lambda: lib.conv_tail(x, n, H, W, cin, wt, cout, bias, lib.ACT_TANH, out, nchw=True))
+    out = _buf((n, cout, H, W) if nchw else (n, H, W, cout), "f32")
+    emu = _run(lambda: lib.conv_tail(x, n, H, W, cin, wt, cout, bias, act, out, nchw=nchw))
     wref = wv[:9 * cout].view(3, 3, cout, cin).permute(2, 3, 0, 1)
-    ref = torch.tanh(F.conv2d(xv.permute(0, 3, 1, 2), wref, bias.double(), padding=1))
+    ref = F.conv2d(xv.permute(0, 3, 1, 2), wref, bias.double(), padding=1)
+    ref = torch.tanh(ref) if nchw else ref.permute(0, 2, 3, 1)
     _check(emu, out, _buf(out.shape, "f32"), ref, "conv_tail")
-    return emu.forms
-
-
-@case(())
-def _tapsum():
-    """RAFT's flow head tail: 3x3 taps of a column-planar [18, ycol] input summed into NHWC [n, h, w, 2]."""
-    n, H, W, cout, k = 2, 7, 13, 2, 3
-    ycol = n * H * W + 10
-    Y = _randn(k * k * cout, ycol, seed=27)
-    bias = _randn(cout, seed=28)
-    out = _buf((n, H, W, cout), "f32")
-    emu = _run(lambda: lib.tapsum(Y, n, H, W, cout, k, bias, lib.ACT_NONE, out, nchw=False))
-    planes = Y[:, :n * H * W].double().view(k * k * cout, n, H, W).permute(1, 0, 2, 3)
-    sel = torch.zeros(cout, k * k * cout, k, k, dtype=torch.float64)   # taps as input channels
-    for t in range(k * k):
-        for c in range(cout):
-            sel[c, t * cout + c, t // k, t % k] = 1.0
-    ref = F.conv2d(planes, sel, bias.double(), padding=k // 2).permute(0, 2, 3, 1)
-    _check(emu, out, _buf(out.shape, "f32"), ref, "tapsum")
     return emu.forms
 
 

@@ -35,10 +35,10 @@ budget); the others are checked for their addresses only.
 Observed on an H100 80GB HBM3, the largest error over all replayed launches in units of the entry's bar: bit-identical
 for upsample2x, f16_to_split, raft_flow_update and unscaled im2col_nchw, and for scaled im2col_nchw (0); attention
 0.20 (split) / 0.35 (fp16); gemm_tc 0.62 (split, fp32) / 0.41 (fp16); avgpool2 0.67; chan_stats 0.0018;
-conv_tail 0.35; convex_upsample 0.013; corr_lookup 0.56 (split); dwconv3x3_res 0.72; fold 0.70; fold_unfold 0.35;
-instnorm_act 0.57 (split), and every fp16 value inside its interval; rownorm 0.69 (0.34 on the low-variance rows);
-swin_prep 0.64 (0.36); tapsum 0.011. The fp16 outputs of corr_lookup, dwconv3x3_res, fold, fold_unfold, rownorm and
-swin_prep reach one fp16 ulp (1.0), never two.
+conv_tail 0.35 (0.29 in RAFT's flow head); convex_upsample 0.013; corr_lookup 0.56 (split); dwconv3x3_res 0.72;
+fold 0.70; fold_unfold 0.35; instnorm_act 0.57 (split), and every fp16 value inside its interval; rownorm 0.69 (0.34
+on the low-variance rows); swin_prep 0.64 (0.36). The fp16 outputs of corr_lookup, dwconv3x3_res, fold, fold_unfold,
+rownorm and swin_prep reach one fp16 ulp (1.0), never two.
 
 Each of these changes to a kernel's arithmetic fails a test here: lookup windows a and b swapped (error 5e4 x the bar),
 eps dropped from rownorm (non-finite on the constant rows; 58 x the bar in FGT's 64 x 96 forward), swin_prep writing a

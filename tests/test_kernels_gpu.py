@@ -327,29 +327,6 @@ def test_fold_unfold_dwconv_dwpool_upsample_pack():
     assert (got[..., 4:] == 0).all()
 
 
-@pytest.mark.parametrize("n,H,W,cin,cout,act,nchw", [(2, 37, 53, 64, 3, 4, True), (3, 16, 20, 256, 2, 0, False),
-                                                      (1, 8, 40, 128, 3, 2, True)])
-def test_taps_as_n_conv(n, H, W, cin, cout, act, nchw):
-    """Tiny-Cout 3x3 conv as a 1x1 GEMM over taps (pack_taps_as_n) + fgt_tapsum == F.conv2d (zero padding)."""
-    lib = _lib()
-    from fgt_b200 import packing
-    dev = torch.device("cuda:0")
-    torch.manual_seed(7)
-    x = torch.randn(n, H, W, cin, device=dev)
-    w = torch.randn(cout, cin, 3, 3, device=dev) / (9 * cin) ** 0.5
-    b = torch.randn(cout, device=dev)
-    ref = F.conv2d(x.permute(0, 3, 1, 2).double(), w.double(), b.double(), padding=1)
-    ref = {0: lambda t: t, 2: torch.relu, 4: torch.tanh}[act](ref)
-    wt = packing.pack_weight(lib.pack_taps_as_n(w)).to(dev)
-    y = torch.empty(32, n * H * W, device=dev)   # column-planar
-    lib.gemm_tc([lib.ASeg(lib.to_split(x.reshape(n * H * W, cin)), cin, n * H * W)], wt, 32, out_w=n * H * W, bn=32,
-                bias=torch.zeros(32, device=dev), out_f32=y, os_x=1, os_c=n * H * W)
-    out = torch.empty((n, cout, H, W) if nchw else (n, H, W, cout), device=dev)
-    lib.tapsum(y, n, H, W, cout, 3, b, act, out, nchw=nchw)
-    got = out if nchw else out.permute(0, 3, 1, 2)
-    assert_close(got, ref, KTOL, "taps-as-N conv")
-
-
 @pytest.mark.parametrize("bt,h,w", [(2, 20, 36), (1, 22, 36), (1, 7, 13)])
 def test_swin_prep_vs_torch(bt, h, w):
     """fgt_swin_prep = zero-pad + window partition + depthwise pooling + the two LayerNorm statistics of SWMHSA's
@@ -403,9 +380,11 @@ def test_swin_prep_vs_torch(bt, h, w):
     assert (got_q[:, nwin * 64:nl] == 0).all() and (got_q[:, nl + G:] == 14.0).all()   # dummy window zeroed, pad rows untouched
 
 
-@pytest.mark.parametrize("n,H,W,cin,cout,act", [(2, 24, 40, 64, 3, 4), (1, 21, 37, 128, 2, 0), (3, 240, 432, 64, 3, 4)])
+@pytest.mark.parametrize("n,H,W,cin,cout,act", [(2, 24, 40, 64, 3, 4), (1, 21, 37, 128, 2, 0), (3, 240, 432, 64, 3, 4),
+                                                  (2, 37, 53, 64, 3, 4), (3, 16, 20, 256, 2, 0), (1, 8, 40, 128, 3, 2)])
 def test_conv_tail_vs_torch(n, H, W, cin, cout, act):
-    """fgt_conv_tail (taps-as-N GEMM + in-SM tap sum + bias + activation) against F.conv2d in fp64, edge tiles included."""
+    """fgt_conv_tail (taps-as-N GEMM + in-SM tap sum + bias + activation) against F.conv2d in fp64, edge tiles included:
+    FGT's decoder tail (64 -> 3, tanh), RAFT's flow head tail (256 -> 2, no activation) and a ReLU case."""
     lib = _lib()
     from fgt_b200 import packing
     dev = torch.device("cuda:0")
@@ -414,8 +393,7 @@ def test_conv_tail_vs_torch(n, H, W, cin, cout, act):
     w = torch.randn(cout, cin, 3, 3, device=dev) / (cin * 9) ** 0.5
     b = torch.randn(cout, device=dev)
     ref = F.conv2d(x.double(), w.double(), b.double(), padding=1)
-    if act == 4:
-        ref = torch.tanh(ref)
+    ref = {0: lambda t: t, 2: torch.relu, 4: torch.tanh}[act](ref)
     xs = lib.to_split(x.permute(0, 2, 3, 1).contiguous())
     ws = packing.pack_weight(lib.pack_taps_as_n(w)).to(dev)
     out = torch.full((n, cout, H, W), float("nan"), device=dev)
