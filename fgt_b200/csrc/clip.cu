@@ -107,20 +107,13 @@ __global__ void comp_to_u8_kernel(const float* __restrict__ comp, long long tota
     out[g] = static_cast<unsigned char>(static_cast<int>(comp[g]));
 }
 
-static unsigned stream_grid(long long total) {
-  long long g = (total + 255) / 256;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  return static_cast<unsigned>(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 }  // namespace fgt
 
 using namespace fgt;
 
 extern "C" int fgt_plane_max(const float* x, int planes, long long plane_size, float* out, fgt_stream_t stream) {
   FGT_REQUIRE(x && out && planes >= 1 && plane_size >= 1, FGT_ERR_ARG, "plane_max: bad argument");
-  launch_k(plane_max_kernel, dim3(planes), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), x, plane_size, out);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(plane_max_kernel, dim3(planes), dim3(256), 0, stream, x, plane_size, out);
   return FGT_OK;
 }
 
@@ -130,9 +123,8 @@ extern "C" int fgt_window_gather(const float* frames, const unsigned char* masks
   FGT_REQUIRE(frames && masks && flows && fmax && ids && out_frames && out_flows && out_masks && t >= 1 && H >= 1 && W >= 1,
               FGT_ERR_ARG, "window_gather: bad argument");
   const long long HW = static_cast<long long>(H) * W;
-  launch_k(window_gather_kernel, dim3(stream_grid(t * HW)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), frames,
-           masks, flows, fmax, ids, t, HW, out_frames, out_flows, out_masks);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(window_gather_kernel, dim3(grid_stride(t * HW, 256)), dim3(256), 0, stream, frames, masks, flows, fmax,
+             ids, t, HW, out_frames, out_flows, out_masks);
   return FGT_OK;
 }
 
@@ -141,16 +133,13 @@ extern "C" int fgt_window_compose(const float* filled, const float* frames, cons
   FGT_REQUIRE(filled && frames && masks && ids && first && comp && k >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG,
               "window_compose: bad argument");
   const long long HW = static_cast<long long>(H) * W;
-  launch_k(window_compose_kernel, dim3(stream_grid(k * HW)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), filled,
-           frames, masks, ids, first, k, HW, comp);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(window_compose_kernel, dim3(grid_stride(k * HW, 256)), dim3(256), 0, stream, filled, frames, masks, ids,
+             first, k, HW, comp);
   return FGT_OK;
 }
 
 extern "C" int fgt_comp_to_u8(const float* comp, long long total, unsigned char* out, fgt_stream_t stream) {
   FGT_REQUIRE(comp && out && total >= 1, FGT_ERR_ARG, "comp_to_u8: bad argument");
-  launch_k(comp_to_u8_kernel, dim3(stream_grid(total)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), comp, total,
-           out);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(comp_to_u8_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, comp, total, out);
   return FGT_OK;
 }

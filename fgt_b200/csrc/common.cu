@@ -1,4 +1,4 @@
-// Error plumbing, device probing and TMA descriptor encoding (driver entry point fetched at run time,
+// Error plumbing, device probing, launch helpers and TMA descriptor encoding (driver entry point fetched at run time,
 // so the library links against the CUDA runtime only and loads on hosts without a driver).
 #include <stdlib.h>
 
@@ -8,7 +8,9 @@
 #include <stdarg.h>
 
 #include <mutex>
+#include <set>
 #include <unordered_map>
+#include <utility>
 
 namespace fgt {
 
@@ -161,6 +163,35 @@ int num_sms() {
     n = prop.multiProcessorCount;
   }
   return n;
+}
+
+int grid_stride(long long items, int block) {
+  const long long g = (items + block - 1) / block, cap = static_cast<long long>(num_sms()) * 16;
+  return static_cast<int>(g > cap ? cap : (g < 1 ? 1 : g));
+}
+
+int allow_dynamic_smem(const void* kernel, size_t bytes, const char* name) {
+  static std::mutex mu;
+  static std::set<std::pair<const void*, int>> done;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) {
+    std::lock_guard<std::mutex> lk(mu);
+    if (done.count({kernel, dev})) return FGT_OK;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) {
+      done.insert({kernel, dev});
+      return FGT_OK;
+    }
+  }
+  return set_err(FGT_ERR_CUDA, "%s: allowing %zu bytes of dynamic shared memory failed: %s", name, bytes,
+                 cudaGetErrorString(e));
+}
+
+int launch_failed(const char* name, cudaError_t e, dim3 grid, dim3 block, size_t smem) {
+  (void)cudaGetLastError();
+  return set_err(FGT_ERR_CUDA, "launching %s (grid %ux%ux%u, block %ux%ux%u, %zu bytes of shared memory) failed: %s",
+                 name, grid.x, grid.y, grid.z, block.x, block.y, block.z, smem, cudaGetErrorString(e));
 }
 
 }  // namespace fgt

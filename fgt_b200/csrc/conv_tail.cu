@@ -240,15 +240,9 @@ extern "C" int fgt_conv_tail(const void* x_hi, long long x_plane, int n, int H, 
   p.total_tiles = p.tiles_x * p.tiles_y * n;
   p.H = H; p.W = W; p.cout = cout; p.act = act; p.bias = bias; p.out = out;
   p.os_n = os_n; p.os_c = os_c; p.os_y = os_y; p.os_x = os_x;
-  static bool attr_set[2] = {false, false};
   auto kern = f16 ? conv_tail_kernel<true> : conv_tail_kernel<false>;
-  if (!attr_set[f16]) {
-    FGT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kTailSmem));
-    attr_set[f16] = true;
-  }
+  if (const int rc = allow_dynamic_smem(kern, kTailSmem, "conv_tail_kernel")) return rc;
   int grid = num_sms();
   if (grid > p.total_tiles) grid = p.total_tiles;
-  launch_k(kern, dim3(grid), dim3(kTailThreads), kTailSmem, reinterpret_cast<cudaStream_t>(stream), p);
-  FGT_CUDA(cudaGetLastError());
-  return FGT_OK;
+  return launch("conv_tail_kernel", kern, dim3(grid), dim3(kTailThreads), kTailSmem, stream, p);
 }

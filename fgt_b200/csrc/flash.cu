@@ -296,7 +296,7 @@ __global__ void __launch_bounds__(kFlashThreads, 1) flash_kernel(const __grid_co
   }
 }
 
-int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
+int attention_launch(const FgtAttnDesc& d, fgt_stream_t stream) {
   FGT_REQUIRE(d.head_dim == 128, FGT_ERR_ARG, "attention: head_dim=%d (only 128 supported)", d.head_dim);
   FGT_REQUIRE(d.batches >= 1 && d.heads >= 1 && d.Lq >= 1 && d.Lk >= 1, FGT_ERR_ARG, "attention: empty problem");
   FGT_REQUIRE(d.q_ld % 8 == 0 && d.k_ld % 8 == 0 && d.v_ld % 8 == 0 && d.out_ld % 8 == 0, FGT_ERR_ARG,
@@ -360,21 +360,15 @@ int attention_launch(const FgtAttnDesc& d, cudaStream_t stream) {
   p.out_ld = d.out_ld;
   p.out_rowmap = d.out_rowmap;
 
-  static bool attr_set[2] = {false, false};
   auto kern = f16 ? flash_kernel<true> : flash_kernel<false>;
-  if (!attr_set[f16]) {
-    FGT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kFlashSmem));
-    attr_set[f16] = true;
-  }
-  dim3 grid((d.Lq + 127) / 128, d.heads, d.batches);
-  launch_k(kern, dim3(grid), dim3(kFlashThreads), kFlashSmem, stream, p);
-  FGT_CUDA(cudaGetLastError());
-  return FGT_OK;
+  if (const int rc = allow_dynamic_smem(kern, kFlashSmem, "flash_kernel")) return rc;
+  const dim3 grid((d.Lq + 127) / 128, d.heads, d.batches);
+  return launch("flash_kernel", kern, grid, dim3(kFlashThreads), kFlashSmem, stream, p);
 }
 
 }  // namespace fgt
 
 extern "C" int fgt_attention(const FgtAttnDesc* desc, fgt_stream_t stream) {
   if (!desc) return fgt::set_err(FGT_ERR_ARG, "fgt_attention: null desc");
-  return fgt::attention_launch(*desc, reinterpret_cast<cudaStream_t>(stream));
+  return fgt::attention_launch(*desc, stream);
 }

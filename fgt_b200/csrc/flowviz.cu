@@ -157,13 +157,12 @@ extern "C" int fgt_flow_to_image(const float* flow, int B, int H, int W, int bgr
   const long long need = fgt_flow_to_image_workspace(B, H, W);
   FGT_REQUIRE(workspace_bytes >= need, FGT_ERR_ARG, "flow_to_image: workspace of %lld bytes, %lld needed",
               workspace_bytes, need);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const long long hw = static_cast<long long>(H) * W;
   const int parts = parts_of(hw);
   const float2* f2 = reinterpret_cast<const float2*>(flow);
   unsigned* ws = static_cast<unsigned*>(workspace);
-  FGT_CUDA(fgt::launch_k(flow_max_kernel, dim3(parts, B), dim3(kThreads), 0, s, f2, hw, ws));
-  FGT_CUDA(fgt::launch_k(flow_colour_kernel, dim3(static_cast<unsigned>((hw + kTile - 1) / kTile), B), dim3(kThreads),
-                         0, s, f2, hw, parts, static_cast<const unsigned*>(ws), bgr ? 1 : 0, out, maxima));
+  FGT_LAUNCH(flow_max_kernel, dim3(parts, B), dim3(kThreads), 0, stream, f2, hw, ws);
+  FGT_LAUNCH(flow_colour_kernel, dim3(static_cast<unsigned>((hw + kTile - 1) / kTile), B), dim3(kThreads), 0, stream,
+             f2, hw, parts, static_cast<const unsigned*>(ws), bgr ? 1 : 0, out, maxima);
   return FGT_OK;
 }

@@ -13,9 +13,6 @@
 #include "common.h"
 #include "ptx.cuh"
 
-#include <mutex>
-#include <unordered_set>
-
 namespace fgt {
 
 constexpr int kMaxAMaps = 18;  // 2 segments x up to 9 stride phases
@@ -617,7 +614,7 @@ static void* gemm_kernel_for(int n) {
   }
 }
 
-int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
+int gemm_tc_launch(const FgtGemmDesc& d, fgt_stream_t stream) {
   FGT_REQUIRE(d.num_segs >= 1 && d.num_segs <= 2, FGT_ERR_ARG, "gemm_tc: num_segs=%d", d.num_segs);
   FGT_REQUIRE(d.kx >= 1 && d.ky >= 1 && d.kz >= 1 && d.kx * d.ky * d.kz <= kMaxTaps, FGT_ERR_ARG,
               "gemm_tc: taps %dx%dx%d unsupported", d.kx, d.ky, d.kz);
@@ -786,29 +783,19 @@ int gemm_tc_launch(const FgtGemmDesc& d, cudaStream_t stream) {
                                                 : gemm_kernel_for<true, 0, false>(bn))
                                : (ext ? gemm_kernel_for<false, 1, false>(bn) : gemm_kernel_for<false, 0, false>(bn)));
   FGT_REQUIRE(kern, FGT_ERR_ARG, "gemm_tc: no instantiation for a %d-wide tile", bn);
-  // raised once per instantiation: the attribute is per kernel
-  static std::mutex attr_mu;
-  static std::unordered_set<void*> attr_done;
-  {
-    std::lock_guard<std::mutex> lk(attr_mu);
-    if (!attr_done.count(kern)) {
-      FGT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_done.insert(kern);
-    }
-  }
+  if (const int rc = allow_dynamic_smem(kern, 227 * 1024, "gemm_tc_kernel")) return rc;
   int grid = num_sms();
   if (grid > p.total_tiles) grid = p.total_tiles;
   FGT_REQUIRE(grid >= 1, FGT_ERR_ARG, "gemm_tc: empty problem");
-  launch_k(reinterpret_cast<void (*)(GemmParams)>(kern), dim3(grid), dim3(kGemmThreads), smem, stream, p);
-  FGT_CUDA(cudaGetLastError());
-  return FGT_OK;
+  return launch("gemm_tc_kernel", reinterpret_cast<void (*)(GemmParams)>(kern), dim3(grid), dim3(kGemmThreads), smem,
+                stream, p);
 }
 
 }  // namespace fgt
 
 extern "C" int fgt_gemm_tc(const FgtGemmDesc* desc, fgt_stream_t stream) {
   if (!desc) return fgt::set_err(FGT_ERR_ARG, "fgt_gemm_tc: null desc");
-  return fgt::gemm_tc_launch(*desc, reinterpret_cast<cudaStream_t>(stream));
+  return fgt::gemm_tc_launch(*desc, stream);
 }
 
 // Debugging aid (not part of the product interface): bit 0 forces per-element epilogue stores, bit 1 per-element aux

@@ -495,14 +495,11 @@ extern "C" int fgt_inpaint_telea_plan(const unsigned char* masks, int n_masks, i
   int rc = telea_check(H, W, 1, radius, &range);
   if (rc == FGT_OK) rc = ws_check(n_masks, H, W, workspace_bytes);
   if (rc != FGT_OK) return rc;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   char* ws = static_cast<char*>(workspace);
   const size_t stride = plan_bytes(H, W);
-  fgt::launch_k(march_kernel, dim3(n_masks), dim3(256), 0, s, masks, static_cast<long long>(H) * W, H, W, range, ws,
-                stride);
-  FGT_CUDA(cudaGetLastError());
-  fgt::launch_k(levels_kernel, dim3(n_masks), dim3(32), 0, s, H, W, range, ws, stride);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(march_kernel, dim3(n_masks), dim3(256), 0, stream, masks, static_cast<long long>(H) * W, H, W, range, ws,
+             stride);
+  FGT_LAUNCH(levels_kernel, dim3(n_masks), dim3(32), 0, stream, H, W, range, ws, stride);
   return FGT_OK;
 }
 
@@ -515,9 +512,8 @@ extern "C" int fgt_inpaint_telea_fill(const unsigned char* images, int B, int H,
   int rc = telea_check(H, W, C, radius, &range);
   if (rc == FGT_OK) rc = ws_check(shared_plan ? 1 : B, H, W, workspace_bytes);
   if (rc != FGT_OK) return rc;
-  fgt::launch_k(fill_kernel, dim3(B), dim3(512), 0, reinterpret_cast<cudaStream_t>(stream), images, out, H, W, C, range,
-                static_cast<const char*>(workspace), plan_bytes(H, W), shared_plan ? 1 : 0);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(fill_kernel, dim3(B), dim3(512), 0, stream, images, out, H, W, C, range,
+             static_cast<const char*>(workspace), plan_bytes(H, W), shared_plan ? 1 : 0);
   return FGT_OK;
 }
 
@@ -560,11 +556,7 @@ extern "C" int fgt_grad_prep_pre(const float* video, const unsigned char* mask, 
                                  fgt_stream_t stream) {
   FGT_REQUIRE(video && mask && u8 && B >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "grad_prep_pre: bad argument");
   const long long n = static_cast<long long>(B) * H * W;
-  long long g = (n * 3 + 255) / 256;
-  if (g > fgt::num_sms() * 16LL) g = fgt::num_sms() * 16LL;
-  fgt::launch_k(grad_pre_kernel, dim3(static_cast<unsigned>(g)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                video, mask, u8, n);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(grad_pre_kernel, dim3(fgt::grid_stride(n * 3, 256)), dim3(256), 0, stream, video, mask, u8, n);
   return FGT_OK;
 }
 
@@ -572,10 +564,6 @@ extern "C" int fgt_grad_prep_post(const unsigned char* u8, const unsigned char* 
                                   float* gy, fgt_stream_t stream) {
   FGT_REQUIRE(u8 && mask_dilated && gx && gy && B >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "grad_prep_post: bad argument");
   const long long n = static_cast<long long>(B) * H * W * 3;
-  long long g = (n + 255) / 256;
-  if (g > fgt::num_sms() * 16LL) g = fgt::num_sms() * 16LL;
-  fgt::launch_k(grad_post_kernel, dim3(static_cast<unsigned>(g)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                u8, mask_dilated, B, H, W, gx, gy);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(grad_post_kernel, dim3(fgt::grid_stride(n, 256)), dim3(256), 0, stream, u8, mask_dilated, B, H, W, gx, gy);
   return FGT_OK;
 }

@@ -145,9 +145,7 @@ static dim3 lap_grid(int B, int H, int W) {
 extern "C" int fgt_regionfill_init(const double* img, const unsigned char* mask, int B, int H, int W, double* x,
                                    double* r, double* p, double* rr, fgt_stream_t stream) {
   FGT_REQUIRE(img && mask && x && r && p && rr && B >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "regionfill_init: bad argument");
-  launch_k(lap_init_kernel, lap_grid(B, H, W), dim3(kLapThreads), 0, reinterpret_cast<cudaStream_t>(stream), img, mask,
-           H, W, x, r, p, rr);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(lap_init_kernel, lap_grid(B, H, W), dim3(kLapThreads), 0, stream, img, mask, H, W, x, r, p, rr);
   return FGT_OK;
 }
 
@@ -156,27 +154,21 @@ extern "C" int fgt_regionfill_iters(const unsigned char* mask, int B, int H, int
                                     fgt_stream_t stream) {
   FGT_REQUIRE(mask && x && r && p0 && p1 && ap && rr && pap && B >= 1 && k0 >= 0 && iters >= 1, FGT_ERR_ARG,
               "regionfill_iters: bad argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const dim3 grid = lap_grid(B, H, W);
   for (int k = k0; k < k0 + iters; ++k) {
     double* p_old = (k & 1) ? p1 : p0;  // iteration k reads the direction written by iteration k-1
     double* p_new = (k & 1) ? p0 : p1;
-    launch_k(lap_dir_kernel, grid, dim3(kLapThreads), 0, st, mask, B, H, W, static_cast<const double*>(r),
-             static_cast<const double*>(p_old), p_new, ap, static_cast<const double*>(rr), pap, k);
-    launch_k(lap_update_kernel, grid, dim3(kLapThreads), 0, st, mask, B, H, W, static_cast<const double*>(p_new),
-             static_cast<const double*>(ap), x, r, rr, static_cast<const double*>(pap), k);
+    FGT_LAUNCH(lap_dir_kernel, grid, dim3(kLapThreads), 0, stream, mask, B, H, W, static_cast<const double*>(r),
+               static_cast<const double*>(p_old), p_new, ap, static_cast<const double*>(rr), pap, k);
+    FGT_LAUNCH(lap_update_kernel, grid, dim3(kLapThreads), 0, stream, mask, B, H, W, static_cast<const double*>(p_new),
+               static_cast<const double*>(ap), x, r, rr, static_cast<const double*>(pap), k);
   }
-  FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }
 
 extern "C" int fgt_regionfill_finish(const double* img, const unsigned char* mask, long long total, const double* x,
                                      double* out, fgt_stream_t stream) {
   FGT_REQUIRE(img && mask && x && out && total >= 1, FGT_ERR_ARG, "regionfill_finish: bad argument");
-  long long g = (total + 255) / 256;
-  if (g > num_sms() * 16) g = num_sms() * 16;
-  launch_k(lap_finish_kernel, dim3(static_cast<unsigned>(g)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), img,
-           mask, total, x, out);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(lap_finish_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, img, mask, total, x, out);
   return FGT_OK;
 }

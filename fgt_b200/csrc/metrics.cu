@@ -222,13 +222,12 @@ inline Gauss gaussian() {
 }
 
 template <typename TA, typename TB>
-cudaError_t launch_tiles(const void* a, const void* b, int N, int H, int W, int C, double* ws, cudaStream_t s) {
+int launch_tiles(const void* a, const void* b, int N, int H, int W, int C, double* ws, fgt_stream_t s) {
   auto kern = metrics_tile_kernel<TA, TB>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmem));
-  if (e != cudaSuccess) return e;
+  if (const int rc = allow_dynamic_smem(kern, kSmem, "metrics_tile_kernel")) return rc;
   const dim3 grid((W - 2 * kR + kTX - 1) / kTX, (H - 2 * kR + kTY - 1) / kTY, N * C);
-  return launch_k(kern, grid, dim3(kThreads), kSmem, s, static_cast<const TA*>(a), static_cast<const TB*>(b), H, W, C,
-                  gaussian(), ws);
+  return launch("metrics_tile_kernel", kern, grid, dim3(kThreads), kSmem, s, static_cast<const TA*>(a),
+                static_cast<const TB*>(b), H, W, C, gaussian(), ws);
 }
 
 inline long long tiles_of(int H, int W) {
@@ -269,15 +268,15 @@ extern "C" int fgt_metrics(const void* a, int a_dtype, const void* b, int b_dtyp
   const long long need = fgt_metrics_workspace(N, H, W, C);
   FGT_REQUIRE(workspace_bytes >= need, FGT_ERR_ARG, "metrics: workspace of %lld bytes, %lld needed", workspace_bytes,
               need);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   double* ws = static_cast<double*>(workspace);
   const bool fa = a_dtype == FGT_METRIC_F32, fb = b_dtype == FGT_METRIC_F32;
-  if (fa && fb) FGT_CUDA((launch_tiles<float, float>(a, b, N, H, W, C, ws, s)));
-  else if (fa) FGT_CUDA((launch_tiles<float, uint8_t>(a, b, N, H, W, C, ws, s)));
-  else if (fb) FGT_CUDA((launch_tiles<uint8_t, float>(a, b, N, H, W, C, ws, s)));
-  else FGT_CUDA((launch_tiles<uint8_t, uint8_t>(a, b, N, H, W, C, ws, s)));
+  if (fa && fb) rc = launch_tiles<float, float>(a, b, N, H, W, C, ws, stream);
+  else if (fa) rc = launch_tiles<float, uint8_t>(a, b, N, H, W, C, ws, stream);
+  else if (fb) rc = launch_tiles<uint8_t, float>(a, b, N, H, W, C, ws, stream);
+  else rc = launch_tiles<uint8_t, uint8_t>(a, b, N, H, W, C, ws, stream);
+  if (rc != FGT_OK) return rc;
   constexpr int kWarps = 4;
-  FGT_CUDA(fgt::launch_k(metrics_reduce_kernel, dim3((N + kWarps - 1) / kWarps), dim3(32 * kWarps), 0, s, ws, N, H, W,
-                         C, static_cast<int>(tiles_of(H, W)), out, ssim_c));
+  FGT_LAUNCH(metrics_reduce_kernel, dim3((N + kWarps - 1) / kWarps), dim3(32 * kWarps), 0, stream, ws, N, H, W, C,
+             static_cast<int>(tiles_of(H, W)), out, ssim_c);
   return FGT_OK;
 }

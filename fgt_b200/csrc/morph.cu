@@ -202,13 +202,6 @@ __global__ void resize_bilinear_f32_kernel(const float* __restrict__ in, float* 
   }
 }
 
-static int morph_grid(long long items, int block) {
-  long long g = (items + block - 1) / block;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  return static_cast<int>(g < 1 ? 1 : g);
-}
-
 }  // namespace fgt
 
 using namespace fgt;
@@ -218,42 +211,37 @@ extern "C" int fgt_binary_dilate(const unsigned char* in, int B, int H, int W, i
   FGT_REQUIRE(in && tmp && out && B >= 1 && H >= 1 && W >= 1 && iterations >= 1, FGT_ERR_ARG, "binary_dilate: bad argument");
   FGT_REQUIRE(in != out && in != tmp && tmp != out, FGT_ERR_ARG, "binary_dilate: buffers must not alias");
   const long long total = static_cast<long long>(B) * H * W;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   // ping-pong so that the last pass lands in `out`
   const unsigned char* src = in;
   for (int it = 0; it < iterations; ++it) {
     unsigned char* dst = ((iterations - 1 - it) % 2 == 0) ? out : tmp;
-    launch_k(dilate_cross_kernel, dim3(morph_grid(total, 256)), dim3(256), 0, s, src, dst, B, H, W);
+    FGT_LAUNCH(dilate_cross_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, src, dst, B, H, W);
     src = dst;
   }
-  FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }
 
 extern "C" int fgt_fill_holes_init(const unsigned char* fg, int B, int H, int W, unsigned char* reach, fgt_stream_t stream) {
   FGT_REQUIRE(fg && reach && B >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "fill_holes: bad argument");
-  FGT_CUDA(cudaMemsetAsync(reach, 0, static_cast<size_t>(B) * H * W, reinterpret_cast<cudaStream_t>(stream)));
+  FGT_CUDA(cudaMemsetAsync(reach, 0, static_cast<size_t>(B) * H * W, stream));
   return FGT_OK;
 }
 
 extern "C" int fgt_fill_holes_pass(const unsigned char* fg, int B, int H, int W, unsigned char* reach, int* changed,
                                    int passes, fgt_stream_t stream) {
   FGT_REQUIRE(fg && reach && changed && passes >= 1, FGT_ERR_ARG, "fill_holes: bad argument");
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  FGT_CUDA(cudaMemsetAsync(changed, 0, sizeof(int), s));
+  FGT_CUDA(cudaMemsetAsync(changed, 0, sizeof(int), stream));
   for (int p = 0; p < passes; ++p) {
-    launch_k(fill_rows_kernel, dim3((B * H + 63) / 64), dim3(64), 0, s, fg, reach, B, H, W, changed);
-    launch_k(fill_cols_kernel, dim3((B * W + 63) / 64), dim3(64), 0, s, fg, reach, B, H, W, changed);
+    FGT_LAUNCH(fill_rows_kernel, dim3((B * H + 63) / 64), dim3(64), 0, stream, fg, reach, B, H, W, changed);
+    FGT_LAUNCH(fill_cols_kernel, dim3((B * W + 63) / 64), dim3(64), 0, stream, fg, reach, B, H, W, changed);
   }
-  FGT_CUDA(cudaGetLastError());
   return FGT_OK;
 }
 
 extern "C" int fgt_fill_holes_finish(const unsigned char* reach, int B, int H, int W, unsigned char* out, fgt_stream_t stream) {
   FGT_REQUIRE(reach && out, FGT_ERR_ARG, "fill_holes: bad argument");
   const long long total = static_cast<long long>(B) * H * W;
-  launch_k(fill_finish_kernel, dim3(morph_grid(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), reach, out, total);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(fill_finish_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, reach, out, total);
   return FGT_OK;
 }
 
@@ -261,8 +249,8 @@ extern "C" int fgt_resize_nearest_u8(const unsigned char* in, int B, int H, int 
                                      fgt_stream_t stream) {
   FGT_REQUIRE(in && out && B >= 1 && H >= 1 && W >= 1 && C >= 1 && OH >= 1 && OW >= 1, FGT_ERR_ARG, "resize_nearest: bad argument");
   const long long total = static_cast<long long>(B) * OH * OW * C;
-  launch_k(resize_nearest_u8_kernel, dim3(morph_grid(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), in, out, B, H, W, C, OH, OW);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(resize_nearest_u8_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, in, out, B, H, W, C, OH,
+             OW);
   return FGT_OK;
 }
 
@@ -270,8 +258,7 @@ extern "C" int fgt_resize_bilinear_f32(const float* in, int B, int H, int W, int
                                        float scale_c1, float* out, fgt_stream_t stream) {
   FGT_REQUIRE(in && out && B >= 1 && H >= 1 && W >= 1 && C >= 1 && OH >= 1 && OW >= 1, FGT_ERR_ARG, "resize_bilinear: bad argument");
   const long long total = static_cast<long long>(B) * OH * OW * C;
-  launch_k(resize_bilinear_f32_kernel, dim3(morph_grid(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), in, out, B, H, W, C, OH,
-           OW, nchw, scale_c0, scale_c1);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(resize_bilinear_f32_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, in, out, B, H, W, C, OH,
+             OW, nchw, scale_c0, scale_c1);
   return FGT_OK;
 }

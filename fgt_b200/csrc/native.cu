@@ -91,13 +91,6 @@ __global__ void composite_kernel(const uint8_t* __restrict__ comp, int cH, int c
   }
 }
 
-inline int grid_for(long long items, int block) {
-  long long g = (items + block - 1) / block;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  return static_cast<int>(g < 1 ? 1 : g);
-}
-
 // Workspace: the uint16 counts of n_masks masks, then the uint8 row sums they are built from.
 inline long long counts_bytes(int n_masks, int H, int W) { return 2LL * n_masks * H * W; }
 
@@ -127,12 +120,11 @@ extern "C" int fgt_native_count(const unsigned char* dilated, int n_masks, int H
   const long long need = fgt_native_workspace(n_masks, H, W, k);
   FGT_REQUIRE(workspace_bytes >= need, FGT_ERR_ARG, "native_count: workspace of %lld bytes, %lld needed", workspace_bytes,
               need);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const long long total = static_cast<long long>(n_masks) * H * W;
   uint16_t* c = static_cast<uint16_t*>(workspace);
   uint8_t* rs = static_cast<uint8_t*>(workspace) + counts_bytes(n_masks, H, W);
-  FGT_CUDA(fgt::launch_k(count_rows_kernel, dim3(grid_for(total, 256)), dim3(256), 0, s, dilated, rs, total, W, k));
-  FGT_CUDA(fgt::launch_k(count_cols_kernel, dim3(grid_for(total, 256)), dim3(256), 0, s, rs, c, total, H, W, k));
+  FGT_LAUNCH(count_rows_kernel, dim3(fgt::grid_stride(total, 256)), dim3(256), 0, stream, dilated, rs, total, W, k);
+  FGT_LAUNCH(count_cols_kernel, dim3(fgt::grid_stride(total, 256)), dim3(256), 0, stream, rs, c, total, H, W, k);
   return FGT_OK;
 }
 
@@ -153,8 +145,8 @@ extern "C" int fgt_native_composite(const unsigned char* comp, int B, int cH, in
   FGT_REQUIRE(workspace_bytes >= need, FGT_ERR_ARG, "native_composite: workspace of %lld bytes, %lld needed",
               workspace_bytes, need);
   const long long total = static_cast<long long>(B) * H * W;
-  FGT_CUDA(fgt::launch_k(composite_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                         comp, cH, cW, frames, B, H, W, static_cast<const uint16_t*>(workspace),
-                         shared_mask ? 0LL : static_cast<long long>(H) * W, (2 * k + 1) * (2 * k + 1), out));
+  FGT_LAUNCH(composite_kernel, dim3(fgt::grid_stride(total, 256)), dim3(256), 0, stream, comp, cH, cW, frames, B, H, W,
+             static_cast<const uint16_t*>(workspace), shared_mask ? 0LL : static_cast<long long>(H) * W,
+             (2 * k + 1) * (2 * k + 1), out);
   return FGT_OK;
 }

@@ -104,8 +104,6 @@ extern "C" int fgt_peer_barrier(void* const* flags_host, int n, int rank, void* 
   pf.n = n;
   pf.rank = rank;
   for (int q = 0; q < n; ++q) FGT_REQUIRE(pf.flags[q], FGT_ERR_ARG, "peer_barrier: flags[%d] is NULL", q);
-  launch_k(peer_barrier_kernel, dim3(1), dim3(32), 0, reinterpret_cast<cudaStream_t>(stream), 
-      pf, reinterpret_cast<unsigned long long*>(epoch_ctr));
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(peer_barrier_kernel, dim3(1), dim3(32), 0, stream, pf, reinterpret_cast<unsigned long long*>(epoch_ctr));
   return FGT_OK;
 }

@@ -489,24 +489,23 @@ extern "C" int fgt_poisson_setup(const double* trg, const double* gx, const doub
   FGT_REQUIRE(trg && gx && gy && hole && code && u && bb && list && cnt && F >= 1 && H >= 2 && W >= 2, FGT_ERR_ARG,
               "poisson_setup: bad argument");
   FGT_REQUIRE(static_cast<long long>(H) * W < (1LL << 24), FGT_ERR_ARG, "poisson_setup: H*W must be below 2^24");
-  launch_k(psn_setup_kernel, psn_grid(F, H, W), dim3(kPsnThreads), 0, reinterpret_cast<cudaStream_t>(stream), trg, gx,
-           gy, hole, gmask, edge, H, W, F * kPsnC, code, u, bb, list, cnt);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(psn_setup_kernel, psn_grid(F, H, W), dim3(kPsnThreads), 0, stream, trg, gx, gy, hole, gmask, edge, H, W,
+             F * kPsnC, code, u, bb, list, cnt);
   return FGT_OK;
 }
 
 static int psn_enqueue(const unsigned* list, int max_cnt, int F, int H, int W, double* u, double* v, double* w, double* x,
                        double* bb, double* aa, double* ww, double* state, int* kctr, int iters, double atol, double btol,
-                       double conlim, int iter_lim, cudaStream_t st) {
+                       double conlim, int iter_lim, fgt_stream_t st) {
   // one block column even when no pixel owns an equation: block 0 of every frame carries the scalar state
   const dim3 grid(max_cnt > 0 ? (max_cnt + kPsnThreads - 1) / kPsnThreads : 1, F);
   const int S = F * kPsnC;
   const double ctol = conlim > 0.0 ? 1.0 / conlim : 0.0;
   for (int it = 0; it < iters; ++it) {
-    FGT_CUDA(launch_k(psn_v_kernel, grid, dim3(kPsnThreads), 0, st, list, H, W, S, static_cast<const double*>(u), v,
-                      static_cast<const double*>(bb), aa, static_cast<const double*>(state), kctr));
-    FGT_CUDA(launch_k(psn_ux_kernel, grid, dim3(kPsnThreads), 0, st, list, H, W, S, u, static_cast<const double*>(v), w, x,
-                      bb, static_cast<const double*>(aa), ww, state, kctr, atol, btol, ctol, iter_lim));
+    FGT_LAUNCH(psn_v_kernel, grid, dim3(kPsnThreads), 0, st, list, H, W, S, static_cast<const double*>(u), v,
+               static_cast<const double*>(bb), aa, static_cast<const double*>(state), kctr);
+    FGT_LAUNCH(psn_ux_kernel, grid, dim3(kPsnThreads), 0, st, list, H, W, S, u, static_cast<const double*>(v), w, x, bb,
+               static_cast<const double*>(aa), ww, state, kctr, atol, btol, ctol, iter_lim);
   }
   return FGT_OK;
 }
@@ -518,11 +517,8 @@ extern "C" int fgt_poisson_iters(const unsigned* list, int max_cnt, int F, int H
                                  double* x, double* bb, double* aa, double* ww, double* state, int* kctr, int iters,
                                  double atol, double btol, double conlim, int iter_lim, fgt_stream_t stream) {
   FGT_REQUIRE(PSN_ITER_ARGS_OK, FGT_ERR_ARG, "poisson_iters: bad argument");
-  const int rc = psn_enqueue(list, max_cnt, F, H, W, u, v, w, x, bb, aa, ww, state, kctr, iters, atol, btol, conlim,
-                             iter_lim, reinterpret_cast<cudaStream_t>(stream));
-  if (rc != FGT_OK) return rc;
-  FGT_CUDA(cudaGetLastError());
-  return FGT_OK;
+  return psn_enqueue(list, max_cnt, F, H, W, u, v, w, x, bb, aa, ww, state, kctr, iters, atol, btol, conlim, iter_lim,
+                     stream);
 }
 
 // The same `iters` iteration pairs captured once into an executable CUDA graph (the iteration index is on the
@@ -554,7 +550,7 @@ extern "C" int fgt_poisson_graph_create(const unsigned* list, int max_cnt, int F
 
 extern "C" int fgt_poisson_graph_launch(void* exec, fgt_stream_t stream) {
   FGT_REQUIRE(exec, FGT_ERR_ARG, "poisson_graph_launch: null graph");
-  FGT_CUDA(cudaGraphLaunch(reinterpret_cast<cudaGraphExec_t>(exec), reinterpret_cast<cudaStream_t>(stream)));
+  FGT_CUDA(cudaGraphLaunch(reinterpret_cast<cudaGraphExec_t>(exec), stream));
   return FGT_OK;
 }
 
@@ -566,21 +562,17 @@ extern "C" int fgt_poisson_graph_destroy(void* exec) {
 extern "C" int fgt_poisson_unfilled(const unsigned char* hole, const unsigned char* gmask, int F, int H, int W,
                                     unsigned char* clr, fgt_stream_t stream) {
   FGT_REQUIRE(hole && clr && F >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG, "poisson_unfilled: bad argument");
-  launch_k(psn_sweep_kernel, dim3(F, 2), dim3(32), 0, reinterpret_cast<cudaStream_t>(stream), hole, gmask, F, H, W,
-           clr);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(psn_sweep_kernel, dim3(F, 2), dim3(32), 0, stream, hole, gmask, F, H, W, clr);
   return FGT_OK;
 }
 
 extern "C" int fgt_poisson_finish(const double* trg, const unsigned char* hole, const double* x, int F, int H, int W,
                                   double* out, const unsigned char* clr, unsigned char* unf, fgt_stream_t stream) {
-  FGT_REQUIRE(trg && hole && x && out && F >= 1 && (!unf || clr), FGT_ERR_ARG, "poisson_finish: bad argument");
+  FGT_REQUIRE(trg && hole && x && out && F >= 1 && H >= 1 && W >= 1 && (!unf || clr), FGT_ERR_ARG,
+              "poisson_finish: bad argument");
   const long long pixels = static_cast<long long>(F) * H * W;
-  long long g = (pixels + 255) / 256;
-  if (g > num_sms() * 16) g = num_sms() * 16;
-  launch_k(psn_finish_kernel, dim3(static_cast<unsigned>(g)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), trg,
-           hole, x, pixels, out, clr, unf);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(psn_finish_kernel, dim3(grid_stride(pixels, 256)), dim3(256), 0, stream, trg, hole, x, pixels, out, clr,
+             unf);
   return FGT_OK;
 }
 

@@ -144,12 +144,6 @@ __global__ void prop_fuse_kernel(const uint8_t* __restrict__ mask, const uint8_t
   }
 }
 
-static int grid1(long long n, int block) {
-  long long g = (n + block - 1) / block;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  return static_cast<int>(g > cap ? cap : (g < 1 ? 1 : g));
-}
-
 }  // namespace fgt
 
 using namespace fgt;
@@ -158,18 +152,16 @@ extern "C" int fgt_prop_step(const uint8_t* mask, const float* flow_step, const 
                              int tn, double thres, double* nn_y, double* nn_x, int* nn_t, uint8_t* have, double* cuv,
                              fgt_stream_t stream) {
   FGT_REQUIRE(mask && flow_step && flow_back && nn_y && nn_x && nn_t && have && cuv, FGT_ERR_ARG, "prop_step: null");
-  launch_k(prop_step_kernel, dim3(grid1(static_cast<long long>(H) * W, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      mask, flow_step, flow_back, H, W, t, tn, thres, nn_y, nn_x, nn_t, have, cuv);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(prop_step_kernel, dim3(grid_stride(static_cast<long long>(H) * W, 256)), dim3(256), 0, stream, mask,
+             flow_step, flow_back, H, W, t, tn, thres, nn_y, nn_x, nn_t, have, cuv);
   return FGT_OK;
 }
 
 extern "C" int fgt_prop_gather(const uint8_t* mask, const double* nn_y, const double* nn_x, const int* nn_t, int N,
                                int H, int W, int s, float* gx, float* gy, fgt_stream_t stream) {
   FGT_REQUIRE(mask && nn_y && nn_x && nn_t && gx && gy, FGT_ERR_ARG, "prop_gather: null");
-  launch_k(prop_gather_kernel, dim3(grid1(static_cast<long long>(N) * H * W, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      mask, nn_y, nn_x, nn_t, N, H, W, s, gx, gy);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(prop_gather_kernel, dim3(grid_stride(static_cast<long long>(N) * H * W, 256)), dim3(256), 0, stream, mask,
+             nn_y, nn_x, nn_t, N, H, W, s, gx, gy);
   return FGT_OK;
 }
 
@@ -179,8 +171,7 @@ extern "C" int fgt_prop_fuse(const uint8_t* mask, const uint8_t* have0, const ui
                              uint8_t* tofill, fgt_stream_t stream) {
   FGT_REQUIRE(mask && have0 && have1 && cuv0 && cuv1 && gx && gy && tofill, FGT_ERR_ARG, "prop_fuse: null");
   const long long total = static_cast<long long>(N) * H * W;
-  launch_k(prop_fuse_kernel, dim3(grid1(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      mask, have0, have1, cuv0, cuv1, total, alpha, gx_bn, gy_bn, gx_fn, gy_fn, gx, gy, tofill);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(prop_fuse_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, mask, have0, have1, cuv0, cuv1,
+             total, alpha, gx_bn, gy_bn, gx_fn, gy_fn, gx, gy, tofill);
   return FGT_OK;
 }

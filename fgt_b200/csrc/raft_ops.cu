@@ -8,14 +8,6 @@
 
 namespace fgt {
 
-static int grid_cap(long long work_items, int block) {
-  long long g = (work_items + block - 1) / block;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
-}
-
 // ------------------------------------------------------------------------------------------
 // per-(image, channel) sum and sum of squares of an NHWC fp32 tensor (nn.InstanceNorm2d statistics,
 // RAFT/extractor.py:29-33,131-132). Block = 256 threads covering `C` channels x row slices; fp32
@@ -299,8 +291,7 @@ using namespace fgt;
 
 extern "C" int fgt_chan_stats(const float* x, int n, int HW, int C, double* stats, fgt_stream_t stream) {
   FGT_REQUIRE(x && stats && C >= 1 && C <= 256, FGT_ERR_ARG, "chan_stats: C=%d", C);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FGT_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * n * C, st));
+  FGT_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * n * C, stream));
   // about two blocks per SM over all images; each block reduces its rows in shared memory first
   int blocks_x = (2 * num_sms() + n - 1) / n;
   const int rstep = 512 / C;
@@ -308,8 +299,7 @@ extern "C" int fgt_chan_stats(const float* x, int n, int HW, int C, double* stat
   rows_per_block = ((rows_per_block + rstep - 1) / rstep) * rstep;
   if (rows_per_block < 8 * rstep) rows_per_block = 8 * rstep;
   dim3 grid((HW + rows_per_block - 1) / rows_per_block, n);
-  launch_k(chan_stats_kernel, dim3(grid), dim3(512), 0, st, x, HW, C, rows_per_block, stats);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(chan_stats_kernel, dim3(grid), dim3(512), 0, stream, x, HW, C, rows_per_block, stats);
   return FGT_OK;
 }
 
@@ -320,18 +310,16 @@ extern "C" int fgt_instnorm_act(const float* x, const double* stats, int n, int 
   FGT_REQUIRE(C <= 256, FGT_ERR_ARG, "instnorm_act: C=%d > 256", C);
   if (const int rc = check_act16("instnorm_act", out_hi, out_plane, 4, true)) return rc;
   const long long total = static_cast<long long>(HW) * (C / 4);
-  const dim3 grid(grid_cap(total, 256), n);
-  launch_k(instnorm_act_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      x, stats, HW, C, eps, relu, res, out, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  const dim3 grid(grid_stride(total, 256), n);
+  FGT_LAUNCH(instnorm_act_kernel, dim3(grid), dim3(256), 0, stream, x, stats, HW, C, eps, relu, res, out,
+             reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
 extern "C" int fgt_avgpool2(const float* in, long long rows, int h, int w, float* out, fgt_stream_t stream) {
   FGT_REQUIRE(in && out && h >= 2 && w >= 2, FGT_ERR_ARG, "avgpool2: %dx%d", h, w);
   const long long total = rows * (h / 2) * (w / 2);
-  launch_k(avgpool2_kernel, dim3(grid_cap(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), in, rows, h, w, out);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(avgpool2_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, in, rows, h, w, out);
   return FGT_OK;
 }
 
@@ -352,9 +340,8 @@ extern "C" int fgt_corr_lookup(const float* const* level_ptrs_host, const int* l
   const int block = 256;
   const size_t smem = (block / 32) * (win + 1) * (win + 1) * sizeof(float);
   const long long items = static_cast<long long>(n_pix) * levels;
-  launch_k(corr_lookup_kernel, dim3(grid_cap(items * 32, block)), dim3(block), smem, reinterpret_cast<cudaStream_t>(stream), 
-      lv, levels, radius, coords, n_pix, out_pitch, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(corr_lookup_kernel, dim3(grid_stride(items * 32, block)), dim3(block), smem, stream, lv, levels, radius,
+             coords, n_pix, out_pitch, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -364,9 +351,9 @@ extern "C" int fgt_raft_flow_update(float* coords, const float* delta, int delta
   FGT_REQUIRE(coords && flow_nchw && n >= 1, FGT_ERR_ARG, "raft_flow_update: null argument");
   FGT_REQUIRE(delta_f16 == 0 || delta_f16 == 1, FGT_ERR_ARG, "raft_flow_update: delta_f16=%d (0 or 1)", delta_f16);
   if (const int rc = check_act16("raft_flow_update", x_hi, x_plane, 1, true)) return rc;
-  launch_k(flow_update_kernel, dim3(grid_cap(static_cast<long long>(n) * h * w, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      coords, delta, delta_f16, n, h, w, flow_nchw, reinterpret_cast<__nv_bfloat16*>(x_hi), x_plane, x_pitch, x_chan);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(flow_update_kernel, dim3(grid_stride(static_cast<long long>(n) * h * w, 256)), dim3(256), 0, stream,
+             coords, delta, delta_f16, n, h, w, flow_nchw, reinterpret_cast<__nv_bfloat16*>(x_hi), x_plane, x_pitch,
+             x_chan);
   return FGT_OK;
 }
 
@@ -375,9 +362,8 @@ extern "C" int fgt_f16_to_split(const void* src, long long n, void* out_hi, long
               FGT_ERR_ARG, "f16_to_split: n=%lld plane=%lld (multiples of 8, 16-byte aligned buffers)", n, out_plane);
   if (const int rc = check_act16("f16_to_split", out_hi, out_plane, 8, false)) return rc;
   if (n == 0) return FGT_OK;
-  launch_k(f16_to_split_kernel, dim3(grid_cap(n / 8, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-      reinterpret_cast<const __half*>(src), n / 8, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(f16_to_split_kernel, dim3(grid_stride(n / 8, 256)), dim3(256), 0, stream,
+             reinterpret_cast<const __half*>(src), n / 8, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -385,8 +371,7 @@ extern "C" int fgt_convex_upsample(const float* mask, const float* flow_nchw, in
                                    fgt_stream_t stream) {
   FGT_REQUIRE(mask && flow_nchw && out && n >= 1, FGT_ERR_ARG, "convex_upsample: null argument");
   const long long total = static_cast<long long>(n) * h * w * 64;
-  launch_k(convex_upsample_kernel, dim3(grid_cap(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      mask, flow_nchw, n, h, w, out);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(convex_upsample_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, mask, flow_nchw, n, h, w,
+             out);
   return FGT_OK;
 }

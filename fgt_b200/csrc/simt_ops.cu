@@ -475,14 +475,6 @@ __global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ in, long lon
   }
 }
 
-static int grid_for(long long work_items, int block) {
-  long long g = (work_items + block - 1) / block;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
-}
-
 }  // namespace fgt
 
 using namespace fgt;
@@ -493,9 +485,8 @@ extern "C" int fgt_pack_nchw(const float* src0, int c0, const float* src1, int c
               "pack_nchw: c0=%d c1=%d cpad=%d", c0, c1, cpad);
   if (const int rc = check_act16("pack_nchw", out_hi, out_plane, 1, false)) return rc;
   const long long total = static_cast<long long>(n) * (H + 2 * pad) * (W + 2 * pad);
-  launch_k(pack_nchw_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      src0, c0, src1, c1, n, H, W, pad, cpad, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(pack_nchw_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, src0, c0, src1, c1, n, H, W, pad,
+             cpad, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -511,15 +502,9 @@ extern "C" int fgt_im2col_nchw(const float* src0, int c0, const float* src1, int
   constexpr size_t kIm2colSmemMax = 160 * 1024;
   FGT_REQUIRE(smem <= kIm2colSmemMax, FGT_ERR_ARG, "im2col_nchw: %zu bytes of staged input rows exceed %zu", smem, kIm2colSmemMax);
   if (const int rc = check_act16("im2col_nchw", out_hi, out_plane, 8, true)) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    FGT_CUDA(cudaFuncSetAttribute(im2col_nchw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kIm2colSmemMax)));
-    attr_set = true;
-  }
-  launch_k(im2col_nchw_kernel, dim3(n * OH), dim3(blk), smem, reinterpret_cast<cudaStream_t>(stream), 
-      src0, c0, src1, c1, n, H, W, k, stride, pad, replicate, OH, OW, cpad, scale, shift,
-      reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  if (const int rc = allow_dynamic_smem(im2col_nchw_kernel, kIm2colSmemMax, "im2col_nchw_kernel")) return rc;
+  FGT_LAUNCH(im2col_nchw_kernel, dim3(n * OH), dim3(blk), smem, stream, src0, c0, src1, c1, n, H, W, k, stride, pad,
+             replicate, OH, OW, cpad, scale, shift, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -553,10 +538,8 @@ extern "C" int fgt_rownorm_bcast(const float* a, int ca, int lda, const float* b
   FGT_REQUIRE(rows_per_batch >= 1 && total_rows >= 1, FGT_ERR_ARG, "rownorm: rows");
   FGT_REQUIRE((gamma == nullptr) == (beta == nullptr), FGT_ERR_ARG, "rownorm: gamma and beta go together");
   const int block = 256;
-  launch_k(rownorm_kernel, dim3(grid_for(total_rows * 32, block)), dim3(block), 0, reinterpret_cast<cudaStream_t>(stream), 
-      a, ca, lda, b, cb, ldb, gather, rows_per_batch, total_rows, dst_batch_rows, dst_row0, gamma, beta, dst,
-      out_plane, eps);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(rownorm_kernel, dim3(grid_stride(total_rows * 32, block)), dim3(block), 0, stream, a, ca, lda, b, cb, ldb,
+             gather, rows_per_batch, total_rows, dst_batch_rows, dst_row0, gamma, beta, dst, out_plane, eps);
   return FGT_OK;
 }
 
@@ -564,9 +547,8 @@ extern "C" int fgt_dwpool(const float* a, int ca, const float* b, int cb, int bt
                           int gw, const float* weight, const float* bias, float* out, fgt_stream_t stream) {
   FGT_REQUIRE(a && weight && bias && out && k >= 1 && gh >= 1 && gw >= 1, FGT_ERR_ARG, "dwpool: bad argument");
   const long long total = static_cast<long long>(bt) * gh * gw * (ca + cb);
-  launch_k(dwpool_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), a, ca, b, cb, bt, h, w, k,
-                                                                                        gh, gw, weight, bias, out);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(dwpool_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, a, ca, b, cb, bt, h, w, k, gh, gw,
+             weight, bias, out);
   return FGT_OK;
 }
 
@@ -576,9 +558,8 @@ extern "C" int fgt_dwconv3x3_res(const float* x, int bt, int h, int w, int C, co
   FGT_REQUIRE(C % 4 == 0, FGT_ERR_ARG, "dwconv3x3_res: C=%d must be a multiple of 4", C);
   if (const int rc = check_act16("dwconv3x3_res", out_hi, out_plane, 4, true)) return rc;
   const int tx = (C / 4) < 128 ? (C / 4 + 31) / 32 * 32 : 128;   // threads along channels (x), tokens of the row along y
-  launch_k(dwconv3_res_kernel, dim3(bt * h, w >= 16 ? 4 : 1), dim3(tx, 256 / tx > 0 ? 256 / tx : 1), 0, reinterpret_cast<cudaStream_t>(stream), 
-      x, bt, h, w, C, weight, bias, out, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(dwconv3_res_kernel, dim3(bt * h, w >= 16 ? 4 : 1), dim3(tx, 256 / tx > 0 ? 256 / tx : 1), 0, stream, x, bt,
+             h, w, C, weight, bias, out, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -590,10 +571,8 @@ extern "C" int fgt_fold(const float* hid, int bt, int th, int tw, int C, int kh,
   if (const int rc = check_act16("fold", out_hi, out_plane, 4, true)) return rc;
   const int gx = (C / 4 + 1) / 2 * 2;  // channel groups per row of the thread block
   const dim3 blk(gx, 256 / gx);
-  launch_k(fold_kernel, dim3(bt * OH), dim3(blk), 0, reinterpret_cast<cudaStream_t>(stream), 
-      hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW, normalize, add, out, reinterpret_cast<__nv_bfloat16*>(out_hi),
-      out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(fold_kernel, dim3(bt * OH), dim3(blk), 0, stream, hid, bt, th, tw, C, kh, kw, stride, pad, OH, OW,
+             normalize, add, out, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -604,9 +583,8 @@ extern "C" int fgt_unfold(const float* img, int bt, int th, int tw, int C, int k
   if (const int rc = check_act16("unfold", out_hi, out_plane, 4, false)) return rc;
   const int gx = (C / 4 + 1) / 2 * 2;
   const dim3 blk(gx, 256 / gx);
-  launch_k(unfold_kernel, dim3(bt * th * tw), dim3(blk), 0, reinterpret_cast<cudaStream_t>(stream), 
-      img, bt, th, tw, C, kh, kw, stride, pad, OH, OW, relu, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(unfold_kernel, dim3(bt * th * tw), dim3(blk), 0, stream, img, bt, th, tw, C, kh, kw, stride, pad, OH, OW,
+             relu, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -620,9 +598,8 @@ extern "C" int fgt_fold_unfold(const float* hid, int bt, int th, int tw, int C, 
               "fold_unfold: patches do not cover the %dx%d map", OH, OW);
   const int gx = (C / 4 + 1) / 2 * 2;
   const dim3 blk(gx, 256 / gx);
-  launch_k(fold_unfold_kernel, dim3(bt * (OH + 2 * pad), 4), dim3(blk), 0, reinterpret_cast<cudaStream_t>(stream), hid, bt, th, tw, C, kh,
-           kw, stride, pad, OH, OW, relu, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(fold_unfold_kernel, dim3(bt * (OH + 2 * pad), 4), dim3(blk), 0, stream, hid, bt, th, tw, C, kh, kw, stride,
+             pad, OH, OW, relu, reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }
 
@@ -634,9 +611,8 @@ extern "C" int fgt_upsample2x(const void* in_hi, long long in_plane, int n, int 
   if (const int rc = check_act16("upsample2x", in_hi, in_plane, 8, true)) return rc;
   if (const int rc = check_act16("upsample2x", out_hi, out_plane, 8, true)) return rc;
   const long long total = (in_plane == 0 ? 1LL : 2LL) * n * (2 * H) * (2 * W) * (C / 8);
-  launch_k(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
-      reinterpret_cast<const __nv_bfloat16*>(in_hi), in_plane, n, H, W, C, reinterpret_cast<__nv_bfloat16*>(out_hi),
-      out_plane);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(upsample2x_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream,
+             reinterpret_cast<const __nv_bfloat16*>(in_hi), in_plane, n, H, W, C,
+             reinterpret_cast<__nv_bfloat16*>(out_hi), out_plane);
   return FGT_OK;
 }

@@ -80,17 +80,13 @@ extern "C" int fgt_flow_splat(const float* feat, const float* flow, int B, int C
                               float* wsum, fgt_stream_t stream) {
   FGT_REQUIRE(feat && flow && out && wsum && B >= 1 && C >= 1 && H >= 1 && W >= 1, FGT_ERR_ARG,
               "flow_splat: bad argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long HW = static_cast<long long>(H) * W;
-  FGT_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * B * C * HW, st));
-  FGT_CUDA(cudaMemsetAsync(wsum, 0, sizeof(float) * B * HW, st));
-  long long g = (B * HW + 255) / 256;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  FGT_CUDA(launch_k(splat_kernel, dim3(static_cast<unsigned>(g > cap ? cap : g)), dim3(256), 0, st, feat, flow, B, C, H,
-                    W, backward, out, wsum));
-  g = (B * C * HW + 255) / 256;
-  FGT_CUDA(launch_k(splat_norm_kernel, dim3(static_cast<unsigned>(g > cap ? cap : g)), dim3(256), 0, st, out,
-                    static_cast<const float*>(wsum), B, C, HW));
+  FGT_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * B * C * HW, stream));
+  FGT_CUDA(cudaMemsetAsync(wsum, 0, sizeof(float) * B * HW, stream));
+  FGT_LAUNCH(splat_kernel, dim3(grid_stride(B * HW, 256)), dim3(256), 0, stream, feat, flow, B, C, H, W, backward, out,
+             wsum);
+  FGT_LAUNCH(splat_norm_kernel, dim3(grid_stride(B * C * HW, 256)), dim3(256), 0, stream, out,
+             static_cast<const float*>(wsum), B, C, HW);
   return FGT_OK;
 }
 

@@ -209,8 +209,6 @@ extern "C" int fgt_swin_prep(const float* x, const float* fp, int d, int df, int
   // the following blocks: 8 window rows each (one warp per row)
   const int block = 256;
   const long long blocks = static_cast<long long>(bt) * gh * gw + (static_cast<long long>(bt) * nl + 7) / 8;
-  fgt::launch_k(fgt::swin_prep_kernel, dim3(static_cast<unsigned>(blocks)), dim3(block), 0,
-                reinterpret_cast<cudaStream_t>(stream), a);
-  FGT_CUDA(cudaGetLastError());
+  FGT_LAUNCH(fgt::swin_prep_kernel, dim3(static_cast<unsigned>(blocks)), dim3(block), 0, stream, a);
   return FGT_OK;
 }

@@ -9,6 +9,7 @@ import shutil
 import subprocess
 
 import pytest
+import torch
 
 from fgt_b200 import lib
 
@@ -42,6 +43,42 @@ def test_struct_layout_matches_the_c_compiler(tmp_path):
     subprocess.run([CC, "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
     got = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()
     assert [int(x) for x in got] == want
+
+
+def test_kernels_launch_only_through_the_checked_launcher():
+    """Launches, the dynamic shared-memory opt-in and grid-stride sizing live in common.h / common.cu: no other source
+    launches a kernel, reads the runtime's last error, sets a kernel attribute or sizes a grid-stride grid itself."""
+    banned = ("cudaLaunchKernelEx", "cudaFuncSetAttribute", "cudaGetLastError", "<<<", "launch_k(", "num_sms()) * 16",
+              "num_sms() * 16")
+    csrc = os.path.join(ROOT, "fgt_b200", "csrc")
+    paths = glob.glob(os.path.join(csrc, "*.cu")) + glob.glob(os.path.join(csrc, "*.cuh"))
+    assert len(paths) > 10
+    for path in paths:
+        if os.path.basename(path) == "common.cu":
+            continue
+        with open(path) as f:
+            src = f.read()
+        found = [b for b in banned if b in src]
+        assert not found, (os.path.basename(path), found)
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="checks the launch errors of a host without a CUDA device")
+def test_launch_errors_name_the_kernel_without_a_device():
+    """With no device the runtime refuses every launch before any pointer is used. Each entry returns FGT_ERR_CUDA
+    with an error naming its own kernel, from its own launch (im2col_nchw: from its shared-memory opt-in), not an
+    error an earlier call left pending."""
+    L = lib.load()
+    p = ctypes.c_void_p(1 << 20)                    # aligned, never dereferenced
+    ll, f32 = ctypes.c_longlong, ctypes.c_float
+    calls = [
+        (L.fgt_avgpool2, (p, ll(1), 4, 4, p, None), "avgpool2_kernel"),
+        (L.fgt_plane_max, (p, 1, ll(16), p, None), "plane_max_kernel"),
+        (L.fgt_im2col_nchw, (p, 4, None, 0, 1, 8, 8, 3, 1, 1, 0, 8, 8, 64, f32(1), f32(0), p, ll(0), None),
+         "im2col_nchw_kernel"),
+    ]
+    for fn, args, kernel in calls * 2:
+        assert fn(*args) == lib.ERR_CUDA, fn.__name__
+        assert kernel in L.fgt_last_error().decode(), (fn.__name__, L.fgt_last_error())
 
 
 def _calls():

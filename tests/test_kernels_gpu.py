@@ -459,3 +459,37 @@ def test_fold_unfold_fused_equals_two_launches(bt, OH, OW, C):
     im = F.fold(cols, (OH, OW), k, stride=s, padding=p) / F.fold(torch.ones_like(cols), (OH, OW), k, stride=s, padding=p)
     ref = F.relu(F.unfold(im, k, stride=s, padding=p)).reshape(bt, C, k * k, th * tw).permute(0, 3, 2, 1).reshape(bt * th * tw, -1)
     assert_close(lib.from_split(one), ref, KTOL, "fold_unfold vs nn.Fold/nn.Unfold")
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two CUDA devices")
+def test_chain_on_two_devices_in_one_process():
+    """The dynamic shared-memory limit the im2col, GEMM, attention and conv-tail kernels raise belongs to each kernel as
+    loaded on one device: the chain run on cuda:0 and then on cuda:1 in one process gives the same bits on both."""
+    lib = _lib()
+    from fgt_b200 import packing
+    g = torch.Generator().manual_seed(11)
+    n, H, W, C = 1, 16, 24, 128
+    M = n * H * W
+    x = torch.randn(n, 3, H, W, generator=g)
+    w1, b1 = torch.randn(C, 64, generator=g) / 8, torch.randn(C, generator=g)
+    w2, b2 = torch.randn(3, C, 3, 3, generator=g) / 32, torch.randn(3, generator=g)
+    outs = []
+    for d in range(2):
+        dev = torch.device("cuda", d)
+        with torch.cuda.device(dev):
+            cols = torch.empty(2, n, H, W, 64, dtype=torch.bfloat16, device=dev)
+            lib.im2col_nchw(x.to(dev), None, cols, k=3, stride=1, pad=1, replicate=False, OH=H, OW=W)
+            h = lib.empty_split((M, C), dev)
+            lib.gemm_tc([lib.ASeg(cols, 64, M)], packing.pack_weight(w1).to(dev), C, out_w=M, bn=128, bias=b1.to(dev),
+                        out_split=h)
+            a = lib.empty_split((M, C), dev)
+            lib.attention(h, h, h, a, batches=1, heads=1, Lq=M, Lk=M, q_ld=C, k_ld=C, v_ld=C, out_ld=C,
+                          q_batch_stride=M * C, k_batch_stride=M * C, v_batch_stride=M * C, out_batch_stride=M * C,
+                          scale=C ** -0.5)
+            out = torch.full((n, 3, H, W), float("nan"), device=dev)
+            lib.conv_tail(a, n, H, W, C, packing.pack_weight(lib.pack_taps_as_n(w2)).to(dev), 3, b2.to(dev),
+                          lib.ACT_TANH, out, nchw=True)
+            torch.cuda.synchronize(dev)
+        outs.append(out.cpu())
+    assert torch.isfinite(outs[0]).all()
+    assert torch.equal(outs[0], outs[1])
