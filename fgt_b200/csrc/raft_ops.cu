@@ -285,6 +285,39 @@ __global__ void convex_upsample_kernel(const float* __restrict__ mask, const flo
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// upflow8 (RAFT/utils/utils.py:80-82), the small model's upsampling: 8 * F.interpolate(flow, (8h, 8w), bilinear,
+// align_corners=True). Source index and weights follow ATen's upsample_bilinear2d: scale = (in - 1) / (out - 1) in fp32
+// (0 for a 1-pixel side), src = scale * dst, i0 = (int)src, i1 = i0 + (i0 < in - 1), lambda = src - i0.
+// One thread per output pixel of one image, both flow channels; flow [n,2,h,w] -> out [n,2,8h,8w] fp32.
+// ------------------------------------------------------------------------------------------
+__global__ void upflow8_kernel(const float* __restrict__ flow, int n_img, int h, int w, float* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int H = 8 * h, W = 8 * w;
+  const float sy = static_cast<float>(h - 1) / static_cast<float>(H - 1);
+  const float sx = static_cast<float>(w - 1) / static_cast<float>(W - 1);
+  const long long total = static_cast<long long>(n_img) * H * W;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int ox = static_cast<int>(i % W);
+    const int oy = static_cast<int>((i / W) % H);
+    const int img = static_cast<int>(i / (static_cast<long long>(W) * H));
+    const float fy = sy * static_cast<float>(oy), fx = sx * static_cast<float>(ox);
+    const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
+    const int y1 = y0 + (y0 < h - 1 ? 1 : 0), x1 = x0 + (x0 < w - 1 ? 1 : 0);
+    const float ly = fy - static_cast<float>(y0), lx = fx - static_cast<float>(x0);
+    const float hy = 1.f - ly, hx = 1.f - lx;
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const float* f = flow + (static_cast<long long>(img) * 2 + c) * h * w;
+      const float v = hy * (hx * __ldg(f + y0 * w + x0) + lx * __ldg(f + y0 * w + x1)) +
+                      ly * (hx * __ldg(f + y1 * w + x0) + lx * __ldg(f + y1 * w + x1));
+      out[(static_cast<long long>(img) * 2 + c) * H * W + static_cast<long long>(oy) * W + ox] = 8.f * v;
+    }
+  }
+}
+
 }  // namespace fgt
 
 using namespace fgt;
@@ -373,5 +406,12 @@ extern "C" int fgt_convex_upsample(const float* mask, const float* flow_nchw, in
   const long long total = static_cast<long long>(n) * h * w * 64;
   FGT_LAUNCH(convex_upsample_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, mask, flow_nchw, n, h, w,
              out);
+  return FGT_OK;
+}
+
+extern "C" int fgt_upflow8(const float* flow_nchw, int n, int h, int w, float* out, fgt_stream_t stream) {
+  FGT_REQUIRE(flow_nchw && out && n >= 1 && h >= 1 && w >= 1, FGT_ERR_ARG, "upflow8: n=%d h=%d w=%d", n, h, w);
+  const long long total = static_cast<long long>(n) * 64 * h * w;
+  FGT_LAUNCH(upflow8_kernel, dim3(grid_stride(total, 256)), dim3(256), 0, stream, flow_nchw, n, h, w, out);
   return FGT_OK;
 }

@@ -5,7 +5,7 @@ through the batched RAFT of the GPU backend (or any callable with its signature)
 fgt_b200.io.write_flo (byte-identical to the reference's writer).
 
     python -m fgt_b200.flow_extract --path videos/ --outroot flows/ --model raft-things.pth [--width 432 --height 256]
-                                    [--mixed_precision]
+                                    [--mixed_precision] [--small]
 """
 import argparse
 import os
@@ -51,12 +51,15 @@ def main(argv=None):
     ap.add_argument("--gpu", type=int, default=0)
     ap.add_argument("--mixed_precision", action="store_true",
                     help="run RAFT with fp16 tensor-core operands, as the reference's autocast mode")
+    ap.add_argument("--small", action="store_true",
+                    help="run RAFT's small model (RAFT-S; --model must then be a small-model checkpoint such as "
+                         "raft-small.pth)")
     ns = ap.parse_args(argv)
+    from . import raft_small
     from .pipeline import GpuBackend
-    from .raft_model import RAFT
     dev = torch.device("cuda", ns.gpu)
-    raft = torch.nn.DataParallel(RAFT(argparse.Namespace(small=False, mixed_precision=ns.mixed_precision,
-                                                         alternate_corr=False)))
+    raft = torch.nn.DataParallel(raft_small.make_raft(argparse.Namespace(small=ns.small, mixed_precision=ns.mixed_precision,
+                                                                         alternate_corr=False)))
     raft.load_state_dict(torch.load(ns.model, map_location="cpu"))
     backend = GpuBackend(raft.module.to(dev).eval(), None, None, device=dev)
     skip = set(os.listdir(ns.expdir)) if ns.expdir and os.path.isdir(ns.expdir) else set()

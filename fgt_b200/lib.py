@@ -477,6 +477,12 @@ def convex_upsample(mask, flow_nchw, h, w, out, n=1, tag=""):
         call("fgt_convex_upsample", mask, flow_nchw, n, h, w, out)
 
 
+def upflow8(flow_nchw, h, w, out, n=1, tag=""):
+    """8 * bilinear x8 upsampling (align_corners=True) of [n,2,h,w] fp32 flow into out [n,2,8h,8w] fp32."""
+    with _Prof("upflow8", tag, 0, 4.0 * n * 2 * h * w * 65):
+        call("fgt_upflow8", flow_nchw, n, h, w, out)
+
+
 def f16_to_split(src, out_split, tag=""):
     """fp16 tensor -> split-bf16 [2, ...] of the same element count (exact)."""
     with _Prof("f16_to_split", tag, 0, 6.0 * src.numel()):

@@ -660,21 +660,22 @@ def write_visualisations(outroot, vis, backend, vis_flows=False, vis_completed_f
 
 # ------------------------------------------------------------------------------------------------ command line
 def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False, fgt_mixed_precision=False,
-                lafc_mixed_precision=False):
+                lafc_mixed_precision=False, small=False):
     """initialize_RAFT / initialize_LAFC / initialize_FGT (:186-230) with the drop-in modules: the same checkpoint
     layout (a `module.`-prefixed RAFT state dict; directories holding one *.tar with `model_state_dict` and one
     *.yaml config). mixed_precision: RAFT's fp16 mode (the reference's --mixed_precision, RAFT only).
     fgt_mixed_precision: the FGT generator's fp16 mode (FGT.enable_mixed_precision). lafc_mixed_precision: the LAFC
-    flow-completion network's fp16 mode (P3DNet.enable_mixed_precision). The three are independent. Returns
+    flow-completion network's fp16 mode (P3DNet.enable_mixed_precision). The three are independent. small: RAFT's
+    small model (the reference's --small; raft_small.SmallRAFT, fp32 only), from a checkpoint of that model. Returns
     (GpuBackend, lafc_config)."""
     import glob
     import os
 
     import yaml
 
+    from . import raft_small
     from .fgt_model import Model as FGTModel
     from .lafc_model import Model as LAFCModel
-    from .raft_model import RAFT
 
     def ckpt_dir(d):
         tars, yamls = glob.glob(os.path.join(d, "*.tar")), glob.glob(os.path.join(d, "*.yaml"))
@@ -683,8 +684,8 @@ def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False
         with open(yamls[0]) as fh:
             return torch.load(tars[0], map_location="cpu")["model_state_dict"], yaml.full_load(fh)
 
-    raft = torch.nn.DataParallel(RAFT(argparse.Namespace(small=False, mixed_precision=bool(mixed_precision),
-                                                         alternate_corr=False)))
+    raft = torch.nn.DataParallel(raft_small.make_raft(argparse.Namespace(
+        small=bool(small), mixed_precision=bool(mixed_precision), alternate_corr=False)))
     raft.load_state_dict(torch.load(raft_model, map_location="cpu"))
     raft = raft.module.to(device).eval()
     lafc_sd, lafc_cfg = ckpt_dir(lafc_ckpts)
@@ -715,6 +716,9 @@ def arg_parser():
     ap.add_argument("--mixed_precision", action="store_true",
                     help="run RAFT with fp16 tensor-core operands, as the reference's autocast mode (faster, not "
                          "fp32-accurate)")
+    ap.add_argument("--small", action="store_true",
+                    help="run RAFT's small model (RAFT-S; --raft_model must then be a small-model checkpoint such as "
+                         "raft-small.pth): faster, coarser flow")
     ap.add_argument("--fgt_mixed_precision", action="store_true",
                     help="run the FGT generator with fp16 tensor-core operands, as the reference under CUDA autocast "
                          "(faster, not fp32-accurate; independent of --mixed_precision)")
@@ -751,6 +755,8 @@ def main(argv=None):
     fgt_kw = dict(fgt_mixed_precision=True) if ns.fgt_mixed_precision else {}
     if ns.lafc_mixed_precision:
         fgt_kw["lafc_mixed_precision"] = True
+    if ns.small:
+        fgt_kw["small"] = True
     backend, lafc_cfg = load_models(ns.raft_model, ns.lafc_ckpts, ns.fgt_ckpts, dev, ns.mixed_precision, **fgt_kw)
     args = make_args(**{k: getattr(ns, k) for k in DEFAULTS if hasattr(ns, k)})
     frames = IO.read_frames(ns.path)

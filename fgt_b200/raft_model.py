@@ -92,7 +92,8 @@ class RAFT(NativeNet):
         super().__init__()
         self.args = args
         if getattr(args, "small", False):
-            raise ValueError("fgt_b200 RAFT implements the basic model (the driver never sets --small)")
+            raise ValueError("fgt_b200.raft_model.RAFT is the basic model; the small model (small=True) is "
+                             "fgt_b200.raft_small.SmallRAFT, and fgt_b200.raft_small.make_raft(args) chooses by args.small")
         if getattr(args, "alternate_corr", False):
             raise ValueError("alternate_corr is unreachable in the reference (RAFT/raft.py:106) and unsupported")
         self.hidden_dim = self.context_dim = 128

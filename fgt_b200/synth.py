@@ -330,6 +330,61 @@ def raft_inputs(seed=0, H=480, W=864, n=1, shift=3.0):
 
 
 # ----------------------------------------------------------------------------------------------
+# RAFT (small model, the reference's --small)
+# ----------------------------------------------------------------------------------------------
+def raft_small_param_shapes():
+    """state_dict contract of RAFT.RAFT(small=True), /root/reference/RAFT/{raft,extractor,update}.py: 106 keys, all
+    conv weights and biases (InstanceNorm2d and the cnet's norm_fn='none' hold no parameters)."""
+    s = {}
+
+    def conv(name, co, ci, k):
+        s[name + ".weight"] = (co, ci, k, k)
+        s[name + ".bias"] = (co,)
+
+    def enc(pre, out_dim):
+        conv(pre + ".conv1", 32, 3, 7)
+        cin = 32
+        for li, (dim, stride) in enumerate(((32, 1), (64, 2), (96, 2)), start=1):
+            for bi in range(2):
+                k = f"{pre}.layer{li}.{bi}"
+                ci = cin if bi == 0 else dim
+                conv(k + ".conv1", dim // 4, ci, 1)
+                conv(k + ".conv2", dim // 4, dim // 4, 3)
+                conv(k + ".conv3", dim, dim // 4, 1)
+                if bi == 0 and stride != 1:
+                    conv(k + ".downsample.0", dim, ci, 1)
+            cin = dim
+        conv(pre + ".conv2", out_dim, 96, 1)
+
+    enc("fnet", 128)
+    enc("cnet", 96 + 64)
+    u = "update_block."
+    conv(u + "encoder.convc1", 96, 196, 1)
+    conv(u + "encoder.convf1", 64, 2, 7)
+    conv(u + "encoder.convf2", 32, 64, 3)
+    conv(u + "encoder.conv", 80, 128, 3)
+    for g in "zrq":
+        conv(u + f"gru.conv{g}", 96, 96 + 146, 3)
+    conv(u + "flow_head.conv1", 128, 96, 3)
+    conv(u + "flow_head.conv2", 2, 128, 3)
+    return s
+
+
+def raft_small_state_dict(seed=0, flow_gain=0.5):
+    """Seeded small-RAFT weights, drawn like raft_state_dict: He-style conv weights (gain 1.4, 1.0 for the GRU,
+    flow_gain for the flow head's last conv) and small random biases."""
+    sd = {}
+    for key, shape in raft_small_param_shapes().items():
+        g = torch.Generator().manual_seed((seed * 1000003 + zlib.crc32(key.encode())) & 0x7FFFFFFF)
+        if len(shape) == 4:
+            gain = flow_gain if "flow_head.conv2" in key else 1.0 if "gru.conv" in key else 1.4
+            sd[key] = torch.randn(shape, generator=g) * (gain / math.sqrt(shape[1] * shape[2] * shape[3]))
+        else:
+            sd[key] = 0.05 * torch.randn(shape, generator=g)
+    return sd
+
+
+# ----------------------------------------------------------------------------------------------
 # flow-guided gradient propagation (get_flowNN_gradient)
 # ----------------------------------------------------------------------------------------------
 def prop_inputs(seed=0, H=64, W=96, N=6):

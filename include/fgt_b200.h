@@ -533,6 +533,10 @@ int fgt_f16_to_split(const void* src, long long n, void* out_hi, long long out_p
 int fgt_convex_upsample(const float* mask, const float* flow_nchw, int n, int h, int w, float* out,
                         fgt_stream_t stream);
 
+/* upflow8 (RAFT/utils/utils.py:80-82), the small model's upsampling: 8 * F.interpolate(flow, (8h, 8w), bilinear,
+ * align_corners=True), flow [n,2,h,w] -> out [n,2,8h,8w] fp32, ATen's source-index arithmetic (scale 0 for h or w 1). */
+int fgt_upflow8(const float* flow_nchw, int n, int h, int w, float* out, fgt_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Flow-guided gradient propagation (tool/get_flowNN_gradient.py:11-534, Nonlocal=False). Dense state
  * per NN slot (0 = backward-flow neighbours, 1 = forward-flow neighbours), all [N,H,W]:
