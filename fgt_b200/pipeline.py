@@ -659,6 +659,21 @@ def write_visualisations(outroot, vis, backend, vis_flows=False, vis_completed_f
 
 
 # ------------------------------------------------------------------------------------------------ command line
+def load_ckpt_dir(d):
+    """A checkpoint directory of the reference (FGT/train.py:45-50): one *.tar holding `model_state_dict` and one
+    *.yaml config. Returns (state_dict, config)."""
+    import glob
+    import os
+
+    import yaml
+
+    tars, yamls = glob.glob(os.path.join(d, "*.tar")), glob.glob(os.path.join(d, "*.yaml"))
+    if len(tars) != 1 or len(yamls) != 1:
+        raise FileNotFoundError(f"{d}: expected exactly one *.tar and one *.yaml (found {len(tars)}, {len(yamls)})")
+    with open(yamls[0]) as fh:
+        return torch.load(tars[0], map_location="cpu")["model_state_dict"], yaml.full_load(fh)
+
+
 def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False, fgt_mixed_precision=False,
                 lafc_mixed_precision=False, small=False):
     """initialize_RAFT / initialize_LAFC / initialize_FGT (:186-230) with the drop-in modules: the same checkpoint
@@ -668,31 +683,19 @@ def load_models(raft_model, lafc_ckpts, fgt_ckpts, device, mixed_precision=False
     flow-completion network's fp16 mode (P3DNet.enable_mixed_precision). The three are independent. small: RAFT's
     small model (the reference's --small; raft_small.SmallRAFT, fp32 only), from a checkpoint of that model. Returns
     (GpuBackend, lafc_config)."""
-    import glob
-    import os
-
-    import yaml
-
     from . import raft_small
     from .fgt_model import Model as FGTModel
     from .lafc_model import Model as LAFCModel
-
-    def ckpt_dir(d):
-        tars, yamls = glob.glob(os.path.join(d, "*.tar")), glob.glob(os.path.join(d, "*.yaml"))
-        if len(tars) != 1 or len(yamls) != 1:
-            raise FileNotFoundError(f"{d}: expected exactly one *.tar and one *.yaml (found {len(tars)}, {len(yamls)})")
-        with open(yamls[0]) as fh:
-            return torch.load(tars[0], map_location="cpu")["model_state_dict"], yaml.full_load(fh)
 
     raft = torch.nn.DataParallel(raft_small.make_raft(argparse.Namespace(
         small=bool(small), mixed_precision=bool(mixed_precision), alternate_corr=False)))
     raft.load_state_dict(torch.load(raft_model, map_location="cpu"))
     raft = raft.module.to(device).eval()
-    lafc_sd, lafc_cfg = ckpt_dir(lafc_ckpts)
+    lafc_sd, lafc_cfg = load_ckpt_dir(lafc_ckpts)
     lafc = LAFCModel(lafc_cfg)
     lafc.load_state_dict(lafc_sd)
     lafc.net.enable_mixed_precision(bool(lafc_mixed_precision))
-    fgt_sd, fgt_cfg = ckpt_dir(fgt_ckpts)
+    fgt_sd, fgt_cfg = load_ckpt_dir(fgt_ckpts)
     fgt = FGTModel(fgt_cfg)
     fgt.load_state_dict(fgt_sd)
     fgt.net.enable_mixed_precision(bool(fgt_mixed_precision))

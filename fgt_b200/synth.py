@@ -226,6 +226,94 @@ def lafc_inputs(seed=0, T=3, H=240, W=432, b=1):
 
 
 # ----------------------------------------------------------------------------------------------
+# single-frame ("2D") LAFC, FGT's validation flow completion (LAFC/config/train_single.yaml)
+# ----------------------------------------------------------------------------------------------
+CFG_LAFC_SINGLE = dict(num_flows=1, cnum=48, in_channel=3, PASSMASK=1, use_residual=1, resBlocks=1, use_bias=1,
+                       conv_type='vanilla', init_weights=1, model='lafc_single')
+
+
+def lafc_single_param_shapes(cfg=CFG_LAFC_SINGLE):
+    """state_dict contract of FGT.models.lafc_single.Model (/root/reference/FGT/models/lafc_single.py:21-68)."""
+    c = cfg['cnum']
+    s = {}
+
+    def c2(name, co, ci, k, bare=False):
+        key = name if bare else name + ".featureConv"
+        s[key + ".weight"] = (co, ci, k, k)
+        s[key + ".bias"] = (co,)
+
+    c2("encoder2.1", c, cfg['in_channel'], 5)
+    c2("encoder2.2", 2 * c, c, 3)
+    c2("encoder4.0", 2 * c, 2 * c, 3)
+    c2("encoder4.1", 4 * c, 2 * c, 3)
+    for i in range(cfg['resBlocks']):
+        c2(f"res_blocks.{i}.conv1", 4 * c, 4 * c, 3, bare=True)
+        c2(f"res_blocks.{i}.conv2", 4 * c, 4 * c, 3, bare=True)
+    for i in range(4):
+        c2(f"middle.{i}", 4 * c, 4 * c, 3)
+    c2("decoder2.0.conv", 2 * c, 8 * c, 3)
+    c2("decoder2.1", 2 * c, 2 * c, 3)
+    c2("decoder2.2", 2 * c, 2 * c, 3)
+    c2("decoder.0.conv", c, 4 * c, 3)
+    c2("decoder.1", c // 2, c, 3)
+    c2("decoder.2", 2, c // 2, 3)
+    c2("edgeDetector.projection", 16, 2, 3)
+    c2("edgeDetector.mid_layer_1", 16, 16, 3)
+    c2("edgeDetector.mid_layer_2", 16, 16, 3)
+    c2("edgeDetector.out_layer", 1, 16, 1)
+    return {"net." + k: v for k, v in s.items()}
+
+
+def lafc_single_state_dict(seed=0, regime="scaled", cfg=CFG_LAFC_SINGLE):
+    """Seeded 2D-LAFC weights in LAFC's two golden regimes: 'scaled' (variance-preserving, random biases) or 'kaiming'
+    (kaiming_normal fan_in, zero biases)."""
+    return make_state_dict(lafc_single_param_shapes(cfg), seed=seed, regime=regime)
+
+
+def lafc_single_inputs(seed=0, n=3, H=240, W=432):
+    """Per-frame diffused flows (pixels) and hole masks as FGT's validation feeds the 2D LAFC
+    (FGT/networks/network.py:299-304): flows [n,2,H,W], masks [n,1,H,W]."""
+    flows, masks = lafc_inputs(seed=seed, T=n, H=H, W=W)
+    return flows[0].transpose(0, 1).contiguous(), masks[0].transpose(0, 1).contiguous()
+
+
+def validation_set(root, seed=0, videos=(("vid_a", 45), ("vid_b", 41), ("vid_short", 25)), H=90, W=150,
+                   flow_hw=(72, 120), flow_ids=None):
+    """Writes a seeded DAVIS-style validation set under `root` in the layout of FGT's valid_config.yaml:
+    JPEGImages/<video>/%05d.jpg (smooth RGB frames, H x W), rectMask/<video>/%05d.png (one moving rectangle, 0 / 255)
+    and flows/<video>/{forward,backward}_flo/%05d.flo (smooth flows of flow_hw, L - 1 per direction, or only the
+    indices in flow_ids). Returns the three roots (frame_root, mask_root, flow_root)."""
+    import os
+
+    from PIL import Image
+
+    from .io import write_flo
+    roots = [os.path.join(root, d) for d in ("JPEGImages", "rectMask", "flows")]
+    g = torch.Generator().manual_seed(seed)
+    fh, fw = flow_hw
+    for vi, (name, n) in enumerate(videos):
+        for r in roots:
+            os.makedirs(os.path.join(r, name), exist_ok=True)
+        base = _smooth(torch.rand(1, 3, H, W, generator=g), k=9)[0]
+        h0, w0 = int(H * (0.25 + 0.1 * vi)), int(W * (0.3 + 0.05 * vi))
+        for i in range(n):
+            shift = (i * 2) % W
+            img = (torch.roll(base, shifts=shift, dims=2) * 255 + 20 * torch.rand(3, H, W, generator=g)).clamp(0, 255)
+            Image.fromarray(img.permute(1, 2, 0).to(torch.uint8).numpy()).save(
+                os.path.join(roots[0], name, f"{i:05d}.jpg"), quality=90)
+            m = torch.zeros(H, W, dtype=torch.uint8)
+            y0, x0 = (H - h0) // 2 + (i % 7) - 3, (i * 3) % (W - w0)
+            m[y0:y0 + h0, x0:x0 + w0] = 255
+            Image.fromarray(m.numpy()).save(os.path.join(roots[1], name, f"{i:05d}.png"))
+        for sub in ("forward_flo", "backward_flo"):
+            os.makedirs(os.path.join(roots[2], name, sub), exist_ok=True)
+            for i in (range(n - 1) if flow_ids is None else sorted(set(flow_ids(n)))):
+                f = _smooth(torch.randn(1, 2, fh, fw, generator=g), k=11)[0] * 40.0
+                write_flo(os.path.join(roots[2], name, sub, f"{i:05d}.flo"), f.permute(1, 2, 0).numpy())
+    return tuple(roots)
+
+
+# ----------------------------------------------------------------------------------------------
 # RAFT (basic model)
 # ----------------------------------------------------------------------------------------------
 def raft_param_shapes():

@@ -281,6 +281,23 @@ int fgt_window_compose(const float* filled, const float* frames, const unsigned 
 int fgt_comp_to_u8(const float* comp, long long total, unsigned char* out, fgt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * The tensor glue of FGT's validation (FGT/networks/network.py:258-352, Network._validate; fgt_b200/validate.py):
+ *   fgt_valid_flow_scale : resized flows [B,H,W,2] float in place, u = u / pre_w * w, v = v / pre_h * h (read_flows)
+ *   fgt_valid_inputs     : frames uint8 [t,H,W,3] and masks uint8 [t,H,W] (0 / non-zero) -> out_frames [t,3,H,W] =
+ *                          x / 127.5 - 1, out_masked = out_frames * (1 - mask), out_masks [t,1,H,W] float 0 / 1
+ *   fgt_valid_norm_flows : out = flows / fmax per plane of plane_size values (norm_flows: signed max, fgt_plane_max)
+ *   fgt_valid_score      : comp = filled * m + frames * (1 - m); comp_u8 and frames_u8 [t,H,W,3] =
+ *                          uint8(clip((x + 1) / 2 * 255, 0, 255)) of comp and of frames (metrics_calc)
+ * Same IEEE single-precision operations in the same order as the reference: bit-identical given the same inputs. */
+int fgt_valid_flow_scale(float* flow, long long pixels, float pre_w, float w, float pre_h, float h, fgt_stream_t stream);
+int fgt_valid_inputs(const unsigned char* frames, const unsigned char* masks, int t, int H, int W, float* out_frames,
+                     float* out_masked, float* out_masks, fgt_stream_t stream);
+int fgt_valid_norm_flows(const float* flows, const float* fmax, int planes, long long plane_size, float* out,
+                         fgt_stream_t stream);
+int fgt_valid_score(const float* filled, const float* frames, const float* masks, int t, int H, int W,
+                    unsigned char* comp_u8, unsigned char* frames_u8, fgt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Forward flow splatting (LAFC/models/utils/flow_warp.py:4-94, flow_prop / warp / sample_one): feat [B,C,H,W] is
  * scattered along flow [B,2,H,W] (channel 0: column shift, channel 1: row shift, as in the reference) to the four
  * integer neighbours of each target with weights exp(-d^2); out [B,C,H,W] = accumulated features / accumulated weight
