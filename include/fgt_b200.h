@@ -440,6 +440,25 @@ int fgt_metrics(const void* a, int a_dtype, const void* b, int b_dtype, int N, i
                 long long workspace_bytes, double* out, double* ssim_c, fgt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Flow warping error of a clip (definition: oracle/warp_error_oracle.py), built from the reference's image_warp and
+ * fbConsistencyCheck (FGT/models/utils/fbConsistencyCheck.py) with grid_sample's align_corners=True convention.
+ * frames [N,H,W,C] (C = 1 or 3) on the 0..255 scale, frame_dtype FGT_METRIC_U8 or FGT_METRIC_F32, I = float32(V) / 255;
+ * masks uint8 [N,H,W] (non-zero = hole; NULL: none); flow_f / flow_b float32 [N-1,2,H,W], F_t: t -> t+1 and
+ * B_t: t+1 -> t, in pixels, x first. Per pair t, with W_t = I_{t+1} sampled at x + F_t(x) and M_t = 1 where
+ * |F + B(x+F)|^2 <= 0.01 (|F|^2 + |B(x+F)|^2) + 0.5, err = sum_c (I_t - W_t)^2 in float64:
+ *   out float64 [N-1][4] = (sum M*err, sum M, sum M*hole_t*err, sum M*hole_t); E_warp of the pair is out[0] / out[1].
+ * H and W at least 2, N at least 2 and N - 1 at most 65535.
+ *   fgt_warp_error_workspace  bytes of workspace for N frames of H x W x C (negative FGT_ERR_* on bad sizes).
+ *   fgt_warp_error            two kernels: per-(pair, 32x32 tile) partial sums into the workspace, then a fixed-order
+ *                             reduction per pair (bit-reproducible). Optional maps (NULL: not written): warped float32
+ *                             [N-1,H,W,C], the warped frame t+1 on the 0..1 scale; valid uint8 [N-1,H,W], M_t.
+ * ------------------------------------------------------------------------------------------ */
+long long fgt_warp_error_workspace(int N, int H, int W, int C);
+int fgt_warp_error(const void* frames, int frame_dtype, const unsigned char* masks, const float* flow_f,
+                   const float* flow_b, int N, int H, int W, int C, void* workspace, long long workspace_bytes,
+                   double* out, float* warped, unsigned char* valid, fgt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Flow colour coding of the driver's --vis_flows (RAFT/utils/flow_viz.py flow_to_image :109-132 with
  * flow_uv_to_colors :70-106 and the 55-entry Middlebury wheel of make_colorwheel :20-67): flows fp32 [B,H,W,2]
  * (8-byte aligned) -> out uint8 [B,H,W,3], RGB (bgr = 0) or BGR (bgr != 0). Each image is divided by its own maximum
