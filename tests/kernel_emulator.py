@@ -2,7 +2,7 @@
 
 `emulating_all()` installs a `KernelEmulator` as the library `lib.load()` returns, the way tests/gemm_emulator.py
 installs its `fgt_gemm_tc` interpreter (which this class extends), so the production launchers fill their arguments as
-they do on the GPU and every launch of a forward is executed here instead: the 16 entries of `ENTRIES` and
+they do on the GPU and every launch of a forward is executed here instead: the 17 entries of `ENTRIES` and
 `fgt_gemm_tc`. Any other entry is refused. `gemm_emulator.emulating()` stays strict (GEMM only).
 
 Semantics are restated from include/fgt_b200.h and from the reference operations the header names (through oracle/),
@@ -29,6 +29,8 @@ not from the kernels' code paths:
 - fgt_raft_flow_update: coords += delta (delta rounded to fp16 first when delta_f16), stored fp32; flow = coords - grid
   (fp32) into NCHW and into channels x_chan, x_chan + 1 of the GRU input.
 - fgt_convex_upsample: RAFT.upsample_flow. fgt_f16_to_split: hi = bf16(v), lo = bf16(v - hi).
+- fgt_upflow8: 8 * bilinear x8 with align_corners=True, source index scale * dst with scale = (in - 1) / (out - 1)
+  (0 for a 1-pixel side), as ATen's upsample_bilinear2d.
 Arithmetic is float64 on the operands as stored (hi + lo for split-bf16, the fp16 value for fp16); each output is
 stored once in its format: fp32 rounded once, split-bf16 as `lib.to_split`, fp16 rounded to nearest. Scalar float
 arguments are taken at the fp32 value the C ABI receives.
@@ -51,7 +53,7 @@ from tests.test_launch_trace import recording
 
 ENTRIES = ("fgt_im2col_nchw", "fgt_rownorm", "fgt_attention", "fgt_fold_unfold", "fgt_fold", "fgt_dwconv3x3_res",
            "fgt_swin_prep", "fgt_conv_tail", "fgt_upsample2x", "fgt_chan_stats", "fgt_instnorm_act", "fgt_avgpool2",
-           "fgt_corr_lookup", "fgt_raft_flow_update", "fgt_convex_upsample", "fgt_f16_to_split")
+           "fgt_corr_lookup", "fgt_raft_flow_update", "fgt_convex_upsample", "fgt_f16_to_split", "fgt_upflow8")
 
 
 def _k16(p, plane):
@@ -523,6 +525,24 @@ class KernelEmulator(GemmEmulator):
     def _f16_to_split(self, a):
         v = self.flat(a["src"], torch.float16)[:a["n"]].double()
         self.st16(a["out_hi"], a["out_plane"], torch.arange(a["n"]), v)
+
+    def _upflow8(self, a):
+        n, h, w = a["n"], a["h"], a["w"]
+        f = self.f32(a["flow_nchw"], n * 2 * h * w).view(n, 2, h, w)
+
+        def axis(size):
+            dst = torch.arange(8 * size, dtype=torch.float64)
+            src = dst * ((size - 1) / (8 * size - 1))
+            i0 = src.long()
+            return i0, (i0 + 1).clamp(max=size - 1), src - i0
+
+        y0, y1, ly = axis(h)
+        x0, x1, lx = axis(w)
+        ly, lx = ly[:, None], lx[None, :]
+        top = (1 - lx) * f[:, :, y0][:, :, :, x0] + lx * f[:, :, y0][:, :, :, x1]
+        bot = (1 - lx) * f[:, :, y1][:, :, :, x0] + lx * f[:, :, y1][:, :, :, x1]
+        up = 8.0 * ((1 - ly) * top + ly * bot)
+        self.st32(a["out"], torch.arange(up.numel()), up)
 
 
 @contextlib.contextmanager

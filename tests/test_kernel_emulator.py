@@ -3,15 +3,16 @@ operations, at the argument forms the forwards use and at the edges where such k
 through them on the CPU against the reference goldens and oracles.
 
 - Coverage: every entry of the launch-trace golden has an interpreter, and every form (`kernel_emulator.form`: the
-  discrete options of one call) that occurs in the six golden traces has a case here. A forward that starts calling a
+  discrete options of one call) that occurs in the seven golden traces has a case here. A forward that starts calling a
   new kernel, or a kernel with a new option, fails `test_every_trace_form_has_a_case`.
 - Cases: each launches the production launcher (`lib.*`) under `emulating_all()` and compares the interpreter's float64
   values with `F.layer_norm`, `F.fold` / `F.unfold`, `F.conv2d` (depthwise and 3x3), `F.instance_norm`,
-  `F.avg_pool2d`, `F.interpolate`, `oracle.raft_oracle.corr_lookup` / `upsample_flow`, or a float64 softmax attention
-  written per zone and per window. Bar EXACT (1e-12 of the largest value): the reference is fed the operands as stored.
-  The stored elements must be exactly the operation's own (rows past nl + G of swin_prep, columns past 324 of the
-  lookup rows, the channels outside the flow slice, dropped attention rows are not), each the float64 value in its
-  output format, and every other element keeps its sentinel bit for bit.
+  `F.avg_pool2d`, `F.interpolate` (nearest, and bilinear for upflow8), `oracle.raft_oracle.corr_lookup` /
+  `upsample_flow`, or a float64 softmax attention written per zone and per window. Bar EXACT (1e-12 of the largest
+  value): the reference is fed the operands as stored. The stored elements must be exactly the operation's own (rows
+  past nl + G of swin_prep, columns past the lookup values of the lookup rows, the channels outside the flow slice,
+  dropped attention rows are not), each the float64 value in its output format, and every other element keeps its
+  sentinel bit for bit. upflow8 is compared on its fp32 output at 1e-6 of (1 + the largest value).
 - Whole forwards in float64 on CPU tensors, bars rel-L2 and max/max <= 1e-4 (rel-L2 / max-over-max observed): FGT fp32
   at 64 x 96, t = 3, 1.55e-5 / 2.13e-5 against both its golden and the oracle (its flow branch is 1-term fp16 by
   design); LAFC at 64 x 96 5.6e-6 / 1.0e-5 (flow) and 4.1e-7 / 1.9e-6 (edge); RAFT at 128 x 160, 3 iterations, against
@@ -459,17 +460,19 @@ def _edge_coords(h, w, seed):
     return torch.stack([xs, ys], 1).contiguous()
 
 
-@case(("split",), ("f16",), ids=["split", "f16"])
-def _corr_lookup(fmt):
+@case(("split", 4, 384), ("f16", 4, 384), ("split", 3, 200), ids=["split", "f16", "split-r3-200"])
+def _corr_lookup(fmt, r, pitch):
+    """Radius 4 into the basic model's 384-wide rows, radius 3 into the small model's 200-wide rows."""
     h, w = 16, 24                                    # coarsest level 2 x 3
     pyr = _pyramid(h, w, 33)
     co = _edge_coords(h, w, 34)
-    out = _buf((h * w, 384), fmt)
+    out = _buf((h * w, pitch), fmt)
     before = out.clone()
-    emu = _run(lambda: lib.corr_lookup(pyr, co, h * w, 4, out))
-    ref = RO.corr_lookup([t[:, None].double() for t in pyr], co.double().t().reshape(1, 2, h, w))
-    full = torch.full((h * w, 384), float("nan"), dtype=torch.float64)
-    full[:, :324] = ref[0].reshape(324, h * w).t()
+    emu = _run(lambda: lib.corr_lookup(pyr, co, h * w, r, out))
+    nv = 4 * (2 * r + 1) ** 2
+    ref = RO.corr_lookup([t[:, None].double() for t in pyr], co.double().t().reshape(1, 2, h, w), r)
+    full = torch.full((h * w, pitch), float("nan"), dtype=torch.float64)
+    full[:, :nv] = ref[0].reshape(nv, h * w).t()
     _check(emu, out, before, full, "corr_lookup", ref_f32=True)
     return emu.forms
 
@@ -531,6 +534,21 @@ def _f16_to_split():
     assert torch.equal(out[0, fin], src[fin].float().to(torch.bfloat16)), "hi"
     assert torch.equal(emu.stored(out)[fin], src[fin].double())
     return emu.forms
+
+
+# ---------------------------------------------------------------------------------------------------------- upflow8
+@case(())
+def _upflow8():
+    """1-pixel sides included: align_corners maps every output of such a side to its one input."""
+    forms = set()
+    for h, w in ((3, 5), (1, 4), (4, 1), (1, 1)):
+        flow = torch.randn(2, 2, h, w, generator=_gen(h * 10 + w))
+        out = _buf((2, 2, 8 * h, 8 * w), "f32")
+        emu = _run(lambda: lib.upflow8(flow, h, w, out, n=2))
+        ref = 8 * F.interpolate(flow.double(), size=(8 * h, 8 * w), mode="bilinear", align_corners=True)
+        assert (out.double() - ref).abs().max() <= 1e-6 * (1 + ref.abs().max()), (h, w)
+        forms |= emu.forms
+    return forms
 
 
 # --------------------------------------------------------------------------------------------------------- the tests

@@ -25,7 +25,7 @@ write must be bit-identical to the pre-launch copy; the elements it writes must 
   in [r16(relu(lo(y16) + res - e)), r16(relu(hi(y16) + res + e))], e the fp32 rounding of the add. So a one-ulp flip of
   y16 before the add is accepted only where y lies within s of an fp16 rounding midpoint; elsewhere the result must be
   the interpreter's. (RAFT's downsample residual is negative: such a flip of a value near 1 survives in a result near 0.)
-Forwards run eagerly, without CUDA graphs: the six launch-trace cases at their geometries with every launch, the GEMMs
+Forwards run eagerly, without CUDA graphs: the seven launch-trace cases at their geometries with every launch, the GEMMs
 included (at 64 x 96 RAFT's coarsest correlation level is 1 x 1, where only the interpreter can serve as reference);
 and the production geometries with every launch but the GEMMs (float64 CPU GEMMs at these sizes add minutes and no
 coverage): FGT 432 x 240, T = 10, fp32 and mixed; RAFT on one 480 x 864 pair, 3 iterations, fp32 and mixed; LAFC at
@@ -37,8 +37,8 @@ for upsample2x, f16_to_split, raft_flow_update and unscaled im2col_nchw, and for
 0.20 (split) / 0.35 (fp16); gemm_tc 0.62 (split, fp32) / 0.41 (fp16); avgpool2 0.67; chan_stats 0.0018;
 conv_tail 0.35 (0.29 in RAFT's flow head); convex_upsample 0.013; corr_lookup 0.56 (split); dwconv3x3_res 0.72;
 fold 0.70; fold_unfold 0.35; instnorm_act 0.57 (split), and every fp16 value inside its interval; rownorm 0.69 (0.34
-on the low-variance rows); swin_prep 0.64 (0.36). The fp16 outputs of corr_lookup, dwconv3x3_res, fold, fold_unfold,
-rownorm and swin_prep reach one fp16 ulp (1.0), never two.
+on the low-variance rows); swin_prep 0.64 (0.36); upflow8 0.013. The fp16 outputs of corr_lookup, dwconv3x3_res,
+fold, fold_unfold, rownorm and swin_prep reach one fp16 ulp (1.0), never two.
 
 Each of these changes to a kernel's arithmetic fails a test here: lookup windows a and b swapped (error 5e4 x the bar),
 eps dropped from rownorm (non-finite on the constant rows; 58 x the bar in FGT's 64 x 96 forward), swin_prep writing a
@@ -341,6 +341,15 @@ def _raft(H, W, iters, mixed=False):
     return lambda: m._forward_impl(im1, im2, iters, None, True, mixed)
 
 
+def _raft_small(H, W, iters):
+    from fgt_b200.raft_small import SmallRAFT
+    m = SmallRAFT(argparse.Namespace(small=True, mixed_precision=False, alternate_corr=False))
+    m.load_state_dict(synth.raft_small_state_dict(seed=3))
+    m = m.to(DEV)
+    im1, im2 = (x.to(DEV) for x in synth.raft_inputs(seed=4, H=H, W=W))
+    return lambda: m._forward_impl(im1, im2, iters, None, True)
+
+
 def _lafc(H, W, T=None):
     from fgt_b200.lafc_model import Model
     m = Model(synth.CFG_LAFC)
@@ -357,6 +366,7 @@ TRACE_CASES = {   # the geometries of tests/test_launch_trace.py
     "fgt_sharded_nccl": lambda: _fgt((64, 96), 2, 64, 96, sharded=True),
     "raft_fp32": lambda: _raft(64, 96, 2),
     "raft_mixed": lambda: _raft(64, 96, 2, mixed=True),
+    "raft_small": lambda: _raft_small(64, 96, 2),
     "lafc": lambda: _lafc(64, 96, T=3),
 }
 

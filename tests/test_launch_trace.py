@@ -117,6 +117,14 @@ def _raft(mixed=False):
     return lambda: m._forward_impl(im1, im2, 2, None, True, mixed)
 
 
+def _raft_small():
+    from fgt_b200.raft_small import SmallRAFT
+    m = SmallRAFT(argparse.Namespace(small=True, mixed_precision=False, alternate_corr=False))
+    m.load_state_dict(synth.raft_small_state_dict(seed=3))
+    im1, im2 = synth.raft_inputs(seed=4, H=64, W=96)
+    return lambda: m._forward_impl(im1, im2, 2, None, True)
+
+
 def _lafc():
     from fgt_b200.lafc_model import Model
     m = Model(synth.CFG_LAFC)
@@ -131,6 +139,7 @@ CASES = {
     "fgt_sharded_nccl": lambda: _fgt(sharded=True),
     "raft_fp32": lambda: _raft(),
     "raft_mixed": lambda: _raft(mixed=True),
+    "raft_small": _raft_small,
     "lafc": _lafc,
 }
 

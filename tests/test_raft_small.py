@@ -5,12 +5,10 @@ import argparse
 
 import pytest
 import torch
-import torch.nn.functional as F
 
-from fgt_b200 import lib, synth
+from fgt_b200 import synth
 from oracle import raft_small_oracle as RSO
-from tests.kernel_emulator import KernelEmulator, _KernelEntry, _raw
-from tests.test_launch_trace import recording
+from tests.kernel_emulator import emulating_all
 from tests.util import assert_close, load_golden
 
 
@@ -65,57 +63,10 @@ def test_constructor_chooses_the_model_and_refusals():
         m(*synth.raft_inputs(seed=0, H=64, W=64), iters=1, test_mode=True)
 
 
-class _Upflow8Entry(_KernelEntry):
-    def __call__(self, *args):
-        a = {k: _raw(v, t) for k, v, t in zip(lib.PROTOS[self.name].names, args, self.argtypes)}
-        self.emu.forms.add((self.name, ()))
-        self.emu._upflow8(a)
-        return 0
-
-
-class SmallRaftEmulator(KernelEmulator):
-    """The float64 interpreters of tests/kernel_emulator.py plus fgt_upflow8: 8 * bilinear x8 with align_corners=True,
-    source index scale * dst with scale = (in - 1) / (out - 1) (0 for a 1-pixel side), as ATen's upsample_bilinear2d."""
-
-    def __getattr__(self, name):
-        if name == "fgt_upflow8":
-            e = _Upflow8Entry(self, name)
-            setattr(self, name, e)
-            return e
-        return super().__getattr__(name)
-
-    def _upflow8(self, a):
-        n, h, w = a["n"], a["h"], a["w"]
-        f = self.f32(a["flow_nchw"], n * 2 * h * w).view(n, 2, h, w)
-
-        def axis(size):
-            dst = torch.arange(8 * size, dtype=torch.float64)
-            src = dst * ((size - 1) / (8 * size - 1))
-            i0 = src.long()
-            return i0, (i0 + 1).clamp(max=size - 1), src - i0
-
-        y0, y1, ly = axis(h)
-        x0, x1, lx = axis(w)
-        ly, lx = ly[:, None], lx[None, :]
-        top = (1 - lx) * f[:, :, y0][:, :, :, x0] + lx * f[:, :, y0][:, :, :, x1]
-        bot = (1 - lx) * f[:, :, y1][:, :, :, x0] + lx * f[:, :, y1][:, :, :, x1]
-        up = 8.0 * ((1 - ly) * top + ly * bot)
-        self.st32(a["out"], torch.arange(up.numel()), up)
-
-
-def _emulated(fn):
-    with torch.no_grad(), recording(SmallRaftEmulator()) as emu:
-        out = fn()
-    return out, emu
-
-
 def test_upflow8_interpreter_matches_interpolate():
-    for h, w in ((3, 5), (1, 4), (4, 1), (1, 1)):
-        flow = torch.randn(2, 2, h, w, generator=torch.Generator().manual_seed(h * 10 + w))
-        out = torch.full((2, 2, 8 * h, 8 * w), -1234.5)
-        _emulated(lambda: lib.upflow8(flow, h, w, out, n=2))
-        ref = 8 * F.interpolate(flow.double(), size=(8 * h, 8 * w), mode="bilinear", align_corners=True)
-        assert (out.double() - ref).abs().max() <= 1e-6 * (1 + ref.abs().max()), (h, w)
+    """The fgt_upflow8 interpreter against F.interpolate, 1-pixel sides included: the interpreter suite's case."""
+    from tests.test_kernel_emulator import CASES
+    CASES["upflow8"]()
 
 
 def test_small_forward_in_float64():
@@ -128,7 +79,8 @@ def test_small_forward_in_float64():
     m = SmallRAFT(_args())
     m.load_state_dict(sd)
     im1, im2 = synth.raft_inputs(seed=meta["seed"] + 1, H=meta["H"], W=meta["W"])
-    (lo, up), emu = _emulated(lambda: m._forward_impl(im1, im2, meta["iters"], None, True))
+    with torch.no_grad(), emulating_all() as emu:
+        lo, up = m._forward_impl(im1, im2, meta["iters"], None, True)
     assert ("fgt_upflow8", ()) in emu.forms and ("fgt_corr_lookup", ("split", 4, 3)) in emu.forms
     assert_close(lo, g["lo"], 1e-4, "small RAFT low vs reference golden")
     assert_close(up, g["up"], 1e-4, "small RAFT up vs reference golden")
