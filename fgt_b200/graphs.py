@@ -80,6 +80,13 @@ class NativeNet(nn.Module):
         self._drop_graphs()
         return super()._apply(fn, *a, **k)
 
+    def _allocators(self, key, dev, mixed):
+        """(B, A) workspace allocators of geometry `key`: B(name, shape, dtype=fp32) and A(name, shape) for the 16-bit
+        activations of the path, split-bf16 (fp32 path) or fp16 (mixed)."""
+        bufs = self._geo.setdefault(key, {})
+        return ((lambda nm, s, dtype=torch.float32: workspace(bufs, nm, s, dev, dtype)),
+                (lambda nm, s, zero=False: workspace(bufs, nm, s, dev, lib.act16_dtype(mixed), zero)))
+
     def enable_cuda_graph(self, on=True):
         """Replay whole forwards as CUDA graphs, one per input geometry and call key."""
         self._graphs = {} if on else None

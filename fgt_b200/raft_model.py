@@ -31,7 +31,7 @@ import torch
 import torch.nn as nn
 
 from . import lib, ops
-from .graphs import NativeNet, workspace
+from .graphs import NativeNet
 
 C3 = dict(kx=3, ky=3, pad_x=1, pad_y=1)
 
@@ -181,13 +181,6 @@ class _RAFTBase(NativeNet):
 
     def _pack_heads(self, put, P):
         """Packs the model's own update-block convs with put(name, state-dict key)."""
-
-    def _allocators(self, key, dev, mixed):
-        """(B, A) workspace allocators of geometry `key`: B(name, shape, dtype=fp32) and A(name, shape) for the 16-bit
-        activations of the path, split-bf16 (fp32 path) or fp16 (mixed)."""
-        bufs = self._geo.setdefault(key, {})
-        return ((lambda nm, s, dtype=torch.float32: workspace(bufs, nm, s, dev, dtype)),
-                (lambda nm, s, zero=False: workspace(bufs, nm, s, dev, lib.act16_dtype(mixed), zero)))
 
     # ------------------------------------------------------------------ encoders
     def _encoder(self, img, net, P, dev, n, mixed=False):

@@ -120,6 +120,7 @@ IM2COL = [  # fmt, two sources, replicate, k, stride, scaled: the forms of the t
     ("split", True, False, 3, 2, False), ("f16", True, False, 3, 2, False), ("f16", False, True, 5, 1, False),
     ("split", False, True, 5, 1, False), ("split", False, False, 3, 1, False), ("split", False, False, 7, 1, False),
     ("f16", False, False, 7, 1, False), ("split", False, False, 7, 2, True), ("f16", False, False, 7, 2, True),
+    ("f16", False, False, 3, 1, False), ("split", True, True, 5, 1, False),
 ]
 
 

@@ -350,13 +350,22 @@ def _raft_small(H, W, iters):
     return lambda: m._forward_impl(im1, im2, iters, None, True)
 
 
-def _lafc(H, W, T=None):
+def _lafc(H, W, T=None, mixed=False):
     from fgt_b200.lafc_model import Model
     m = Model(synth.CFG_LAFC)
     m.load_state_dict(synth.make_state_dict(synth.lafc_param_shapes(synth.CFG_LAFC), seed=5))
     m = m.to(DEV)
     kw = {} if T is None else dict(T=T)
     flows, masks = (x.to(DEV) for x in synth.lafc_inputs(seed=6, H=H, W=W, **kw))
+    return lambda: m.net._forward_impl(flows, masks, mixed=mixed)
+
+
+def _lafc_single(n, H, W):
+    from fgt_b200.lafc_single import Model
+    m = Model(synth.CFG_LAFC_SINGLE)
+    m.load_state_dict(synth.lafc_single_state_dict(seed=5))
+    m = m.to(DEV)
+    flows, masks = (x.to(DEV) for x in synth.lafc_single_inputs(seed=6, n=n, H=H, W=W))
     return lambda: m.net._forward_impl(flows, masks)
 
 
@@ -368,6 +377,8 @@ TRACE_CASES = {   # the geometries of tests/test_launch_trace.py
     "raft_mixed": lambda: _raft(64, 96, 2, mixed=True),
     "raft_small": lambda: _raft_small(64, 96, 2),
     "lafc": lambda: _lafc(64, 96, T=3),
+    "lafc_mixed": lambda: _lafc(64, 96, T=3, mixed=True),
+    "lafc_single": lambda: _lafc_single(2, 64, 96),
 }
 
 

@@ -1,11 +1,9 @@
 """LAFC's mixed-precision mode (P3DNet.enable_mixed_precision), CPU side: the autocast emulation of
 oracle/lafc_mixed_oracle.py, the switch, the per-precision weight and workspace caches, the command-line option, and
-the launch sequence of one fp16 forward against a fixed golden. The numerics are defined by CUDA autocast and checked
-on the GPU (tests/test_lafc_mixed_gpu.py)."""
+the launch sequence of one fp16 forward against its case of the launch-trace golden. The numerics are defined by CUDA
+autocast and checked on the GPU (tests/test_lafc_mixed_gpu.py)."""
 import ctypes
-import gzip
 import json
-import os
 from types import SimpleNamespace
 
 import pytest
@@ -17,8 +15,6 @@ from oracle import lafc_mixed_oracle as LM
 from oracle import lafc_oracle as LO
 from tests.test_launch_trace import load_golden as load_trace_golden
 from tests.test_launch_trace import recording
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "lafc_mixed_trace.json.gz")
 
 
 class _Stop(Exception):
@@ -139,8 +135,7 @@ def test_fp32_launch_sequence_is_unchanged():
 
 def test_mixed_launch_sequence_matches_golden():
     _, calls = _trace(True)
-    with gzip.open(GOLDEN, "rt") as f:
-        want = json.load(f)
+    want = load_trace_golden()["lafc_mixed"]
     assert [c[0] for c in calls] == [c[0] for c in want], "entry sequence differs"
     for i, (g, w) in enumerate(zip(calls, want)):
         assert g == w, f"call {i} ({g[0]}) differs"

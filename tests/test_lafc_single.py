@@ -1,9 +1,8 @@
 """The single-frame ("2D") LAFC of FGT's validation on the CPU: the oracle against goldens of the unmodified reference
 (tests/golden/lafc_single_*.npz), the module's state-dict contract and refusals, the C-ABI call sequence of one forward
-against a fixed golden, and the whole native forward through the float64 interpreters of its launches."""
-import gzip
+against its case of the launch-trace golden, and the whole native forward through the float64 interpreters of its
+launches."""
 import json
-import os
 
 import pytest
 import torch
@@ -11,10 +10,10 @@ import torch
 from fgt_b200 import synth
 from oracle import lafc_single_oracle as LSO
 from tests.kernel_emulator import emulating_all
+from tests.test_launch_trace import load_golden as load_trace_golden
 from tests.test_launch_trace import recording
 from tests.util import assert_close, load_golden
 
-TRACE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "lafc_single_trace.json.gz")
 FULL = ["lafc_single_scaled", "lafc_single_kaiming", "lafc_single_odd"]
 SAMPLED = ["lafc_single_full_scaled", "lafc_single_full_kaiming"]
 
@@ -101,8 +100,7 @@ def trace():
 
 
 def test_launch_trace_matches_golden():
-    with gzip.open(TRACE, "rt") as f:
-        want = json.load(f)
+    want = load_trace_golden()["lafc_single"]
     got = trace()
     assert [c[0] for c in got] == [c[0] for c in want], "entry sequence differs"
     for i, (g, w) in enumerate(zip(got, want)):

@@ -125,11 +125,19 @@ def _raft_small():
     return lambda: m._forward_impl(im1, im2, 2, None, True)
 
 
-def _lafc():
+def _lafc(mixed=False):
     from fgt_b200.lafc_model import Model
     m = Model(synth.CFG_LAFC)
     m.load_state_dict(synth.make_state_dict(synth.lafc_param_shapes(synth.CFG_LAFC), seed=5))
     flows, masks = synth.lafc_inputs(seed=6, T=3, H=64, W=96)
+    return lambda: m.net._forward_impl(flows, masks, mixed=mixed)
+
+
+def _lafc_single():
+    from fgt_b200.lafc_single import Model
+    m = Model(synth.CFG_LAFC_SINGLE)
+    m.load_state_dict(synth.lafc_single_state_dict(seed=5))
+    flows, masks = synth.lafc_single_inputs(seed=6, n=2, H=64, W=96)
     return lambda: m.net._forward_impl(flows, masks)
 
 
@@ -140,7 +148,9 @@ CASES = {
     "raft_fp32": lambda: _raft(),
     "raft_mixed": lambda: _raft(mixed=True),
     "raft_small": _raft_small,
-    "lafc": _lafc,
+    "lafc": lambda: _lafc(),
+    "lafc_mixed": lambda: _lafc(mixed=True),
+    "lafc_single": _lafc_single,
 }
 
 
