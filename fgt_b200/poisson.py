@@ -37,8 +37,9 @@ def poisson_blend_batch(trg, gx, gy, hole, gmask=None, edge=None, device=None, r
                         atol=1e-6, btol=1e-6, conlim=1e8, max_iters=MAX_ITERS, use_graph=True):
     """trg [F,H,W,3], gx [F,H,W-1,3], gy [F,H-1,W,3] (forward differences of the source), hole [F,H,W],
     optional gmask / edge [F,H,W] -> (blend float64 [F,H,W,3], UnfilledMask bool [F,H,W]) on the device
-    (+ per-system (istop, itn) int tensors [F,3] with return_info). use_graph: replay each chunk of iterations as one
-    CUDA graph (default) or launch its kernels one by one."""
+    (+ per-system (istop, itn) int tensors [F,3] with return_info). max_iters is scipy's iter_lim (default 2*H*W): a
+    system still running at iteration max_iters stops there with istop 7 and returns its iterate. use_graph: replay
+    each chunk of iterations as one CUDA graph (default) or launch its kernels one by one."""
     dev = _dev(device)
     # host arrays cross the bus in their own dtype (float32 in the driver) and are widened on the device (exact)
     t64 = lambda a: torch.as_tensor(np.ascontiguousarray(a) if not torch.is_tensor(a) else a).to(dev).to(torch.float64).contiguous()
@@ -60,9 +61,11 @@ def poisson_blend_batch(trg, gx, gy, hole, gmask=None, edge=None, device=None, r
     u = z64(F, 4, H * W, C)
     v, w, x = z64(F, H * W, C), z64(F, H * W, C), z64(F, H * W, C)
     iter_lim = 2 * H * W                               # scipy.sparse.linalg.lsqr's default for an [m, H*W] system
-    if max_iters is None:
-        max_iters = iter_lim                           # the device-side test k >= iter_lim stops every system by then
-    slots = min(max_iters, iter_lim) + CHUNK + 2       # a replay may run past the last stop by < CHUNK (frozen) iterations
+    if max_iters is not None:
+        if max_iters < 1:
+            raise ValueError(f"poisson: max_iters {max_iters} must be at least 1")
+        iter_lim = min(max_iters, iter_lim)            # the device-side test k >= iter_lim stops every system there
+    slots = iter_lim + CHUNK + 2                       # a replay may run past the last stop by < CHUNK (frozen) iterations
     bb, aa, ww = z64(slots * S), z64(slots * S), z64(slots * S)
     state = z64(2, S, 16)
     plist = torch.zeros(F, H * W, dtype=torch.int32, device=dev)    # uint32 entries: pixel | code << 24, 0 = none
@@ -79,8 +82,8 @@ def poisson_blend_batch(trg, gx, gy, hole, gmask=None, edge=None, device=None, r
     k = 0
     try:
         while True:
-            if k > min(max_iters, iter_lim) + CHUNK:   # cannot happen with max_iters = iter_lim (istop = 7 by then)
-                raise RuntimeError(f"poisson: LSQR did not stop within {max_iters} iterations")
+            if k > iter_lim + CHUNK:                   # cannot happen: every system stops by iteration iter_lim (istop 7)
+                raise RuntimeError(f"poisson: LSQR did not stop within {iter_lim} iterations")
             if use_graph:
                 lib.call("fgt_poisson_graph_launch", exec_, kernels=2 * CHUNK)
             else:

@@ -13,12 +13,17 @@ CHUNK = 64           # iterations between convergence checks (one host sync each
 MAX_ITERS = None     # None: max(10000, 50 * (H + W)) — CG on a hole of diameter d needs ~25 d iterations at tol 1e-12
 
 
-def regionfill_batch(images, masks, tol=1e-12, device=None, return_iters=False, max_iters=MAX_ITERS):
-    """images [B,H,W] float (numpy or tensor), masks [B,H,W] bool/uint8 -> float64 tensor [B,H,W] on the device:
-    harmonic fill inside each mask, the image unchanged outside."""
+def _dev(device):
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if dev.type != "cuda":
         raise RuntimeError("fgt_b200 regionfill runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+    return dev
+
+
+def regionfill_batch(images, masks, tol=1e-12, device=None, return_iters=False, max_iters=MAX_ITERS):
+    """images [B,H,W] float (numpy or tensor), masks [B,H,W] bool/uint8 -> float64 tensor [B,H,W] on the device:
+    harmonic fill inside each mask, the image unchanged outside."""
+    dev = _dev(device)
     img = torch.as_tensor(images).to(dev, torch.float64).contiguous()
     msk = (torch.as_tensor(masks).to(dev) != 0).to(torch.uint8).contiguous()
     if img.dim() != 3 or img.shape != msk.shape:

@@ -205,7 +205,11 @@ int fgt_rownorm_bcast(const float* a, int ca, int lda, const float* b, int cb, i
  *   fgt_regionfill_init  : x = 0, r = p0 = right-hand side (region_fill.py:69-112), rr[0..B) = <r,r>
  *   fgt_regionfill_iters : CG iterations k0 .. k0+iters-1; rr / pap are zero-initialised arrays of
  *                          (max_iters+1)*B doubles (iteration k uses rr[k*B+b], pap[k*B+b], writes rr[(k+1)*B+b]);
- *                          the host reads rr to decide convergence
+ *                          the host reads rr to decide convergence. Iteration k, inside the mask only:
+ *                          beta = rr[k]/rr[k-1] (0 for k = 0 or rr[k-1] = 0), p = r + beta p' with p' the direction
+ *                          of iteration k-1 (p' in p0 for even k, p in p1; odd k the other way round), ap = A p,
+ *                          pap[k] += <p,ap>; alpha = rr[k]/pap[k] (0 unless pap[k] > 0), x += alpha p,
+ *                          r -= alpha ap, rr[(k+1)*B+b] += <r,r>. Nothing outside the mask is written.
  *   fgt_regionfill_finish: out = x inside the mask, img outside (region_fill.py:15-16)
  * All arrays are caller-owned device memory. */
 int fgt_regionfill_init(const double* img, const unsigned char* mask, int B, int H, int W, double* x, double* r,
@@ -224,7 +228,16 @@ int fgt_regionfill_finish(const double* img, const unsigned char* mask, long lon
  *   trg [F,H,W,3], gx [F,H,W-1,3], gy [F,H-1,W,3] (forward differences); hole / gmask / edge uint8 [F,H,W]
  *   (gmask, edge may be NULL = all zero); code uint8 [F,H,W]; u [F,4,H*W,3]; v, w, x [F,H*W,3];
  *   bb, aa, ww: (max_iters + chunk + 2) * 3F per-iteration sums (slot k*3F + s); state [2, 3F, 16] (ping-pong by iteration
- *   parity; per system s = 3*frame + channel: [12] = stopped, [13] = scipy's istop, [14] = itn).
+ *   parity; per system s = 3*frame + channel: [0] alfa, [1] rhobar, [2] phibar, [3] anorm, [4] ddnorm, [5] xxnorm,
+ *   [6] z, [7] cs2, [8] sn2 as scipy names them, [9] 1/alfa (1 if alfa = 0), [10] 1/beta (1 if beta = 0), [11] bnorm,
+ *   [12] = stopped, [13] = scipy's istop, [14] = itn, [15] beta).
+ *   u and v hold LSQR's vectors unnormalised, u = beta u^ and v = alfa v^ in scipy's terms with u^, v^ of unit norm, and
+ *   are scaled on read: bb[k] = |u|^2 = beta_k^2, aa[k] = |v|^2 = alfa_k^2, ww[k] = |w|^2 at the start of iteration k.
+ *   Iteration k of a running system s, with P = state[(k-1) & 1] and N = state[k & 1]: if beta_k > 0,
+ *   v = A^T u / beta_k - beta_k P[9] v (the second term 0 for k = 0) and aa[k] += |v|^2; then N = scipy's scalar step
+ *   (itn = k, iter_lim from the caller; k = 0 only sets the state up), x += t1 w, w = v N[9] + t2 w (t1 = t2 = 0 for
+ *   k = 0), ww[k+1] += |w|^2; and, unless it stopped at k, u = A (v N[9]) - N[0] N[10] u, bb[k+1] += |u|^2. A stopped
+ *   system's vectors and sums are never written again; its state is carried forward.
  *   fgt_poisson_setup   : equation codes, u = b, bb[0] = |b|^2 (constructEquation :176-266); appends the pixels
  *                         that own equations to list [F,H*W] uint32 (pixel index | code << 24; zero-initialised, H*W <
  *                         2^24) and counts them in cnt [F] (zero-initialised) — the host reads max(cnt) once and
@@ -235,7 +248,8 @@ int fgt_regionfill_finish(const double* img, const unsigned char* mask, long lon
  *   fgt_poisson_graph_* : the same `iters` kernel pairs captured once into an executable CUDA graph (a host-side driver
  *                         object, the only thing this library ever creates; destroy it with _graph_destroy) and
  *                         replayed with _graph_launch — every replay continues at the device-side k
- *   fgt_poisson_unfilled: the two raster sweeps of the connectivity check (:139-172) -> clr [2,F,H,W]
+ *   fgt_poisson_unfilled: the two raster sweeps of the connectivity check (:139-172) -> clr [2,F,H,W]: clr[0] / clr[1]
+ *                         = 1 where the forward / backward sweep clears the pixel (every pixel outside the hole), else 0
  *   fgt_poisson_finish  : out = hole ? float64(float32(x)) : trg (:29,40-44); unf = hole & !clr[0] & !clr[1]
  *                         (unf / clr may be NULL)
  *   fgt_poisson_advance_host: HOST-ONLY — runs the scalar recurrence of one iteration (the same

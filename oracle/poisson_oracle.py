@@ -92,8 +92,8 @@ def _shift(a, n):
 
 
 def matvec(code, v):
-    """(A v)[n,p] = v_p - [q in hole] v_q for the equations that exist. v [H,W]."""
-    u = np.zeros((4,) + v.shape)
+    """(A v)[n,p] = v_p - [q in hole] v_q for the equations that exist. v [H,W] (any float dtype, kept)."""
+    u = np.zeros((4,) + v.shape, dtype=v.dtype)
     for n in range(4):
         valid = ((code >> n) & 1).astype(bool)
         inh = ((code >> (4 + n)) & 1).astype(bool)
@@ -103,7 +103,7 @@ def matvec(code, v):
 
 def rmatvec(code, u):
     """(A^T u)[p] = sum_n u[n,p] - sum_n u[(n+2)%4, q_n] over neighbours q_n whose equation towards p is in-hole."""
-    out = np.zeros(u.shape[1:])
+    out = np.zeros(u.shape[1:], dtype=u.dtype)
     for n in range(4):
         out += np.where(((code >> n) & 1).astype(bool), u[n], 0.0)
         m = (n + 2) % 4
@@ -218,6 +218,12 @@ def lsqr(code, b, atol=1e-6, btol=1e-6, conlim=1e8, iter_lim=None):
 
 def unfilled_mask(hole, gmask):
     """Poisson_blend_img.py:139-172 / getUnfilledMask :270-309. hole, gmask [H,W] -> bool [H,W]."""
+    tl, br = unfilled_sweeps(hole, gmask)
+    return tl & br
+
+
+def unfilled_sweeps(hole, gmask):
+    """The two sweeps of unfilled_mask: (forward, backward) bool [H,W], True = hole pixel the sweep leaves unfilled."""
     hole = np.asarray(hole).astype(bool)
     gm = np.asarray(gmask) != 0
     H, W = hole.shape
@@ -238,7 +244,7 @@ def unfilled_mask(hole, gmask):
             if row[j] and not row[j + 1] and ok[i, j]:
                 row[j] = False
         br[i] = row
-    return tl & br
+    return tl, br
 
 
 def poisson_blend(trg, gx, gy, hole, gmask=None, edge=None, return_info=False):

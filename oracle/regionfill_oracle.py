@@ -14,34 +14,46 @@ from scipy import sparse
 from scipy.sparse.linalg import spsolve
 
 
-def regionfill(I, mask):
-    """I [H,W] float, mask [H,W] bool -> float64 [H,W]."""
-    I = np.asarray(I, dtype=np.float64)
+def system(mask):
+    """The operator of regionfill for mask [H,W] bool: (A [n,n] csr, R [n,H*W] csr) over the n mask pixels in raster
+    order, so that the hole values solve A u = R I.ravel(). A's diagonal holds the number of in-image 4-neighbours,
+    -1 couples in-mask neighbours; R sums the image values of the in-image neighbours outside the mask."""
     mask = np.asarray(mask).astype(bool)
-    if not mask.any():
-        return I.copy()
-    H, W = I.shape
+    H, W = mask.shape
     idx = -np.ones((H, W), dtype=np.int64)
     idx[mask] = np.arange(int(mask.sum()))
     ys, xs = np.nonzero(mask)
     n = ys.size
     diag = np.zeros(n)
-    rhs = np.zeros(n)
-    rows, cols, vals = [], [], []
+    rows, cols, vals, brow, bcol = [], [], [], [], []
     for dy, dx in ((-1, 0), (0, 1), (1, 0), (0, -1)):
         yy, xx = ys + dy, xs + dx
         ok = (yy >= 0) & (yy < H) & (xx >= 0) & (xx < W)
         diag += ok
         yc, xc = np.clip(yy, 0, H - 1), np.clip(xx, 0, W - 1)
         inside = ok & mask[yc, xc]
-        rhs += np.where(ok & ~inside, I[yc, xc], 0.0)
         rows.append(np.arange(n)[inside])
         cols.append(idx[yc, xc][inside])
         vals.append(-np.ones(int(inside.sum())))
+        out = ok & ~inside
+        brow.append(np.arange(n)[out])
+        bcol.append((yc * W + xc)[out])
     rows.append(np.arange(n)); cols.append(np.arange(n)); vals.append(diag)
     A = sparse.coo_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(n, n)).tocsr()
+    br = np.concatenate(brow)
+    R = sparse.coo_matrix((np.ones(br.size), (br, np.concatenate(bcol))), shape=(n, H * W)).tocsr()
+    return A, R
+
+
+def regionfill(I, mask):
+    """I [H,W] float, mask [H,W] bool -> float64 [H,W]."""
+    I = np.asarray(I, dtype=np.float64)
+    mask = np.asarray(mask).astype(bool)
+    if not mask.any():
+        return I.copy()
+    A, R = system(mask)
     out = I.copy()
-    out[mask] = spsolve(A, rhs)
+    out[mask] = spsolve(A, R @ I.ravel())
     return out
 
 
