@@ -143,7 +143,12 @@ typedef struct {
   int batches, heads, head_dim; /* head_dim must be 128 */
   int Lq;                       /* query rows per batch */
   int Lk;                       /* dense: valid keys per batch */
-  int Lk_rows;                  /* addressable key rows per batch (>= Lk; windowed: local + global rows) */
+  int Lk_rows;                  /* addressable key rows per batch (>= Lk; windowed: local + global rows). Key tiles
+                                   read whole 64-row tiles: dense rows [Lk, min(Lk_rows, 64 ceil(Lk / 64))), windowed
+                                   rows [glob_start + glob_count, + 64 ceil(glob_count / 64)) within Lk_rows are read
+                                   and masked. K there may hold anything (NaN and Inf included: the scores are masked);
+                                   V there must be finite, since P = 0 multiplies it and a NaN or Inf makes every output
+                                   row of that batch NaN. Rows past Lk_rows are never read. */
   float scale;                  /* 1/sqrt(head_dim) */
   int mode;
   int glob_start, glob_count;   /* windowed mode */
